@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the HippoRAG retrieval hot path on B200 (contract: see the task statement).
+"""Benchmark of the HippoRAG retrieval hot path on H100.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C1|C2|C3|C5] [--impl reference]
+                    [--dump-outputs DIR]
 
 A *step* = one batch of ``--queries`` queries through the whole path
 (stage A: query x fact similarity + top-5 -> identity recognition-memory filter -> stage B:
@@ -13,8 +14,11 @@ sides, max over ranks.  Inputs (hundreds of MB of state + GBs of embeddings) exc
 explicit L2 flush is needed between iterations (C1 is the exception and says so).
 
 Workloads (BASELINE.json configs): C1 = MuSiQue-1k (the reference's own index() output, committed as
-tests/golden/musique1k.npz; 64 queries), C2 / C3 = synthetic uniform KGs, C5 = 10M-node power-law KG with
-1024-d embeddings (facts uploaded streamed, bf16 planes only).
+tests/golden/musique1k.npz; 64 queries), C2 / C3 = synthetic uniform KGs, C5 = 4M-node power-law KG with
+1024-d embeddings (facts uploaded streamed, bf16 planes only: 45 GB of the H100's 80 GB).
+
+``--dump-outputs DIR`` writes what the timed path returned in its last step (top-k passage ids and scores, float64 /
+float32 .npy) so two builds can be compared output for output; inputs are seeded, identical from run to run.
 
 N > 1 (launched under torch.distributed.run): ``value`` = *replicas* -- every rank holds the whole graph and
 its own batch of queries (queries are independent units, SURVEY.md 8(e)); no data-path collective;
@@ -45,11 +49,12 @@ WORKLOADS = {
                desc="synthetic 100k-node / 1M-edge KG, 768-d embeddings, 1k queries"),
     "C3": dict(n_nodes=1_000_000, n_edges=10_000_000, dim=768, queries=10_000, topology="uniform",
                desc="synthetic 1M-node / 10M-edge KG, 768-d embeddings, 10k batched queries"),
-    "C5": dict(n_nodes=10_000_000, n_edges=100_000_000, dim=1024, queries=128, topology="powerlaw", streamed=True,
-               desc="synthetic 10M-node / 100M-edge power-law KG, 1024-d embeddings"),
+    "C5": dict(n_nodes=4_000_000, n_edges=40_000_000, dim=1024, queries=128, topology="powerlaw", streamed=True,
+               desc="synthetic 4M-node / 40M-edge power-law KG, 1024-d embeddings"),
 }
 TOPK, LINK_TOP_K, DAMPING, PNW = 200, 5, 0.5, 0.05
-DTYPE = "bf16x4-split tcgen05 GEMM (fp32 accumulate) + fp16-state PPR with fp32 residual refinement; fp32 outputs"
+DTYPE = "bf16x4-split wgmma GEMM (fp32 accumulate) + fp16-state PPR with fp32 residual refinement; fp32 outputs"
+DUMP_LIMIT_BYTES = 64 << 20
 
 
 def log(*a):
@@ -61,7 +66,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, STREAM-style copy)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def emb_chunk_torch(rows_lo, rows_hi, dim, seed, device):
@@ -208,6 +213,24 @@ class ClockSampler:
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
+def dump_outputs(out_dir, arrays):
+    """Writes every array as out_dir/<name>.npy: integers as float64 (exact below 2^53), floats as float32.  Above
+    DUMP_LIMIT_BYTES in all, the same seeded sample of rows is kept from every array (and saved as sample_rows)."""
+    os.makedirs(out_dir, exist_ok=True)
+    conv = {k: v.astype(np.float64) if np.issubdtype(v.dtype, np.integer) else v.astype(np.float32)
+            for k, v in arrays.items()}
+    rows = len(next(iter(conv.values())))
+    total = sum(v.nbytes for v in conv.values())
+    if total > DUMP_LIMIT_BYTES:
+        keep = max(1, int(rows * DUMP_LIMIT_BYTES / total) - 1)
+        sel = np.sort(np.random.default_rng(0).choice(rows, keep, replace=False))
+        conv = {k: v[sel] for k, v in conv.items()}
+        conv["sample_rows"] = sel.astype(np.float64)
+    for k, v in conv.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), v)
+    log(f"[bench] outputs of the last timed step -> {out_dir}: " + ", ".join(f"{k} {v.shape}" for k, v in conv.items()))
+
+
 def ppr_bytes_per_sweep(n_rows, nnz, B):
     """SURVEY.md 8(d): nnz*(4 col + 4 val) + (N+1)*4 row_ptr + B*N*4*3 (read X, write Y, read V)."""
     return nnz * 8 + (n_rows + 1) * 4 + 3 * n_rows * B * 4
@@ -332,6 +355,8 @@ def main():
     ap.add_argument("--cpu-best-effort-sample", type=int, default=128, help="queries in the best-effort CPU leg (0 = skip)")
     ap.add_argument("--ref-queries", type=int, default=4, help="queries per step of --impl reference")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
 
@@ -350,7 +375,7 @@ def main():
     import torch
     import torch.distributed as dist
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device -- the B200 arm has no CPU fallback (use --impl reference)")
+        raise SystemExit("bench.py: no CUDA device -- the GPU arm has no CPU fallback (use --impl reference)")
     torch.cuda.set_device(local_rank)
     device = torch.device("cuda", local_rank)
     if world > 1:
@@ -436,6 +461,7 @@ def main():
         sampler = ClockSampler(local_rank) if rank == 0 else None
         ms_total = timed(resident_step, args.steps)
         clocks = sampler.stop() if sampler else None
+        last = {"topk_ids": out_ids.cpu().numpy(), "topk_scores": out_scores.cpu().numpy()}
         st = eng.stats()
         e2e = None
         if not args.no_e2e:
@@ -448,8 +474,8 @@ def main():
             e2e = {"value": Q * args.steps * n_eff / (ms_e2e / 1000.0), "unit": "queries/s",
                    "h2d_bytes_per_step": int(st2["h2d_bytes"] // args.steps),
                    "d2h_bytes_per_step": int(st2["d2h_bytes"] // args.steps), "ms_per_step": ms_e2e / args.steps}
-        res = dict(ms_total=ms_total, st=st, clocks=clocks, e2e=e2e, out_ids=out_ids[:max(args.cpu_sample, 8)].cpu().numpy(),
-                   h_qf=h_qf_np, h_qp=h_qp_np)
+        res = dict(ms_total=ms_total, st=st, clocks=clocks, e2e=e2e, out_ids=last["topk_ids"][:max(args.cpu_sample, 8)],
+                   last=last, h_qf=h_qf_np, h_qp=h_qp_np)
         eng.close()
         del eng
         torch.cuda.empty_cache()
@@ -474,6 +500,8 @@ def main():
             dist.destroy_process_group()
         return
 
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, main_res["last"])
     peak, peak_src = measured_peaks()
 
     def roofline_of(res, mode):
@@ -488,19 +516,10 @@ def main():
         achieved = bytes_sweep / (ms_sweep * 1e-3) / 1e9
         mixed = abs(Bavg - 32.0) < 1e-6
         bytes_layout = (nnz_local * 8 + (n_rows_local + 1) * 4 + 3 * n_rows_local * Bavg * 2) if mixed else bytes_sweep
-        traffic, traffic_src = None, None
-        tpath = os.path.join(ROOT, "profiles", "k1_traffic.json")
-        if os.path.exists(tpath) and not sharded:
-            try:
-                tj = json.load(open(tpath))
-                traffic = tj.get(f"{args.workload}_B{int(Bavg)}")
-                traffic_src = tj.get("source")
-            except Exception:
-                traffic = None
         return {"kernel": ("k_sweep_h (K1m: CSR SpMM PPR sweep, fp16 state / fp32 math, B=32)" if mixed else
                            "k_sweep_rows (K1: CSR SpMM PPR sweep, fp32 state)"),
                 "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                "peak_source": peak_src,
                 "bytes_per_launch": bytes_sweep, "bytes_per_launch_in_this_layout": bytes_layout,
                 "achieved_in_this_layout": bytes_layout / (ms_sweep * 1e-3) / 1e9,
                 "ms_per_launch": ms_sweep, "launches": sweeps, "batch_width": Bavg,

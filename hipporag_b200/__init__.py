@@ -1,5 +1,5 @@
 """hipporag_b200 -- HippoRAG's online retrieval hot path (embedding similarity -> seeds ->
-Personalized PageRank -> top-k passages) as hand-written CUDA for B200 (sm_100a), behind the
+Personalized PageRank -> top-k passages) as hand-written CUDA for H100 (sm_90a), behind the
 reference's own ``HippoRAG.retrieve()`` API.  See DESIGN.md / INTEGRATION.md."""
 from ._lib import (HragError, PPR_CHEBYSHEV, PPR_FP32, PPR_MIXED, PPR_POWER, SIM_BF16, SIM_BF16X3,  # noqa: F401
                    SIM_FP32)

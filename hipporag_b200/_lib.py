@@ -1,7 +1,7 @@
 """ctypes binding of ``libhrag_b200.so`` (C ABI declared in ``include/hrag_b200.h``).
 
 There is no CPU fallback and no alternative backend: if the shared library is missing (not
-built) this module raises, and ``hrag_create`` fails when no B200 is visible.
+built) this module raises, and ``hrag_create`` fails when no H100 is visible.
 """
 from __future__ import annotations
 

@@ -1,11 +1,11 @@
-"""Drop-in: put a ``HippoRAG`` object's online retrieval path on the B200 engine.
+"""Drop-in: put a ``HippoRAG`` object's online retrieval path on the H100 engine.
 
     import hipporag_b200
     rag = HippoRAG(...); rag.index(docs)
     hipporag_b200.accelerate(rag, device=0)
     rag.retrieve(queries) / rag.rag_qa(queries)        # same signatures, same return types
 
-What is rebound (all paths under ``/root/reference/src/hipporag/``):
+What is rebound (all paths under the reference's ``src/hipporag/``):
 
 * ``prepare_retrieval_objects`` (``HippoRAG.py:1287-1389``) -- the original runs, then the graph,
   the integer tables equivalent to its dicts, and the embeddings are uploaded once;
@@ -26,7 +26,7 @@ What is rebound (all paths under ``/root/reference/src/hipporag/``):
 ``linking_top_k`` (``config_utils.py:184``) may be anything in [1, 32] (<= 8 is selected inside the GEMM
 epilogue, larger values by an exact radix select); beyond 32 ``retrieve`` raises instead of clamping.
 
-The engine never falls back to the CPU: if the CUDA library or a B200 is missing this raises.
+The engine never falls back to the CPU: if the CUDA library or an H100 is missing this raises.
 """
 from __future__ import annotations
 
@@ -162,7 +162,7 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
             raise ValueError(f"linking_top_k must be a positive integer, got {link_top_k!r}")
         if link_top_k > MAX_LINKING_TOP_K:
             raise ValueError(f"linking_top_k = {link_top_k} exceeds the {MAX_LINKING_TOP_K} candidate facts per query "
-                             "the B200 engine keeps (it does not clamp silently)")
+                             "the engine keeps (it does not clamp silently)")
         k = int(link_top_k)
         nq = len(queries)
         Qf = _query_matrix(self, queries, "triple")

@@ -1,11 +1,11 @@
 // C ABI of libhrag_b200.so (declared in include/hrag_b200.h): handle, uploads, and the
 // stage orchestration that stands in for the body of HippoRAG.retrieve()'s per-query loop
-// (reference HippoRAG.py:459-480) -- batched, on one B200, all intermediate state in HBM.
+// (reference HippoRAG.py:459-480) -- batched, on one H100, all intermediate state in HBM.
 //
 // HBM layout per handle (N nodes, P passages, F facts, d dims; DESIGN.md section 3):
 //   graph     row_ptr int32[n_rows+1], cv int2[nnz] {col, fp32 bits of P[i,j]}, row_order int32[n_rows]   (resident)
 //   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N], slot_map[2][N] (node -> rhs slot)       (resident)
-//   emb       bf16 hi/lo planes [rows, d] x 2 (tcgen05 similarity); fp32 [rows, d] only when uploaded whole  (resident)
+//   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
 //   state     mixed solver: H0..H3, H0b [N, 32] fp16 in one IPC-exportable slab; fp32 solver: V, XA, XC [N, B] fp32
 //   rhs       compact: Vc [P + 2048, 32] fp32 (exact v) + R16 [P + 2048, 32] fp16 (scaled), two sets (double-buffered)
 //   scores    S_pass [chunk, P] fp32; fact scores are never materialised in the fused modes (72 B per query x tile)
@@ -117,9 +117,9 @@ struct hrag_handle {
     SeedTables t;
     float* emb[2] = {nullptr, nullptr};
     bool emb_owned[2] = {false, false};
-    void* emb_hi[2] = {nullptr, nullptr};   // bf16 split of emb for the tcgen05 path
+    void* emb_hi[2] = {nullptr, nullptr};   // bf16 split of emb for the tensor-core path
     void* emb_lo[2] = {nullptr, nullptr};
-    int num_sms = 148;
+    int num_sms = 132;
     int64_t emb_rows[2] = {0, 0};   // rows held by THIS handle (node-range sharding: the rank's slice of the facts)
     int64_t fact_row_lo = 0;        // first global fact row of the local slice
     int64_t n_facts_global = 0;
@@ -146,8 +146,6 @@ struct hrag_handle {
     Buf H0b, mixed_aux1, prep_scratch;
     Buf slot_map[2], slot_vid[2], Vc[2], R16[2], rho;
     bool slot_maps_valid = false;
-    alignas(128) unsigned char xmap[5][128];   // CUtensorMap of H[0..3], H0b for the TMA-gather sweep (K1t)
-    bool xmaps_valid = false;
     int use_tma = -1;                          // HRAG_MIXED_TMA=1 routes plain fp16 sweeps through k_sweep_h_tma
     // CUDA graphs of the mixed solve, one per (buffer set, sweep plan); `graph_generation` changes whenever anything a
     // captured launch depends on does (graph / tables reload, state reallocation, tuning switches)
@@ -315,15 +313,9 @@ int ensure_state_mixed(hrag_t* h) {
             HRAG_CUDA(cudaMalloc(&h->d_done_ctr, sizeof(unsigned int)));
             HRAG_CUDA(cudaMemset(h->d_done_ctr, 0, sizeof(unsigned int)));
         }
-        h->xmaps_valid = false;
         h->graph_generation += 1;
     }
     if (h->use_tma < 0) { const char* e = getenv("HRAG_MIXED_TMA"); h->use_tma = e ? atoi(e) : 0; }
-    if (h->use_tma && !h->xmaps_valid) {
-        hrag::Buf* views[5] = {&h->H[0], &h->H[1], &h->H[2], &h->H[3], &h->H0b};
-        for (int i = 0; i < 5; ++i) HRAG_TRY(tma_state_map(views[i]->p, (int64_t)rows, h->xmap[i]));
-        h->xmaps_valid = true;
-    }
     HRAG_TRY(h->partials.ensure((size_t)std::max(mixed_partial_rows(h->g), 1024) * 32 * sizeof(float)));
     HRAG_TRY(h->sums.ensure(192 * sizeof(double)));      // sums of x0, of d, of |r|, and of v (two sets)
     HRAG_TRY(h->mixed_aux.ensure(32 * sizeof(float)));   // column scales, set 0
@@ -427,11 +419,9 @@ int p2p_signal(hrag_t* h) {
 int mixed_sweep_x(hrag_t* h, int mode, const void* x, const int* slot_map, const void* rhs, const float* v32,
                   const float* scale, const void* prev, void* y, float alpha, float w, float t, float* part,
                   int* n_part) {
-    if (h->use_tma == 1 && mode == 0 && part == nullptr && !h->p2p && h->g.n_long == 0 && h->xmaps_valid) {
-        // K1t: gathered rows through TMA gather4 (x is one of the five slab buffers)
-        const int xi = (int)((static_cast<const char*>(x) - static_cast<const char*>(h->slab)) / (ptrdiff_t)h->slab_hb);
-        HRAG_CHECK(xi >= 0 && xi < 5, "internal: x is not a slab buffer");
-        HRAG_TRY(mixed_sweep_tma(h->g, h->xmap[xi], slot_map, rhs, prev, y, alpha, w, peers_for(h, y), h->stream));
+    if (h->use_tma == 1 && mode == 0 && part == nullptr && !h->p2p && h->g.n_long == 0) {
+        // K1t: gathered rows through bulk asynchronous copies into a shared-memory ring
+        HRAG_TRY(mixed_sweep_tma(h->g, x, slot_map, rhs, prev, y, alpha, w, peers_for(h, y), h->stream));
         return exchange_rows_bytes(h, y, 32 * 2);
     }
     HRAG_TRY(mixed_sweep(h->g, mode, x, slot_map, rhs, v32, scale, prev, y, alpha, w, t, part, n_part, peers_for(h, y),
@@ -479,7 +469,7 @@ constexpr float kMixedT = 64.f;    // residual scale: r ~ 5e-4 x, keeps it in fp
 // P is similar to a symmetric stochastic matrix, so the spectrum of aP is real in [-a, a]: Chebyshev
 // semi-iteration contracts by sigma = a / (1 + sqrt(1 - a^2)) per sweep (0.268 at a = 0.5), the plain power
 // sweep by a.  fp16 storage of the iterate leaves a relative L1 error of about kHalfNoise / (1 - a) in a
-// converged fp16 solve (measured 5e-4 at a = 0.5, profiles/r1_accuracy_mixed.txt); one refinement round
+// converged fp16 solve (5e-4 at a = 0.5 against the float64 oracle); one refinement round
 // multiplies the error by kappa = that + 2 sigma^m2.
 constexpr double kHalfNoise = 2.5e-4;
 constexpr double kDefaultTol = 1e-6;     // relative L1 accuracy of the PPR vector when the caller passes tol <= 0
@@ -864,7 +854,7 @@ int d2h(hrag_t* h, void* dst, const void* src, size_t bytes) {
 extern "C" {
 
 const char* hrag_last_error(void) { return g_error.c_str(); }
-const char* hrag_version(void) { return "hrag_b200 0.1 (sm_100a)"; }
+const char* hrag_version(void) { return "hrag_b200 0.1 (sm_90a)"; }
 
 int hrag_create(const int* device_ids, int n_devices, int shard_mode, hrag_t** out) {
     HRAG_CHECK(out != nullptr, "hrag_create: out is null");
@@ -880,7 +870,7 @@ int hrag_create(const int* device_ids, int n_devices, int shard_mode, hrag_t** o
     HRAG_CUDA(cudaSetDevice(device_ids[0]));
     cudaDeviceProp prop;
     HRAG_CUDA(cudaGetDeviceProperties(&prop, device_ids[0]));
-    HRAG_CHECK(prop.major == 10, "hrag_create: this library is built for sm_100a (B200) only");
+    HRAG_CHECK(prop.major == 9 && prop.minor == 0, "hrag_create: this library is built for sm_90a (H100) only");
     hrag_t* h = new hrag_handle();
     h->device = device_ids[0];
     h->shard_mode = shard_mode;
@@ -1227,7 +1217,7 @@ int hrag_load_embeddings(hrag_t* h, int which, int64_t rows, int32_t dim, const 
         h->emb_owned[which] = true;
         HRAG_CUDA(cudaMemcpy(h->emb[which], emb, (size_t)rows * dim * sizeof(float), cudaMemcpyHostToDevice));
     }
-    if (dim % 8 == 0) {   // bf16 hi/lo split for the tcgen05 similarity kernel
+    if (dim % 8 == 0) {   // bf16 hi/lo split for the tensor-core similarity kernel
         const size_t n = (size_t)rows * dim;
         HRAG_CUDA(cudaMalloc(&h->emb_hi[which], n * 2));
         HRAG_CUDA(cudaMalloc(&h->emb_lo[which], n * 2));
@@ -1532,7 +1522,7 @@ int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float mi
     HRAG_CHECK(kmax >= 1 && kmax <= kCandidateCap && B >= 0, "hrag_knn_threshold: kmax must be in [1, 512]");
     HRAG_CHECK(h->dim > 0 && h->emb_rows[which] > 0 && h->emb_hi[which] != nullptr,
                "hrag_knn_threshold: embeddings not loaded (needs the tensor-core layout: dim % 8 == 0)");
-    HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, "hrag_knn_threshold: the threshold epilogue lives in the tcgen05 kernel");
+    HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, "hrag_knn_threshold: the threshold epilogue lives in the tensor-core kernel");
     HRAG_CUDA(cudaSetDevice(h->device));
     const int64_t M = h->emb_rows[which];
     const int64_t chunk = 1024;
@@ -1695,14 +1685,7 @@ int hrag_set_tuning(hrag_t* h, int mixed_hint, int use_tma, int sorted_rows, int
         HRAG_CHECK(mixed_hint <= 4, "hrag_set_tuning: mixed_hint in [0, 4]");
         set_mixed_hint(mixed_hint);
     }
-    if (use_tma >= 0) {
-        h->use_tma = use_tma ? 1 : 0;
-        if (h->use_tma && h->slab) {
-            hrag::Buf* views[5] = {&h->H[0], &h->H[1], &h->H[2], &h->H[3], &h->H0b};
-            for (int i = 0; i < 5; ++i) HRAG_TRY(tma_state_map(views[i]->p, (int64_t)state_rows(h), h->xmap[i]));
-            h->xmaps_valid = true;
-        }
-    }
+    if (use_tma >= 0) h->use_tma = use_tma ? 1 : 0;
     return 0;
 }
 

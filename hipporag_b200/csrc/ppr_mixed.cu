@@ -29,8 +29,8 @@
 // Row walk: 4 gathers in flight per lane, the ragged end of a row is one PREDICATED batch (not a
 // serial tail), and the 64 rows of a CTA are handed to the groups by length (row_order) so the 8
 // rows that share a warp finish together.  Cache-policy variants (createpolicy descriptors on
-// gathers / streams, L1::no_allocate) are kept as template HINTs; plain read-only loads win once
-// the tail is predicated -- profiles/r2_k1m_variants_{a,b,c}.txt.
+// gathers / streams, L1::no_allocate) are kept as template HINTs (hrag_set_tuning); plain read-only
+// loads are the default.
 //
 // K5 (node-range sharding, k_sweep_h_push): each CTA stages its 64 output rows in shared memory
 // and pushes the 4-KB block into every peer GPU's copy of y with one TMA bulk copy per peer over
@@ -82,7 +82,7 @@ __device__ __forceinline__ void fma8(float (&acc)[8], float a, const uint4& u) {
 // HINT 0: plain read-only loads.  1: gathers L2 evict_last, streams L2 evict_first (createpolicy descriptors).
 // 2: as 1 with only half of the gathered lines marked evict_last.  3: as 1, gathers also bypass L1 allocation.
 // 4: gathers bypass L1 allocation, nothing else (no descriptor: every gathered row is its own line, so L1 holds
-// nothing reusable and is left to the (col, val) stream).  Measured in profiles/r2_k1m_variants*.txt.
+// nothing reusable and is left to the (col, val) stream).
 template <int HINT>
 struct Policies {
     uint64_t keep, stream;
@@ -307,9 +307,8 @@ struct SweepArgs {
     float* partials;
 };
 
-// Single-GPU sweep: one block of 64 rows per CTA.  (Kept free of the exchange code of k_sweep_h_push below: sharing one
-// body -- a block loop with the staging / bulk-copy code behind a uniform branch -- cost the plain sweep 13 %:
-// 0.178 vs 0.157 ms on C3, profiles/r2_k1m_variants_d.txt.)
+// Single-GPU sweep: one block of 64 rows per CTA.  (Kept free of the exchange code of k_sweep_h_push below: a block
+// loop with the staging / bulk-copy code behind a uniform branch slows the plain sweep down.)
 template <bool CHEB, int MODE, bool FINAL, int U, int MINB, int HINT>
 __global__ void __launch_bounds__(kThreads, MINB)
 k_sweep_h(const SweepArgs a) {
@@ -754,9 +753,8 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
     // HRAG_K5_MODE: 0 (default) = persistent grid, the epoch is published by the last CTA of the sweep itself (one system
     // fence per CTA, no extra launch; the staging ring is double-buffered so a block's bulk copies overlap the next
     // block's gathers); 1 = one CTA per 64-row block, no fence inside, the epoch is published by a one-warp kernel behind
-    // the sweep (the kernel boundary orders the peer writes).  The wait is inside the sweep either way.  Measured
-    // (profiles/r2_k5_*): equal on 2 GPUs (0.132 vs 0.135 ms), mode 0 ahead on 8 (0.124-0.130 vs 0.144 ms): without the
-    // second staging buffer a CTA sits on its slot until the TMA engine has drained its 7 copies into a congested link.
+    // the sweep (the kernel boundary orders the peer writes).  The wait is inside the sweep either way.  Without the
+    // second staging buffer a CTA would sit on its slot until the TMA engine has drained its copies into a congested link.
     static int k5_mode = -1;
     if (k5_mode < 0) { const char* e = getenv("HRAG_K5_MODE"); k5_mode = e ? atoi(e) : 0; }
     const bool sharded = sync.flags != nullptr;

@@ -1,4 +1,4 @@
-// K1 -- batched CSR SpMM sweep of the Personalized-PageRank iteration (sm_100a).
+// K1 -- batched CSR SpMM sweep of the Personalized-PageRank iteration (sm_90a).
 //
 // Replaces the numeric core of HippoRAG.run_ppr (reference HippoRAG.py:1736-1743, which
 // hands one reset vector at a time to igraph/PRPACK) with a batched fixed-point sweep
@@ -194,8 +194,8 @@ k_sweep_long_finalize(int n_long, int row_base, const int* __restrict__ long_row
 // A row block = consecutive rows whose non-zeros (<= kStageCap entries) are ONE contiguous byte
 // range of cv[], fetched by one cp.async.bulk (TMA 1-D bulk copy) that completes on an mbarrier.
 // Two stages: the copy of block i+1 is in flight while the CTA gathers for block i, so a row's
-// gathers no longer wait for its (col,val) loads -- ncu showed the plain kernel latency-bound
-// on exactly that dependency (profiles/r1_k1_fp32_sweep_ncu.md).
+// gathers no longer wait for its (col,val) loads, the dependency that leaves the plain kernel
+// latency-bound.
 constexpr int kStageCap = 2048;                  // cv entries per stage (16 KB)
 constexpr int kStageEntries = kStageCap + 2;     // +2: 16-byte alignment slack at both ends
 
@@ -338,8 +338,7 @@ k_colsum_reduce(const float* __restrict__ partials, int n_partials, int B, doubl
 }
 
 // 0 (default) = one row group per slot, (col,val) read through L1; 1 = persistent CTAs with the
-// (col,val) stream staged in shared memory by cp.async.bulk.  Measured on B200 (C3, B=16):
-// 0.140 ms vs 0.144-0.159 ms per sweep -- both sit on the same L1TEX wavefront bound, see DESIGN.md.
+// (col,val) stream staged in shared memory by cp.async.bulk.
 int sweep_variant() {
     static int v = -1;
     if (v < 0) {

@@ -1,20 +1,19 @@
-// K1t -- the fp16-state PPR sweep with the gathered state rows fetched by TMA (sm_100a).
+// K1t -- the fp16-state PPR sweep with the gathered state rows fetched by the TMA unit (sm_90a).
 // (A variant of K1m; like it, one sweep of the iteration that stands in for igraph's personalized_pagerank call in
 // HippoRAG.run_ppr, reference HippoRAG.py:1736-1743.)
 //
 // Same arithmetic as k_sweep_h (ppr_mixed.cu), different data path for the operand that bounds
 // the sweep: the rows x[j, :] named by the non-zeros of a row block.  Producer warps read the
-// block's (col, val) stream once (coalesced) and issue one `cp.async.bulk.tensor.2d ...
-// tile::gather4` per four non-zeros: the TMA unit fetches the four 64-byte state rows into a
-// shared-memory stage and signals an mbarrier (complete_tx); the values go to the same stage with
-// plain shared stores.  Consumer groups (4 lanes per row, as in k_sweep_h) then take their
+// block's (col, val) stream once (coalesced) and issue one bulk asynchronous copy
+// (`cp.async.bulk.shared::cluster.global`) per non-zero: the TMA unit fetches the 64-byte state row
+// into a shared-memory stage and signals an mbarrier (complete_tx); the values go to the same stage
+// with plain shared stores.  Consumer groups (4 lanes per row, as in k_sweep_h) then take their
 // row's operands from shared memory.  Loads in flight are bounded by the ring (3 stages x 1024
 // rows x 64 B = 192 KB per SM), not by registers x resident warps.
 //
 // Row blocks: <= 64 rows and <= 1024 non-zeros, contiguous in the CSR (built at graph load);
 // rows longer than long_thresh keep the segment path of ppr_mixed.cu and are skipped here.
-// Measured against k_sweep_h in profiles/r2_k1m_variants.txt.
-#include <cuda.h>
+// Selected with HRAG_MIXED_TMA=1; k_sweep_h stays the default.
 #include <cuda_fp16.h>
 
 #include <algorithm>
@@ -28,7 +27,6 @@ namespace hrag {
 
 namespace {
 
-constexpr int kB = 32;
 constexpr int kLPR = 4;
 constexpr int kBlkRows = 64;                  // rows per block = consumer groups per CTA
 constexpr int kBlkNnz = 1024;                 // non-zeros per block (one stage)
@@ -62,13 +60,11 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         "DONE:\n\t"
         "}" ::"r"(bar), "r"(parity) : "memory");
 }
-// four rows r0..r3 of the 2-D tensor (column offset c) -> 4 consecutive box rows at dst
-__device__ __forceinline__ void tma_gather4(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c, int r0, int r1,
-                                            int r2, int r3, uint64_t policy) {
+// one 64-byte state row global -> shared, completion counted on bar (complete_tx)
+__device__ __forceinline__ void bulk_row64(uint32_t dst, const void* src, uint32_t bar, uint64_t policy) {
     asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cta.global.tile::gather4.mbarrier::complete_tx::bytes.cta_group::1.L2::cache_hint "
-        "[%0], [%1, {%2, %3, %4, %5, %6}], [%7], %8;"
-        ::"r"(dst), "l"(map), "r"(c), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(bar), "l"(policy) : "memory");
+        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], 64, [%2], %3;"
+        ::"r"(dst), "l"(src), "r"(bar), "l"(policy) : "memory");
 }
 
 __device__ __forceinline__ void h8_to_f(const uint4& u, float (&f)[8]) {
@@ -91,6 +87,7 @@ __device__ __forceinline__ uint4 f_to_h8(const float (&f)[8]) {
 
 struct TmaSweepArgs {
     int n_blk;
+    const uint4* xh;           // [rows, 32] fp16 state: 4 x 16 bytes per row
     const int* blk_row;        // [n_blk + 1] first local row of each block; bit 31 = a long row (skipped here)
     int row_base;
     const int* row_ptr;
@@ -104,7 +101,7 @@ struct TmaSweepArgs {
 
 template <bool CHEB>
 __global__ void __launch_bounds__(kTmaThreads, 1)
-k_sweep_h_tma(const __grid_constant__ CUtensorMap tmap_x, const TmaSweepArgs a, const PeerOut peers) {
+k_sweep_h_tma(const TmaSweepArgs a, const PeerOut peers) {
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)kStages * kStageBytes);
@@ -142,8 +139,10 @@ k_sweep_h_tma(const __grid_constant__ CUtensorMap tmap_x, const TmaSweepArgs a, 
                 const int i = s0 + 4 * q;
                 int2 c[4];
 #pragma unroll
-                for (int j = 0; j < 4; ++j) c[j] = __ldg(a.cv + min(i + j, e0 - 1));   // tail: repeat the last entry
-                tma_gather4(smem_u32(xs + (size_t)q * 256), &tmap_x, full, 0, c[0].x, c[1].x, c[2].x, c[3].x, keep);
+                for (int j = 0; j < 4; ++j) {
+                    c[j] = __ldg(a.cv + min(i + j, e0 - 1));   // tail: repeat the last entry
+                    bulk_row64(smem_u32(xs + (size_t)q * 256 + 64 * j), a.xh + (size_t)c[j].x * 4, full, keep);
+                }
                 *reinterpret_cast<float4*>(vs + 4 * q) =
                     make_float4(__int_as_float(c[0].y), __int_as_float(c[1].y), __int_as_float(c[2].y),
                                 __int_as_float(c[3].y));
@@ -228,34 +227,7 @@ k_sweep_h_tma(const __grid_constant__ CUtensorMap tmap_x, const TmaSweepArgs a, 
     }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn g_encode_x = nullptr;
-
 }  // namespace
-
-// [n_rows, 32] fp16 state -> gather4 tensor map: box = one 64-byte row (the instruction names four rows)
-int tma_state_map(const void* xh, int64_t n_rows, void* map128) {
-    if (!g_encode_x) {
-        void* fn = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        HRAG_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres));
-        HRAG_CHECK(fn != nullptr && qres == cudaDriverEntryPointSuccess, "cuTensorMapEncodeTiled not available");
-        g_encode_x = reinterpret_cast<EncodeTiledFn>(fn);
-    }
-    static_assert(sizeof(CUtensorMap) == 128, "CUtensorMap is 128 bytes");
-    cuuint64_t gdim[2] = {(cuuint64_t)kB, (cuuint64_t)n_rows};
-    cuuint64_t gstride[1] = {(cuuint64_t)kB * 2};
-    cuuint32_t box[2] = {(cuuint32_t)kB, 1};
-    cuuint32_t estride[2] = {1, 1};
-    CUresult r = g_encode_x(reinterpret_cast<CUtensorMap*>(map128), CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
-                            const_cast<void*>(xh), gdim, gstride, box, estride, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    HRAG_CHECK(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (state map) failed (" + std::to_string((int)r) + ")");
-    return 0;
-}
 
 // Row blocks of the TMA sweep for local rows [0, n_rows): <= 64 rows, <= 1024 non-zeros; a long row is a block of
 // its own with bit 31 set.  Host helper (called at graph load).
@@ -279,7 +251,7 @@ void tma_build_blocks(const int* row_ptr, int n_rows, int long_thresh, std::vect
 }
 
 // MODE 0, non-final sweep over the short rows through the TMA gather; long rows are NOT handled here.
-int mixed_sweep_tma(const PprGraph& g, const void* map128, const int* slot_map, const void* rhs_h, const void* prevh,
+int mixed_sweep_tma(const PprGraph& g, const void* xh, const int* slot_map, const void* rhs_h, const void* prevh,
                     void* yh, float alpha, float w, const PeerOut& peers, cudaStream_t st) {
     HRAG_CHECK(g.tma_blk_row != nullptr && g.n_tma_blk > 0, "mixed_sweep_tma: row blocks not built");
     static bool attr_set = false;
@@ -290,6 +262,7 @@ int mixed_sweep_tma(const PprGraph& g, const void* map128, const int* slot_map, 
     }
     TmaSweepArgs a;
     a.n_blk = g.n_tma_blk;
+    a.xh = reinterpret_cast<const uint4*>(xh);
     a.blk_row = g.tma_blk_row;
     a.row_base = g.row_lo;
     a.row_ptr = g.row_ptr;
@@ -301,9 +274,8 @@ int mixed_sweep_tma(const PprGraph& g, const void* map128, const int* slot_map, 
     a.alpha = alpha;
     a.w = w;
     const int grid = std::min(g.n_tma_blk, g.num_sms);
-    const CUtensorMap& map = *reinterpret_cast<const CUtensorMap*>(map128);
-    if (prevh) k_sweep_h_tma<true><<<grid, kTmaThreads, kSmemBytes, st>>>(map, a, peers);
-    else k_sweep_h_tma<false><<<grid, kTmaThreads, kSmemBytes, st>>>(map, a, peers);
+    if (prevh) k_sweep_h_tma<true><<<grid, kTmaThreads, kSmemBytes, st>>>(a, peers);
+    else k_sweep_h_tma<false><<<grid, kTmaThreads, kSmemBytes, st>>>(a, peers);
     count_launch();
     HRAG_CUDA(cudaGetLastError());
     return 0;

@@ -1,4 +1,4 @@
-// K3 / K4 glue kernels (sm_100a): the reset vector of graph_search_with_fact_entities
+// K3 / K4 glue kernels (sm_90a): the reset vector of graph_search_with_fact_entities
 // (reference HippoRAG.py:1577-1638 + get_top_k_weights :1505-1542), the passage-score gather
 // of run_ppr (:1745) and the layout changes around hrag_ppr.  The reference does this with
 // O(N) + O(P) Python loops and md5/dict lookups per query; here the dicts are the integer

@@ -1,4 +1,4 @@
-// Selection kernels (sm_100a): per-query min/max + small top-k of the fact scores (the
+// Selection kernels (sm_90a): per-query min/max + small top-k of the fact scores (the
 // argsort of rerank_facts, reference HippoRAG.py:1683-1688, and min_max_normalize,
 // misc_utils.py:130-139) and the exact top-k of the passage scores (the argsort + slice of
 // run_ppr / _build_retrieval_result, HippoRAG.py:1746-1747, 501-507).

@@ -3,7 +3,7 @@
 // Replaces the per-query sgemv of get_fact_scores / dense_passage_retrieval (reference
 // HippoRAG.py:1459, :1496: np.dot(E, q)) with one batched contraction S = Q E^T.  This is the
 // HRAG_SIM_FP32 mode: every product is an exact fp32 FMA, so it is the in-library reference
-// the tcgen05 split-bf16 kernel (sim_tc.cu) is checked against, and the mode of choice for
+// the wgmma split-bf16 kernel (sim_tc.cu) is checked against, and the mode of choice for
 // tiny corpora.  Register-tiled 64x64x16, 4x4 outputs per thread, operands staged K-major in
 // shared memory.
 #include "common.cuh"

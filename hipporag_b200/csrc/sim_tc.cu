@@ -1,25 +1,22 @@
-// K2 -- batched query x embedding similarity on the 5th-gen tensor cores (tcgen05, sm_100a).
+// K2 -- batched query x embedding similarity on the Hopper tensor cores (wgmma, sm_90a).
 //
 // Replaces the per-query fp32 sgemv of get_fact_scores / dense_passage_retrieval (reference
 // HippoRAG.py:1459, :1496: np.dot(E, q)) with one batched contraction S = Q E^T:
-//   D[128 queries, 256 embeddings] (fp32, TMEM) += A[128, 64] (bf16, smem) * B[256, 64]^T (bf16, smem)
-// Both operands are K-major (a row = one embedding), staged by TMA (128-byte swizzle) into a
-// 4-stage shared-memory ring; one elected thread issues tcgen05.mma; accumulators live in TMEM,
-// double-buffered (2 x 256 columns) so the epilogue of tile t overlaps the MMAs of tile t+1.
+//   D[128 queries, 256 embeddings] (fp32, registers) += A[128, BK] (bf16, smem) * B[256, BK]^T (bf16, smem)
+// Both operands are K-major (a row = one embedding), staged by TMA (swizzled) into a 4-stage
+// shared-memory ring of 48-KB stages (192 KB of the 227 KB a block may use).  Warpgroup 2 issues the
+// TMA loads (one thread); warpgroups 0 and 1 each own 64 of the tile's 128 query rows, issue wgmma.m64n256k16 straight
+// from shared memory and keep their 64 x 256 fp32 accumulator in registers (128 per thread).
 //
 // Precision (SURVEY.md 7, hard part 3): a single bf16 pass flips top-k membership, so the parity
 // mode is the fp32-faithful split  x = hi + lo (both bf16, 16 mantissa bits together):
-//     q.e ~= q_lo.e_lo + q_hi.e_lo + q_lo.e_hi + q_hi.e_hi      (fp32 accumulate in TMEM)
+//     q.e ~= q_lo.e_lo + q_hi.e_lo + q_lo.e_hi + q_hi.e_hi      (fp32 accumulate)
 // All four products are issued per k-block from ONE stage holding {q_hi, q_lo, e_hi, e_lo}:
 // 4 products per byte-set of operand traffic, where three separate K-passes would move 1.5x the
-// bytes for 3.  Split stages are 32 K-columns wide (64-byte swizzle, 48 KB, 4 stages) so three
-// TMA batches are in flight while one is consumed (2 x 96-KB stages left the MMA issuer waiting
-// on load latency: ncu 39 % tensor pipe, profiles/r1_k2_sim_tc_ncu.md).  The lo.lo term is kept because it is systematic (always positive)
+// bytes for 3.  Split stages are 32 K-columns wide (64-byte swizzle), so three TMA batches are in
+// flight while one is consumed.  The lo.lo term is kept because it is systematic (always positive)
 // exactly for the highly correlated query/fact pairs that end up in the top-k.
-// HRAG_SIM_BF16 = hi.hi only (48 KB stages, 4 of them).
-//
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2..5 = epilogue (TMEM -> registers -> global, one query row per thread).
+// HRAG_SIM_BF16 = hi.hi only (64 K-columns a stage, 128-byte swizzle).
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -33,13 +30,18 @@ namespace hrag {
 
 namespace {
 
-constexpr int BM = 128;          // queries per tile  (UMMA M)
-constexpr int BN = 256;          // embeddings per tile (UMMA N)
+constexpr int BM = 128;          // queries per tile (two warpgroups x wgmma M = 64)
+constexpr int BN = 256;          // embeddings per tile (wgmma N)
 constexpr int BK = 64;           // bf16 elements per k-block = one 128-byte swizzle row
-constexpr int UK = 16;           // UMMA K for 16-bit inputs
-constexpr int RING_BYTES = 4 * (BM + BN) * BK * 2;   // 192 KB = 4 stages of 48 KB in both modes
-constexpr int TMEM_COLS = 512;                 // 2 accumulators x 256 fp32 columns
-constexpr int TC_THREADS = 192;
+constexpr int UK = 16;           // wgmma K for 16-bit inputs
+constexpr int STAGES = 4;
+constexpr int RING_BYTES = STAGES * (BM + BN) * BK * 2;   // 192 KB = 4 stages of 48 KB in both modes
+constexpr int CONSUMER_WARPS = 8;                          // warpgroups 0 and 1
+constexpr int PRODUCER_WARP = CONSUMER_WARPS;              // first warp of warpgroup 2: TMA
+constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 4);      // 384
+// register budget per thread: the producer warpgroup gives up what the consumers' 128-register accumulators need
+// (128 x 40 + 256 x 232 <= 64 K registers of the SM)
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
 constexpr size_t SMEM_BYTES = (size_t)RING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 
 // ---- PTX wrappers ------------------------------------------------------------------------
@@ -73,57 +75,55 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* map, int c0, int c1) {
     asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global [%0, {%1, %2}];" ::"l"(map), "r"(c0), "r"(c1) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers are written asynchronously by wgmma: pin every read after wgmma_wait
+__device__ __forceinline__ void acc_fence(float (&d)[128]) {
+#pragma unroll
+    for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols));
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
+
+#define HRAG_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                   "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64, 256] (fp32, 128 registers per thread of the warpgroup) (+)= A[64, 16] * B[256, 16]^T, both bf16 K-major in smem
+__device__ __forceinline__ void wgmma_bf16(float (&d)[128], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = TMEM lane = query row)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+        "setp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
         "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+        "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,"
+        "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,"
+        "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,"
+        "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,"
+        "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,"
+        "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, "
+        "%128, %129, p, 1, 1, 0, 0;\n\t"
+        "}"
+        : HRAG_D8(0), HRAG_D8(8), HRAG_D8(16), HRAG_D8(24), HRAG_D8(32), HRAG_D8(40), HRAG_D8(48), HRAG_D8(56),
+          HRAG_D8(64), HRAG_D8(72), HRAG_D8(80), HRAG_D8(88), HRAG_D8(96), HRAG_D8(104), HRAG_D8(112), HRAG_D8(120)
+        : "l"(desc_a), "l"(desc_b), "r"(accumulate)
+        : "memory");
 }
+#undef HRAG_D8
 
-// UMMA shared-memory descriptor of a K-major operand tile whose rows are ROW_BYTES wide
-// (128 -> SWIZZLE_128B, 64 -> SWIZZLE_64B): 8-row swizzle atoms 8*ROW_BYTES apart (SBO); LBO unused
-// for these layouts; descriptor version 1 (sm_100).
+// wgmma shared-memory descriptor of a K-major operand tile whose rows are ROW_BYTES wide
+// (128 -> SWIZZLE_128B, 64 -> SWIZZLE_64B): 8-row swizzle atoms 8*ROW_BYTES apart (SBO); LBO is
+// unused by these layouts.
 template <int ROW_BYTES>
-__device__ __forceinline__ uint64_t umma_desc_kmajor(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t gmma_desc_kmajor(uint32_t smem_addr) {
     static_assert(ROW_BYTES == 128 || ROW_BYTES == 64, "row = one swizzle span");
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);        // start address, 16-byte units
+    d |= (uint64_t)1 << 16;                              // leading byte offset (ignored)
     d |= (uint64_t)((8u * ROW_BYTES) >> 4) << 32;        // stride byte offset
-    d |= (uint64_t)1 << 46;                              // version
-    d |= (uint64_t)(ROW_BYTES == 128 ? 2 : 4) << 61;     // layout: SWIZZLE_128B = 2, SWIZZLE_64B = 4
+    d |= (uint64_t)(ROW_BYTES == 128 ? 1 : 2) << 62;     // layout: SWIZZLE_128B = 1, SWIZZLE_64B = 2
     return d;
 }
-// Instruction descriptor, kind::f16: D fp32, A/B bf16, both K-major, M = 128, N = 256.
-constexpr uint32_t kIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) |
-                            ((uint32_t)(BM >> 4) << 24);
 
 struct TcParams {
     int Bq;            // valid query rows
@@ -146,33 +146,63 @@ struct TcParams {
 
 constexpr int kFuseK = 8;
 
+__device__ __forceinline__ void insert_best(uint64_t (&best)[kFuseK], uint64_t key) {
+    if (key > best[kFuseK - 1]) {
+#pragma unroll
+        for (int k = 0; k < kFuseK; ++k)
+            if (key > best[k]) { const uint64_t tmp = best[k]; best[k] = key; key = tmp; }
+    }
+}
+__device__ __forceinline__ void cmp_swap_desc(uint64_t& a, uint64_t& b) {
+    const uint64_t hi = a > b ? a : b, lo = a > b ? b : a;
+    a = hi;
+    b = lo;
+}
+// best <- the 8 largest of best and lane (lane ^ off)'s best, both sorted descending: max(best[k], other[7 - k])
+// holds exactly those 8 as a bitonic sequence, which three compare-exchange rounds sort.  Pairs (k, 7 - k) are
+// exchanged together so neither lane reads an entry its partner has already replaced.
+__device__ __forceinline__ void merge_best_xor(uint64_t (&best)[kFuseK], int off) {
+#pragma unroll
+    for (int k = 0; k < kFuseK / 2; ++k) {
+        const uint64_t o_hi = __shfl_xor_sync(0xffffffffu, best[kFuseK - 1 - k], off);
+        const uint64_t o_lo = __shfl_xor_sync(0xffffffffu, best[k], off);
+        best[k] = best[k] > o_hi ? best[k] : o_hi;
+        best[kFuseK - 1 - k] = best[kFuseK - 1 - k] > o_lo ? best[kFuseK - 1 - k] : o_lo;
+    }
+#pragma unroll
+    for (int stride = kFuseK / 2; stride >= 1; stride >>= 1)
+#pragma unroll
+        for (int k = 0; k < kFuseK; ++k)
+            if ((k & stride) == 0) cmp_swap_desc(best[k], best[k + stride]);
+}
+
 template <bool SPLIT, int FUSE>          // FUSE: 0 = store scores, 1 = min/max + 8 best per tile, 2 = threshold append
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ CUtensorMap map_q_lo,
          const __grid_constant__ CUtensorMap map_e_hi, const __grid_constant__ CUtensorMap map_e_lo, TcParams p) {
-    constexpr int STAGES = 4;
     constexpr int BKs = SPLIT ? BK / 2 : BK;                 // K-columns per stage
-    constexpr int ROW_BYTES = BKs * 2;                       // = the TMA / UMMA swizzle span
+    constexpr int ROW_BYTES = BKs * 2;                       // = the TMA / wgmma swizzle span
     constexpr int A_BYTES = BM * ROW_BYTES, B_BYTES = BN * ROW_BYTES;
     constexpr int STAGE_BYTES = (SPLIT ? 2 : 1) * (A_BYTES + B_BYTES);   // 48 KB either way
     // stage layout: [A_hi | B_hi] or [A_hi | A_lo | B_hi | B_lo]
     constexpr int OFF_A_LO = A_BYTES, OFF_B_HI = SPLIT ? 2 * A_BYTES : A_BYTES, OFF_B_LO = 2 * A_BYTES + B_BYTES;
+    constexpr int WG_A_OFF = 64 * ROW_BYTES;                 // a warpgroup's 64 query rows inside an A tile
     extern __shared__ uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B tiles need 1024-B alignment
     const uint32_t bars = base + RING_BYTES;                      // barrier block
     auto full_bar = [&](int s) { return bars + 8u * s; };
     auto empty_bar = [&](int s) { return bars + 64u + 8u * s; };
-    auto tfull_bar = [&](int a) { return bars + 128u + 8u * a; };
-    auto tempty_bar = [&](int a) { return bars + 160u + 8u * a; };
-    const uint32_t tmem_slot = bars + 192u;
-    volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nkb = (p.dim + BKs - 1) / BKs;
     const int total_tiles = p.num_m_tiles * p.num_n_tiles;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONSUMER_WARPS); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    if (warp == PRODUCER_WARP && lane == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_e_hi) : "memory");
         if (SPLIT) {
@@ -180,21 +210,11 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
             asm volatile("prefetch.tensormap [%0];" ::"l"(&map_e_lo) : "memory");
         }
     }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-            for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 4); }
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-        tmem_alloc(tmem_slot, TMEM_COLS);
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
 
-    if (warp == 0) {
+    if (warp >= PRODUCER_WARP) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(PRODUCER_REGS));
+        if (warp != PRODUCER_WARP) return;
         // ===== TMA producer =====
         if (lane == 0) {
             int stage = 0;
@@ -203,7 +223,7 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                 const int mt = t % p.num_m_tiles, nt = t / p.num_m_tiles;
                 // L2 prefetch of this CTA's share of the NEXT embedding tile: the num_m_tiles CTAs that
                 // will work on it each pull every num_m_tiles-th k-block, a whole tile ahead, so the
-                // later TMA loads are L2 hits (ncu before: 3x algorithmic DRAM reads, 39 % tensor pipe)
+                // later TMA loads of all of them are L2 hits instead of num_m_tiles DRAM reads
                 const int tn = t + gridDim.x;
                 if (tn < total_tiles) {
                     const int mtn = tn % p.num_m_tiles, ntn = tn / p.num_m_tiles;
@@ -227,110 +247,106 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one thread) =====
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-                mbar_wait(tempty_bar(acc), acc_phase ^ 1u);     // epilogue drained this accumulator
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(full_bar(stage), phase);
-                    tc_fence_after();
-                    const uint32_t sa = base + stage * STAGE_BYTES;
-                    const uint64_t a_hi = umma_desc_kmajor<ROW_BYTES>(sa), b_hi = umma_desc_kmajor<ROW_BYTES>(sa + OFF_B_HI);
-                    if (p.debug_mode == 1) {
-                        // probe: no MMAs; the commits below complete immediately
-                    } else if (SPLIT) {
-                        const uint64_t a_lo = umma_desc_kmajor<ROW_BYTES>(sa + OFF_A_LO);
-                        const uint64_t b_lo = umma_desc_kmajor<ROW_BYTES>(sa + OFF_B_LO);
-                        // smallest terms first: lo.lo, hi.lo, lo.hi, then hi.hi
+        return;
+    }
+
+    // ===== consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64) of each tile =====
+    const int wg = warp >> 2;
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(CONSUMER_REGS));
+    float d[128];
 #pragma unroll
-                        for (int k = 0; k < BKs / UK; ++k)
-                            umma_bf16(tmem_d, a_lo + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), kIdesc,
-                                      (kb > 0 || k > 0) ? 1u : 0u);
+    for (int i = 0; i < 128; ++i) d[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+        const int mt = t % p.num_m_tiles, nt = t / p.num_m_tiles;
+        int prev_stage = -1;
+        for (int kb = 0; kb < nkb; ++kb) {
+            mbar_wait(full_bar(stage), phase);
+            const uint32_t sa = base + stage * STAGE_BYTES;
+            const uint64_t a_hi = gmma_desc_kmajor<ROW_BYTES>(sa + wg * WG_A_OFF);
+            const uint64_t b_hi = gmma_desc_kmajor<ROW_BYTES>(sa + OFF_B_HI);
+            if (p.debug_mode != 1) {
+                wgmma_fence();
+                if (SPLIT) {
+                    const uint64_t a_lo = gmma_desc_kmajor<ROW_BYTES>(sa + OFF_A_LO + wg * WG_A_OFF);
+                    const uint64_t b_lo = gmma_desc_kmajor<ROW_BYTES>(sa + OFF_B_LO);
+                    // smallest terms first: lo.lo, hi.lo, lo.hi, then hi.hi; +32 bytes (2 x 16-byte units) along K per step
 #pragma unroll
-                        for (int k = 0; k < BKs / UK; ++k)
-                            umma_bf16(tmem_d, a_hi + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), kIdesc, 1u);
+                    for (int k = 0; k < BKs / UK; ++k)
+                        wgmma_bf16(d, a_lo + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
 #pragma unroll
-                        for (int k = 0; k < BKs / UK; ++k)
-                            umma_bf16(tmem_d, a_lo + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), kIdesc, 1u);
+                    for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), 1u);
 #pragma unroll
-                        for (int k = 0; k < BKs / UK; ++k)
-                            umma_bf16(tmem_d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), kIdesc, 1u);
-                    } else {
+                    for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_lo + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), 1u);
 #pragma unroll
-                        for (int k = 0; k < BKs / UK; ++k)   // +32 bytes (2 x 16-byte units) along K per step
-                            umma_bf16(tmem_d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), kIdesc,
-                                      (kb > 0 || k > 0) ? 1u : 0u);
-                    }
-                    umma_commit(empty_bar(stage));               // smem slot free once these MMAs retire
-                    if (kb == nkb - 1) umma_commit(tfull_bar(acc));
-                    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+                    for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), 1u);
+                } else {
+#pragma unroll
+                    for (int k = 0; k < BKs / UK; ++k)
+                        wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
                 }
-                if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
+                wgmma_commit();
             }
+            // at most this k-block's MMAs are still in flight: the previous stage can be refilled
+            wgmma_wait<1>();
+            if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+            prev_stage = stage;
+            if (++stage == STAGES) { stage = 0; phase ^= 1u; }
         }
-    } else {
-        // ===== epilogue: warps 2..5, TMEM lane quarter = warp % 4 =====
-        const int quarter = warp & 3;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-            const int mt = t % p.num_m_tiles, nt = t / p.num_m_tiles;
-            mbar_wait(tfull_bar(acc), acc_phase);
-            tc_fence_after();
-            const int q = mt * BM + quarter * 32 + lane;
-            const int64_t n0 = (int64_t)nt * BN;
-            if (FUSE == 2) {
-                // this thread owns query q: every score of the tile that clears the threshold joins q's candidate list
-#pragma unroll 1
-                for (int c = 0; c < BN / 32; ++c) {
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + c * 32), r);
-                    if (q < p.Bq) {
+        wgmma_wait<0>();
+        acc_fence(d);
+        if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
+
+        // ===== epilogue from the wgmma accumulator layout: register 4j + 2h + c of this thread holds
+        // row 16 (warp % 4) + lane / 4 + 8h, column 8j + 2 (lane % 4) + c of the warpgroup's 64 x 256 block;
+        // the four lanes of a quad share a row and hold 64 of its 256 columns each
+        const int64_t n0 = (int64_t)nt * BN;
+        const int c0 = 2 * (lane & 3);
+        const int n_valid = p.M - n0 < BN ? (int)(p.M - n0) : BN;     // columns of this tile below M
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) {
-                            const int64_t col = n0 + c * 32 + j;
-                            const float f = __uint_as_float(r[j]);
-                            if (col < p.M && f >= p.thr) {
+        for (int h = 0; h < 2; ++h) {
+            const int q = mt * BM + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+            if (FUSE == 2) {
+                if (q < p.Bq) {
+#pragma unroll
+                    for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                        for (int c = 0; c < 2; ++c) {
+                            const int col = 8 * j + c0 + c;
+                            const float f = d[4 * j + 2 * h + c];
+                            if (col < n_valid && f >= p.thr) {
                                 const int pos = atomicAdd(p.cand_count + q, 1);
-                                if (pos < p.cand_cap) p.cand_keys[(size_t)q * p.cand_cap + pos] = rank_key(f, (uint32_t)col);
+                                if (pos < p.cand_cap) p.cand_keys[(size_t)q * p.cand_cap + pos] = rank_key(f, (uint32_t)(n0 + col));
                             }
                         }
-                    }
                 }
             } else if (FUSE == 1) {
-                // this thread owns query q: scan the tile's 256 scores once, keep min / max / 8 best
                 float mn = INFINITY, mx = -INFINITY;
                 uint64_t best[kFuseK];
 #pragma unroll
-                for (int j = 0; j < kFuseK; ++j) best[j] = 0ull;
-#pragma unroll 1
-                for (int c = 0; c < BN / 32; ++c) {
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + c * 32), r);
+                for (int k = 0; k < kFuseK; ++k) best[k] = 0ull;
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int64_t col = n0 + c * 32 + j;
-                        if (col < p.M) {
-                            const float f = __uint_as_float(r[j]);
+                for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int col = 8 * j + c0 + c;
+                        if (col < n_valid) {
+                            const float f = d[4 * j + 2 * h + c];
                             mn = fminf(mn, f);
                             mx = fmaxf(mx, f);
-                            uint64_t key = rank_key(f, (uint32_t)col);
-                            if (key > best[kFuseK - 1]) {
-#pragma unroll
-                                for (int k = 0; k < kFuseK; ++k)
-                                    if (key > best[k]) { const uint64_t tmp = best[k]; best[k] = key; key = tmp; }
-                            }
+                            insert_best(best, rank_key(f, (uint32_t)(n0 + col)));
                         }
                     }
+                // merge the quad's four partial results: after two butterfly rounds every lane holds the row's
+                // min / max and its 8 best keys
+#pragma unroll
+                for (int off = 1; off <= 2; off <<= 1) {
+                    mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, off));
+                    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+                    merge_best_xor(best, off);
                 }
-                if (q < p.Bq) {
+                if (q < p.Bq && (lane & 3) == 0) {
                     const size_t o = (size_t)q * p.num_n_tiles + nt;
                     p.part_mm[o] = make_float2(mn, mx);
 #pragma unroll
@@ -338,280 +354,15 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                         *reinterpret_cast<ulonglong2*>(p.part_keys + o * kFuseK + k) = make_ulonglong2(best[k], best[k + 1]);
                 }
             } else {
-            float* row = p.S + (size_t)q * p.ldS + n0;
-#pragma unroll 1
-            for (int c = 0; c < BN / 32; ++c) {
-                uint32_t r[32];
-                tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + c * 32), r);
                 if (q < p.Bq) {
+                    float* row = p.S + (size_t)q * p.ldS + n0;
 #pragma unroll
-                    for (int j = 0; j < 32; j += 4) {
-                        if (n0 + c * 32 + j < p.ldS)     // ldS is a multiple of 4: whole float4 in range
-                            *reinterpret_cast<float4*>(row + c * 32 + j) =
-                                make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                            __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-                    }
-                }
-            }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(acc));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, TMEM_COLS);
-    }
-}
-
-// ================================================================================================
-// 2-CTA variant of the split GEMM (tcgen05 cta_group::2).  A pair of CTAs on one TPC computes a
-// 256-query x 256-embedding tile: each CTA keeps its own 128 query rows (A) and loads only HALF of the
-// embedding tile (128 of the 256 B rows); the MMA unit reads both halves.  Per SM that is 32 KB of
-// operands per stage instead of 48 KB for the same MMA time and the 192-KB ring holds 6 stages instead
-// of 4.  Correct (same parity tests) but measured SLOWER than the 1-CTA kernel on B200 (221 vs 195 ms,
-// DESIGN.md section 4), so it is kept selectable (HRAG_SIM_2CTA=1) and is not the default.
-// Protocol: both CTAs' TMA loads complete on the LEADER's full barrier (count 2: leader arrive.expect_tx
-// + peer remote arrive); the leader's single MMA thread issues cta_group::2 MMAs and multicasts its
-// commits to both CTAs' empty / tmem-full barriers; the 8 epilogue warps of the pair arrive on the
-// leader's tmem-empty barrier.
-// ================================================================================================
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-    return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* map, uint32_t leader_bar, int c0,
-                                                int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(map), "r"(leader_bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t smem_dst, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(cols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols));
-}
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar) {   // arrives on `bar` in BOTH CTAs of the pair
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
-__device__ __forceinline__ void umma_bf16_2sm(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// kind::f16, D fp32, A/B bf16 K-major, N = 256, M = 256 (128 rows per CTA)
-constexpr uint32_t kIdesc2 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) |
-                             ((uint32_t)((2 * BM) >> 4) << 24);
-
-template <bool FUSE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1)
-k_sim_tc2(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ CUtensorMap map_q_lo,
-          const __grid_constant__ CUtensorMap map_e_hi /* box 32 x 128 */,
-          const __grid_constant__ CUtensorMap map_e_lo, TcParams p) {
-    constexpr int STAGES = 6;
-    constexpr int BKs = BK / 2, ROW_BYTES = BKs * 2;               // 32 K-columns, 64-byte swizzle rows
-    constexpr int A_BYTES = BM * ROW_BYTES;                        // 8 KB: this CTA's 128 query rows (hi or lo)
-    constexpr int BH_BYTES = (BN / 2) * ROW_BYTES;                 // 8 KB: this CTA's half of the embedding tile
-    constexpr int STAGE_BYTES = 2 * (A_BYTES + BH_BYTES);          // 32 KB  [A_hi | A_lo | B_hi | B_lo]
-    constexpr int OFF_A_LO = A_BYTES, OFF_B_HI = 2 * A_BYTES, OFF_B_LO = 2 * A_BYTES + BH_BYTES;
-    static_assert(STAGES * STAGE_BYTES == RING_BYTES, "ring size");
-    extern __shared__ uint8_t smem_raw[];
-    const uint32_t raw = smem_u32(smem_raw);
-    const uint32_t base = (raw + 1023u) & ~1023u;
-    const uint32_t bars = base + RING_BYTES;
-    auto full_bar = [&](int s) { return bars + 8u * s; };           // used in the leader only
-    auto empty_bar = [&](int s) { return bars + 64u + 8u * s; };
-    auto tfull_bar = [&](int a) { return bars + 128u + 8u * a; };
-    auto tempty_bar = [&](int a) { return bars + 160u + 8u * a; };  // used in the leader only
-    const uint32_t tmem_slot = bars + 192u;
-    volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + (tmem_slot - raw));
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const int nkb = (p.dim + BKs - 1) / BKs;
-    const int num_mp = (p.Bq + 2 * BM - 1) / (2 * BM);             // 256-query tiles
-    const int total = num_mp * p.num_n_tiles;
-    const int cluster_id = blockIdx.x >> 1, n_clusters = gridDim.x >> 1;
-
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_e_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_e_lo) : "memory");
-    }
-    if (warp == 1) {
-        if (lane == 0) {
-            for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 2); mbar_init(empty_bar(s), 1); }
-            for (int a = 0; a < 2; ++a) { mbar_init(tfull_bar(a), 1); mbar_init(tempty_bar(a), 8); }
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncwarp();
-        tmem_alloc_2sm(tmem_slot, TMEM_COLS);
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();            // peer barriers are initialised before anyone signals them
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_ptr;
-
-    if (warp == 0) {
-        // ===== TMA producer (one per CTA): own query rows + own half of the embedding tile =====
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int w = cluster_id; w < total; w += n_clusters) {
-                const int mp = w % num_mp, nt = w / num_mp;
-                const int row_a = mp * 2 * BM + (int)rank * BM;
-                const int row_b = nt * BN + (int)rank * (BN / 2);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(empty_bar(stage), phase ^ 1u);
-                    const uint32_t lbar = mapa_u32(full_bar(stage), 0);
-                    if (leader) mbar_expect_tx(full_bar(stage), 2 * STAGE_BYTES);
-                    else mbar_arrive_cluster(lbar);
-                    const uint32_t sa = base + stage * STAGE_BYTES;
-                    tma_load_2d_2sm(sa, &map_q_hi, lbar, kb * BKs, row_a);
-                    tma_load_2d_2sm(sa + OFF_A_LO, &map_q_lo, lbar, kb * BKs, row_a);
-                    tma_load_2d_2sm(sa + OFF_B_HI, &map_e_hi, lbar, kb * BKs, row_b);
-                    tma_load_2d_2sm(sa + OFF_B_LO, &map_e_lo, lbar, kb * BKs, row_b);
-                    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
+                    for (int j = 0; j < BN / 8; ++j)
+                        if (n0 + 8 * j + c0 < p.ldS)     // ldS is a multiple of 4: the whole float2 is in range
+                            *reinterpret_cast<float2*>(row + 8 * j + c0) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer: one thread of the LEADER CTA drives both tensor cores =====
-        if (leader && lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0;
-            int acc = 0;
-            uint32_t acc_phase = 0;
-            for (int w = cluster_id; w < total; w += n_clusters) {
-                mbar_wait(tempty_bar(acc), acc_phase ^ 1u);      // both CTAs' epilogues drained this accumulator
-                tc_fence_after();
-                const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-                for (int kb = 0; kb < nkb; ++kb) {
-                    mbar_wait(full_bar(stage), phase);
-                    tc_fence_after();
-                    const uint32_t sa = base + stage * STAGE_BYTES;
-                    const uint64_t a_hi = umma_desc_kmajor<ROW_BYTES>(sa), a_lo = umma_desc_kmajor<ROW_BYTES>(sa + OFF_A_LO);
-                    const uint64_t b_hi = umma_desc_kmajor<ROW_BYTES>(sa + OFF_B_HI);
-                    const uint64_t b_lo = umma_desc_kmajor<ROW_BYTES>(sa + OFF_B_LO);
-#pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k)
-                        umma_bf16_2sm(tmem_d, a_lo + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), kIdesc2,
-                                      (kb > 0 || k > 0) ? 1u : 0u);
-#pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k)
-                        umma_bf16_2sm(tmem_d, a_hi + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), kIdesc2, 1u);
-#pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k)
-                        umma_bf16_2sm(tmem_d, a_lo + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), kIdesc2, 1u);
-#pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k)
-                        umma_bf16_2sm(tmem_d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), kIdesc2, 1u);
-                    umma_commit_2sm(empty_bar(stage));           // frees the slot in both CTAs
-                    if (kb == nkb - 1) umma_commit_2sm(tfull_bar(acc));
-                    if (++stage == STAGES) { stage = 0; phase ^= 1u; }
-                }
-                if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-            }
-        }
-    } else {
-        // ===== epilogue (both CTAs): warps 2..5, TMEM lane quarter = warp % 4 =====
-        const int quarter = warp & 3;
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        for (int w = cluster_id; w < total; w += n_clusters) {
-            const int mp = w % num_mp, nt = w / num_mp;
-            mbar_wait(tfull_bar(acc), acc_phase);
-            tc_fence_after();
-            const int q = mp * 2 * BM + (int)rank * BM + quarter * 32 + lane;
-            const int64_t n0 = (int64_t)nt * BN;
-            if (FUSE) {
-                float mn = INFINITY, mx = -INFINITY;
-                uint64_t best[kFuseK];
-#pragma unroll
-                for (int j = 0; j < kFuseK; ++j) best[j] = 0ull;
-#pragma unroll 1
-                for (int c = 0; c < BN / 32; ++c) {
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + c * 32), r);
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int64_t col = n0 + c * 32 + j;
-                        if (col < p.M) {
-                            const float f = __uint_as_float(r[j]);
-                            mn = fminf(mn, f);
-                            mx = fmaxf(mx, f);
-                            uint64_t key = rank_key(f, (uint32_t)col);
-                            if (key > best[kFuseK - 1]) {
-#pragma unroll
-                                for (int k = 0; k < kFuseK; ++k)
-                                    if (key > best[k]) { const uint64_t tmp = best[k]; best[k] = key; key = tmp; }
-                            }
-                        }
-                    }
-                }
-                if (q < p.Bq) {
-                    const size_t o = (size_t)q * p.num_n_tiles + nt;
-                    p.part_mm[o] = make_float2(mn, mx);
-#pragma unroll
-                    for (int k = 0; k < kFuseK; k += 2)
-                        *reinterpret_cast<ulonglong2*>(p.part_keys + o * kFuseK + k) = make_ulonglong2(best[k], best[k + 1]);
-                }
-            } else {
-                float* row = p.S + (size_t)q * p.ldS + n0;
-#pragma unroll 1
-                for (int c = 0; c < BN / 32; ++c) {
-                    uint32_t r[32];
-                    tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(acc * BN + c * 32), r);
-                    if (q < p.Bq) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            if (n0 + c * 32 + j < p.ldS)
-                                *reinterpret_cast<float4*>(row + c * 32 + j) =
-                                    make_float4(__uint_as_float(r[j]), __uint_as_float(r[j + 1]),
-                                                __uint_as_float(r[j + 2]), __uint_as_float(r[j + 3]));
-                        }
-                    }
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa_u32(tempty_bar(acc), 0));
-            if (++acc == 2) { acc = 0; acc_phase ^= 1u; }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();            // nobody frees TMEM / exits while the pair still uses its smem or barriers
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm(tmem_base, TMEM_COLS);
     }
 }
 
@@ -728,8 +479,6 @@ int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const v
         HRAG_CUDA(cudaFuncSetAttribute(k_sim_tc<false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
         HRAG_CUDA(cudaFuncSetAttribute(k_sim_tc<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
         HRAG_CUDA(cudaFuncSetAttribute(k_sim_tc<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-        HRAG_CUDA(cudaFuncSetAttribute(k_sim_tc2<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
-        HRAG_CUDA(cudaFuncSetAttribute(k_sim_tc2<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
         attr_set = true;
     }
     CUtensorMap mqh, mql, meh, mel;
@@ -750,23 +499,6 @@ int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const v
     const int64_t tiles = (int64_t)p.num_m_tiles * p.num_n_tiles;
     int grid = (int)std::min<int64_t>(tiles, num_sms);
     if (const char* eg = getenv("HRAG_SIM_GRID")) grid = std::max(1, std::min(grid, atoi(eg)));   // experiment knob
-    // HRAG_SIM_2CTA=1 selects the cta_group::2 kernel.  Measured on B200 (C3 stage A, 10k queries): 221 ms
-    // vs 195 ms for the 1-CTA kernel -- fewer operand bytes per SM did not help, so it is not the default.
-    static int use_2cta = -1;
-    if (use_2cta < 0) { const char* e2 = getenv("HRAG_SIM_2CTA"); use_2cta = e2 ? atoi(e2) : 0; }
-    if (n_seg == 4 && use_2cta && num_sms >= 2) {
-        CUtensorMap meh2, mel2;                                  // embedding maps with a 128-row box (half tile)
-        HRAG_TRY(make_map(&meh2, e_hi, M, dim, bkc, BN / 2));
-        HRAG_TRY(make_map(&mel2, e_lo, M, dim, bkc, BN / 2));
-        const int64_t work = (int64_t)ceil_div(Bq, 2 * BM) * p.num_n_tiles;
-        int g2 = (int)std::min<int64_t>(work, num_sms / 2) * 2;
-        if (const char* eg = getenv("HRAG_SIM_GRID")) g2 = std::max(2, std::min(g2, atoi(eg) & ~1));
-        if (fuse) k_sim_tc2<true><<<g2, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh2, mel2, p);
-        else k_sim_tc2<false><<<g2, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh2, mel2, p);
-        count_launch(1);
-        HRAG_CUDA(cudaGetLastError());
-        return 0;
-    }
     if (n_seg == 4 && fuse) k_sim_tc<true, 1><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
     else if (n_seg == 4) k_sim_tc<true, 0><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
     else if (fuse) k_sim_tc<false, 1><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);

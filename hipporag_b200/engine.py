@@ -1,7 +1,7 @@
-"""Python host side of the B200 retrieval engine: thin, typed wrappers over the C ABI.
+"""Python host side of the H100 retrieval engine: thin, typed wrappers over the C ABI.
 
 ``Engine`` mirrors the state ``HippoRAG.prepare_retrieval_objects`` materialises
-(``/root/reference/src/hipporag/HippoRAG.py:1287-1389``) -- graph, integer tables, fact and
+(reference ``src/hipporag/HippoRAG.py:1287-1389``) -- graph, integer tables, fact and
 passage embeddings -- as device-resident arrays, and exposes the two GPU stages that bracket the
 recognition-memory (LLM) filter of ``HippoRAG.retrieve`` (``:459-480``):
 
@@ -105,7 +105,7 @@ def _ptr(a: Optional[np.ndarray]):
 
 
 class Engine:
-    """One handle = one B200.  Not thread-safe (like the reference's ``HippoRAG`` object)."""
+    """One handle = one H100.  Not thread-safe (like the reference's ``HippoRAG`` object)."""
 
     def __init__(self, device: int = 0, shard_mode: int = 0):
         self._lib = _lib.load()

@@ -1,10 +1,10 @@
-"""Index-time synonymy KNN on the B200 engine (SURVEY.md 8(f)-2).
+"""Index-time synonymy KNN on the H100 engine (SURVEY.md 8(f)-2).
 
 Drop-in for ``hipporag.utils.embed_utils.retrieve_knn``
-(``/root/reference/src/hipporag/utils/embed_utils.py:6-94``, called from ``add_synonymy_edges``,
+(reference ``src/hipporag/utils/embed_utils.py:6-94``, called from ``add_synonymy_edges``,
 ``HippoRAG.py:986-992``): cosine top-k of every query vector against all key vectors.  The reference
 tiles ``torch.mm`` + ``torch.topk`` with CPU<->GPU ping-pong per tile; here the keys are uploaded once
-and every query chunk is one tcgen05 GEMM.
+and every query chunk is one wgmma GEMM.
 
 Two forms:
 

@@ -2,7 +2,7 @@
 
 There is no network for datasets, so configs C2-C5 are generated: a knowledge graph with
 the edge mix the reference's ``index()`` produces on MuSiQue
-(``/root/reference/src/hipporag/HippoRAG.py:867-957,959-1020``):
+(reference ``src/hipporag/HippoRAG.py:867-957,959-1020``):
 
 * ~55 % of the igraph edges are *fact* edges, emitted as PAIRS of parallel edges (s,o) and
   (o,s), each carrying the co-occurrence count (``:907-910``);

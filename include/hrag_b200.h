@@ -1,9 +1,9 @@
-/* hrag_b200.h -- C ABI of libhrag_b200.so: HippoRAG's online retrieval hot path on B200 (sm_100a).
+/* hrag_b200.h -- C ABI of libhrag_b200.so: HippoRAG's online retrieval hot path on H100 (sm_90a).
  *
  * The reference (OSU-NLP-Group/HippoRAG) is pure Python and has no FFI of its own; the
  * boundary this library replaces is a set of methods on the `HippoRAG` object.  Each entry
  * point below names the reference code it stands in for (paths under
- * /root/reference/src/hipporag/).  INTEGRATION.md shows the ctypes binding a maintainer
+ * the reference's src/hipporag/).  INTEGRATION.md shows the ctypes binding a maintainer
  * would add on the reference side.
  *
  * Conventions: every function returns 0 on success, non-zero on failure
@@ -36,8 +36,8 @@ typedef struct hrag_handle hrag_t;
 
 /* Similarity precision modes. */
 #define HRAG_SIM_FP32     0   /* SIMT fp32 FMA kernel (exact fp32 products)                  */
-#define HRAG_SIM_BF16X3   1   /* tcgen05 bf16 hi/lo split, all 4 products, fp32-faithful (default) */
-#define HRAG_SIM_BF16     2   /* tcgen05 single bf16 pass (fast mode, NOT the parity mode)    */
+#define HRAG_SIM_BF16X3   1   /* wgmma bf16 hi/lo split, all 4 products, fp32-faithful (default)   */
+#define HRAG_SIM_BF16     2   /* wgmma single bf16 pass (fast mode, NOT the parity mode)      */
 
 typedef struct hrag_stats {
     double ms_sim_fact;      /* stage A: query x fact similarity (K2)                 */

@@ -15,7 +15,7 @@ Parity status
   offline and ``tests/golden/`` holds its outputs.
 * Row E (the PPR solve itself) is **parity unpinned** at the igraph boundary:
   the arithmetic lives in python-igraph 0.11.8 -> igraph C core 0.10.x ->
-  PRPACK, none of which is in /root/reference or installed here.  The oracle
+  PRPACK, none of which is in the reference checkout or installable offline.  The oracle
   restates the published definition (see ``oracle/ppr.py``), is cross-checked
   against ``networkx.pagerank`` (an independent implementation of the same
   definition) and hand-derived closed forms, and a gated test compares with the

@@ -3,7 +3,7 @@ reference's own dtypes -- the timed ``cpu_baseline`` / ``--impl reference`` leg 
 TEST / BENCH INFRASTRUCTURE ONLY (see ``oracle/__init__.py``).
 
 ``oracle/retrieve.py`` is the float64 *arbiter*; this file is the *stopwatch*: the same serial
-one-query-at-a-time loop as ``HippoRAG.retrieve`` (``/root/reference/src/hipporag/HippoRAG.py:459-480``)
+one-query-at-a-time loop as ``HippoRAG.retrieve`` (reference ``src/hipporag/HippoRAG.py:459-480``)
 with fp32 BLAS ``np.dot`` for the two similarities (``:1459``, ``:1496``), full ``np.argsort``
 (``:1500``, ``:1688``, ``:1746``) and a PPR solve to PRPACK's 1e-10 tolerance.  python-igraph is
 not installable offline, so the PPR is a scipy float64 CSR power iteration (kind = "port");

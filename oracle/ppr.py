@@ -2,13 +2,13 @@
 igraph/PRPACK.  TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``).
 
 **Parity unpinned at the igraph boundary**: the reference's call site is
-``/root/reference/src/hipporag/HippoRAG.py:1736-1743``
+reference ``src/hipporag/HippoRAG.py:1736-1743``
 
     graph.personalized_pagerank(vertices=range(N), damping=damping, directed=False,
                                 weights='weight', reset=reset_prob, implementation='prpack')
 
 and the arithmetic is in python-igraph 0.11.8 (``requirements.txt:9``) -> igraph C
-core 0.10.x -> bundled PRPACK, which is neither under /root/reference nor
+core 0.10.x -> bundled PRPACK, which is neither in the reference checkout nor
 installed.  What is restated here is the published definition:
 
 * the graph is an undirected multigraph (``config_utils.py:176``); parallel edges

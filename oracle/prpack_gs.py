@@ -5,7 +5,7 @@ TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``).
 Why it exists: ``oracle/ppr.py`` defines PPR through the linear system ``(I - aP) x = v`` and its
 three solvers (LU, power iteration, networkx) all check that one formula.  The reference calls
 ``graph.personalized_pagerank(..., implementation='prpack')`` (``HippoRAG.py:1736-1743``);
-python-igraph 0.11.8 -> igraph C core 0.10 -> bundled PRPACK is not under /root/reference and is
+python-igraph 0.11.8 -> igraph C core 0.10 -> bundled PRPACK is not in the reference checkout and is
 not installable offline, so the **parity of row E stays unpinned**.  What can be done offline is
 to restate what PRPACK computes, from its own formulation, and check that it lands on the same
 numbers -- in particular the two claims DESIGN.md makes about the igraph side:

@@ -1,6 +1,7 @@
 """Runs the reference's own, unmodified ``HippoRAG`` class offline.
-TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``); usable only where
-``/root/reference`` exists (this container, not the GPU box).
+TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``); usable only where a checkout of the
+reference exists, named by the ``HIPPORAG_REFERENCE_ROOT`` environment variable.  The tests never
+need it: what they compare with the reference's run is stored under ``tests/golden/``.
 
 Recipe (SURVEY.md appendix B): inert stub modules for the network/LLM dependencies
 that are not installed, ``oracle/fake_igraph.py`` registered as ``igraph``, the shipped
@@ -20,7 +21,7 @@ import types
 
 import numpy as np
 
-REFERENCE_ROOT = "/root/reference"
+REFERENCE_ROOT = os.environ.get("HIPPORAG_REFERENCE_ROOT", "")
 
 
 class _Anything:

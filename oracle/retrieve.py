@@ -2,7 +2,7 @@
 A-F) on integer tables.  TEST INFRASTRUCTURE ONLY (see ``oracle/__init__.py``).
 
 Every function cites the reference lines it follows (paths under
-``/root/reference/src/hipporag/``).  Differences from the reference, all deliberate:
+the reference's ``src/hipporag/``).  Differences from the reference, all deliberate:
 
 * arithmetic is float64 from the same fp32 inputs (the reference's ``np.dot`` is an
   fp32 BLAS sgemv whose summation order no GPU kernel reproduces; float64 is the

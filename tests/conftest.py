@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     # the shared library is a build artefact (git-ignored): build it in-tree when a checkout lacks it
     lib = os.path.join(ROOT, "hipporag_b200", "libhrag_b200.so")
     if not os.path.exists(lib):

@@ -1,5 +1,5 @@
 """A duck-typed stand-in for the reference's ``HippoRAG`` object (and the two helpers of
-``hipporag.utils.misc_utils`` the drop-in imports), for boxes where /root/reference is absent.
+``hipporag.utils.misc_utils`` the drop-in imports), for machines without a checkout of the reference.
 Only what ``hipporag_b200.accelerate`` touches is modelled."""
 import hashlib
 import sys
@@ -180,3 +180,63 @@ class FakeRag:
 
     def delete(self, docs):
         self.ready_to_retrieve = False
+
+
+class GoldenRag(FakeRag):
+    """The reference's own ``HippoRAG`` object as stored by ``tests/golden/make_accelerate_golden.py``: its graph, node
+    names, fact rows and entity -> chunk counts, embeddings regenerated from the stored seeds, queries embedded with the
+    reference's instructions by the same md5-seeded mock model.  Passage ``i`` reads as ``passage_doc(i)``."""
+
+    def __init__(self, g, working_dir):
+        import json
+        from oracle.ref_harness import MockEmbeddingModel, seeded_unit_vectors
+        cfg = json.loads(str(g["config"]))
+        self.global_config = types.SimpleNamespace(**cfg)
+        self.working_dir = working_dir
+        names = [str(n) for n in g["vertex_names"]]
+        graph = Graph(directed=False)
+        graph.add_vertices(len(names), attributes={"name": names})
+        graph.add_edges([tuple(e) for e in g["graph_edges"].tolist()], attributes={"weight": g["graph_weights"].tolist()})
+        self.graph = graph
+        self.passage_node_keys = [str(k) for k in g["passage_node_keys"]]
+        self.fact_node_keys = [str(k) for k in g["fact_node_keys"]]
+        self.fact_embedding_store = _Store(self.fact_node_keys, [str(c) for c in g["fact_contents"]])
+        self.chunk_embedding_store = _Store(self.passage_node_keys,
+                                            [self.passage_doc(i) for i in range(len(self.passage_node_keys))])
+        self.chunk_metadata = {}
+        dim = int(g["dim"])
+        self._fact_emb = seeded_unit_vectors(g["fact_seed"], dim)
+        self._passage_emb = seeded_unit_vectors(g["passage_seed"], dim)
+        self._ent_chunks = {str(k): set(range(int(c))) for k, c in zip(g["ent_chunk_keys"], g["ent_chunk_counts"])}
+        self._embed = MockEmbeddingModel(dim)
+        self._instr = {"triple": str(g["q_fact_instruction"]), "passage": str(g["q_passage_instruction"])}
+        self.ready_to_retrieve = False
+        self.ppr_time = self.rerank_time = self.all_retrieval_time = 0.0
+        self.rerank_filter = lambda q, cands, idxs, len_after_rerank=None: (idxs[:len_after_rerank],
+                                                                          cands[:len_after_rerank], {})
+        self.prompt_template_manager = types.SimpleNamespace(
+            is_template_name_valid=lambda name: True,
+            render=lambda name, prompt_user: [{"role": "user", "content": prompt_user}])
+        self.entity_keys = [n for n in names if n.startswith("entity-")]
+        self.set_entity_embeddings(np.zeros((len(self.entity_keys), dim), np.float32))
+
+    @staticmethod
+    def passage_doc(i):
+        return f"passage {int(i)}"
+
+    def prepare_retrieval_objects(self):
+        """HippoRAG.py:1287-1389: vertex lookup from the graph's names, embeddings of the stores."""
+        self.node_name_to_vertex_idx = {n: i for i, n in enumerate(self.graph.vs["name"])}
+        self.passage_node_idxs = [self.node_name_to_vertex_idx[k] for k in self.passage_node_keys]
+        self.fact_embeddings, self.passage_embeddings = self._fact_emb, self._passage_emb
+        self.ent_node_to_chunk_ids = dict(self._ent_chunks)
+        self.query_to_embedding = {"triple": {}, "passage": {}}
+        self.ready_to_retrieve = True
+
+    def get_query_embeddings(self, queries):
+        """HippoRAG.py:1391-1425: every new query string embedded with the reference's two query instructions."""
+        for kind in ("triple", "passage"):
+            new = [q for q in queries if q not in self.query_to_embedding[kind]]
+            if new:
+                for q, v in zip(new, self._embed.batch_encode(new, instruction=self._instr[kind])):
+                    self.query_to_embedding[kind][q] = v

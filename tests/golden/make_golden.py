@@ -3,11 +3,11 @@
 the first 1,000 MuSiQue passages of the shipped OpenIE file, the first 64 MuSiQue questions,
 768-d md5-seeded mock embeddings, identity recognition-memory filter.
 
-Run here (needs /root/reference):   PYTHONHASHSEED=0 python tests/golden/make_golden.py
+Needs a checkout of the reference:   HIPPORAG_REFERENCE_ROOT=<path> PYTHONHASHSEED=0 python tests/golden/make_golden.py
 
 What the file pins: rows A-D and F of SURVEY.md 8(a) come from the reference's code
 verbatim.  Row E (PPR) went through ``oracle/fake_igraph.py`` -- python-igraph is not
-installable here -- so the PPR scores in it are the oracle's float64 direct solve, NOT
+installable offline -- so the PPR scores in it are the oracle's float64 direct solve, NOT
 PRPACK's ("parity unpinned" at that boundary).
 
 Embeddings are not stored (33 MB); the fixture keeps their 64-bit seeds and tests rebuild

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), f"libhrag_b200.so does not export {n}"
     assert sorted(_lib.SIGNATURES) == names, "ctypes SIGNATURES out of sync with include/hrag_b200.h"
-    assert b"sm_100a" in lib.hrag_version()
+    assert b"sm_90a" in lib.hrag_version()
 
 
 def test_no_cpu_fallback_without_a_device():

@@ -1,5 +1,5 @@
 """The drop-in (hipporag_b200.accelerate): host glue against the reference's own object (CPU,
-oracle-backed engine double) and the GPU path through a duck-typed HippoRAG (GPU box)."""
+oracle-backed engine double) and the GPU path through a duck-typed HippoRAG (GPU)."""
 import os
 import tempfile
 
@@ -62,13 +62,32 @@ class OracleEngine:
         return ids, sc
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/src"), reason="needs the reference checkout")
+class FakeQALLM:
+    """IRCoT reasoning stand-in: the thought depends on the question and on how many thoughts came before."""
+    def infer(self, messages):
+        text = messages[-1]["content"] if isinstance(messages[-1], dict) else str(messages[-1])
+        q = text.rsplit("Question:", 1)[-1]
+        n_prev = q.count("thought-")
+        tag = "thought-%d about %s" % (n_prev, q.split("\n")[0].strip()[:40])
+        return [tag + (" So the answer is: x" if n_prev >= 1 and len(q) % 2 == 0 else "")]
+
+
 def test_accelerate_glue_against_reference_object():
-    from oracle import ref_harness as H
+    """The drop-in on the state of the reference's own HippoRAG object after index() of 150 MuSiQue passages, against
+    what the reference's own methods returned on that object (tests/golden/accelerate_glue150.npz, made by
+    tests/golden/make_accelerate_golden.py): retrieve, the serial retrieve_ircot loop, retrieve at linking_top_k 10."""
+    import json
+    from tests import fake_hipporag
+    fake_hipporag.install_stub_package()
     import hipporag_b200
-    rag = H.build_reference_rag(tempfile.mkdtemp(prefix="hrag_acc_"), 150, 64)
-    questions = H.musique_questions(12)
-    ref = rag.retrieve(questions, num_to_retrieve=20)
+    from hipporag.utils.misc_utils import QuerySolution
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "accelerate_glue150.npz"))
+    rag = fake_hipporag.GoldenRag(g, tempfile.mkdtemp(prefix="hrag_acc_"))
+    questions = [str(q) for q in g["questions"]]
+    doc = rag.passage_doc
+    ref = [QuerySolution(question=q, docs=[doc(i) for i in ids], doc_scores=sc,
+                           graph_seeds=[tuple(f) for f in seeds])
+           for q, ids, sc, seeds in zip(questions, g["ref_ids"], g["ref_scores"], json.loads(str(g["ref_seeds"])))]
     hipporag_b200.accelerate(rag, engine=OracleEngine())
     rag.ready_to_retrieve = False
     acc = rag.retrieve(questions, num_to_retrieve=20)
@@ -89,21 +108,15 @@ def test_accelerate_glue_against_reference_object():
     rag.ready_to_retrieve = False
     par = rag.retrieve(questions, num_to_retrieve=20)
     assert [p.docs for p in par] == [a.docs for a in acc]
-    # IRCoT: the batched, step-synchronous drop-in must equal the reference's serial loop
-    class FakeQALLM:
-        def infer(self, messages):
-            text = messages[-1]["content"] if isinstance(messages[-1], dict) else str(messages[-1])
-            q = text.rsplit("Question:", 1)[-1]
-            n_prev = q.count("thought-")
-            tag = "thought-%d about %s" % (n_prev, q.split("\n")[0].strip()[:40])
-            return [tag + (" So the answer is: x" if n_prev >= 1 and len(q) % 2 == 0 else "")]
+    # IRCoT: the batched, step-synchronous drop-in must equal the reference's serial loop (over single-query
+    # retrieve calls of the same drop-in)
     rag.qa_llm = FakeQALLM()
-    serial_ircot = type(rag).retrieve_ircot                    # the reference's own method (HippoRAG.py:509)
-    want = serial_ircot(rag, questions[:6], max_qa_steps=3, num_to_retrieve=10)
     got = rag.retrieve_ircot(questions[:6], max_qa_steps=3, num_to_retrieve=10)
-    for a, b in zip(got, want):
-        assert a.docs == b.docs and a.thoughts == b.thoughts
-        np.testing.assert_allclose(a.doc_scores, b.doc_scores)
+    want = zip(json.loads(str(g["ircot_ids"])), json.loads(str(g["ircot_scores"])), json.loads(str(g["ircot_thoughts"])))
+    assert len(got) == 6
+    for a, (ids, scores, thoughts) in zip(got, want):
+        assert a.docs == [doc(i) for i in ids] and a.thoughts == thoughts
+        np.testing.assert_allclose(a.doc_scores, scores)
     # the binary cache (8(f)-3): written next to graph.pickle on the first prepare, reused while the index is unchanged
     import sys as _sys
     from hipporag_b200 import cache as cache_mod
@@ -135,12 +148,10 @@ def test_accelerate_glue_against_reference_object():
     orig_filter = rag.rerank_filter
     rag.rerank_filter = lambda q, c, i, len_after_rerank=None: (seen.append(len(c)) or (i[:len_after_rerank], c[:len_after_rerank], {}))
     rag.global_config.linking_top_k = 10
-    ref10 = type(rag).retrieve(rag, questions[:4], num_to_retrieve=10)      # the reference's own method
-    seen.clear()
     acc10 = rag.retrieve(questions[:4], num_to_retrieve=10)
     assert seen == [10, 10, 10, 10]
-    for a, r in zip(acc10, ref10):
-        assert [tuple(f) for f in a.graph_seeds] == [tuple(f) for f in r.graph_seeds] and len(a.graph_seeds) == 10
+    for a, r in zip(acc10, json.loads(str(g["ref10_seeds"]))):
+        assert [tuple(f) for f in a.graph_seeds] == [tuple(f) for f in r] and len(a.graph_seeds) == 10
     rag.global_config.linking_top_k = 40
     with pytest.raises(ValueError, match="linking_top_k"):
         rag.retrieve(questions[:2], num_to_retrieve=5)
@@ -148,7 +159,7 @@ def test_accelerate_glue_against_reference_object():
     rag.rerank_filter = orig_filter
     # add_synonymy_edges is wrapped: the KNN it calls is swapped for the engine's for the duration of the call only
     import sys
-    ref_mod = sys.modules[type(rag).__module__]              # hipporag.HippoRAG, the module (the package re-exports the class)
+    ref_mod = sys.modules[type(rag).__module__]              # the module whose retrieve_knn add_synonymy_edges calls
     from hipporag_b200 import knn as knn_mod
     calls = {}
 

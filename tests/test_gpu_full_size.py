@@ -71,7 +71,7 @@ def test_full_size_spot_check_against_the_oracle(c3):
 
 
 def test_full_size_768_wide_against_the_oracle():
-    """The exact configuration bench.py times (C3 at d = 768): 40 queries through the default path (tcgen05 split
+    """The exact configuration bench.py times (C3 at d = 768): 40 queries through the default path (wgmma split
     GEMM with the fused selection epilogue, mixed-precision PPR), 8 of them checked against the float64 oracle --
     top-5 facts identical, top-200 passages and scores per tests/util.py."""
     import hipporag_b200 as hb

@@ -282,27 +282,6 @@ def test_similarity_modes_vs_float64(hb, dim, rows, bq):
     assert idx[0, 0] == 3
 
 
-def test_two_cta_gemm_variant_in_a_subprocess():
-    """The cta_group::2 kernel (HRAG_SIM_2CTA=1, read once per process) must give the same answers."""
-    import subprocess, sys, os
-    code = (
-        "import numpy as np, hipporag_b200 as hb\n"
-        "from hipporag_b200 import synth\n"
-        "E = synth.unit_rows(3000, 768, seed=1); Q = synth.unit_rows(300, 768, seed=2); Q[0] = E[3]\n"
-        "e = hb.Engine(0); e.load_embeddings(E, synth.unit_rows(8, 768, seed=9))\n"
-        "i1, s1, _ = e.stage_a(Q, 5)\n"
-        "e.debug_keep_scores(True); i2, s2, _ = e.stage_a(Q, 5); got = e.debug_scores(0)\n"
-        "want = Q.astype(np.float64) @ E.astype(np.float64).T\n"
-        "assert np.array_equal(i1, i2) and np.array_equal(s1, s2)\n"
-        "assert np.max(np.abs(got - want)) < 8e-6, np.max(np.abs(got - want))\n"
-        "assert i1[0, 0] == 3\n"
-        "print('2cta ok')\n")
-    env = dict(os.environ, HRAG_SIM_2CTA="1")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0 and "2cta ok" in out.stdout, out.stdout + out.stderr
-
-
 def test_knn_matches_exact_cosine_topk(hb):
     """8(f)-2: retrieve_knn drop-in (utils/embed_utils.py:6) vs float64 cosine + deterministic top-k."""
     from hipporag_b200.knn import retrieve_knn

@@ -1,5 +1,5 @@
 """CPU-only tests of host-side product code: the synthetic KG generator, the drop-in's table
-extraction (against the harness run of the reference), bench.py's bookkeeping and reference arm."""
+extraction (against the stored harness run of the reference), bench.py's bookkeeping and reference arm."""
 import json
 import os
 import subprocess
@@ -58,19 +58,33 @@ def test_roofline_byte_model():
     assert 3000 < peak < 9000 and ("measured" in src or "fallback" in src)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/src"), reason="needs the reference checkout")
 def test_dropin_table_extraction_matches_the_harness():
     """accelerate.extract_tables (product) and oracle.ref_harness.extract_tables (test infrastructure) are
-    written independently from the same reference lines; on the reference's own object they must agree."""
-    from oracle import ref_harness as H
+    written independently from the same reference lines; on the reference's own object they must agree.  The object's
+    state after index() of 120 MuSiQue passages and the harness's tables from it are stored in
+    tests/golden/dropin_tables120.npz (tests/golden/make_dropin_golden.py); the product reads a stand-in that holds
+    exactly that state."""
+    import types
+    from oracle.fake_igraph import Graph
+    from tests import fake_hipporag
     from hipporag_b200.accelerate import extract_tables
-    rag = H.build_reference_rag(tempfile.mkdtemp(prefix="hrag_tb_"), 120, 32)
-    want = H.extract_tables(rag)
+    fake_hipporag.install_stub_package()
+    g = np.load(os.path.join(ROOT, "tests", "golden", "dropin_tables120.npz"))
+    names = [str(n) for n in g["vertex_names"]]
+    graph = Graph(directed=False)
+    graph.add_vertices(len(names), attributes={"name": names})
+    graph.add_edges([tuple(e) for e in g["graph_edges"].tolist()], attributes={"weight": g["graph_weights"].tolist()})
+    keys = [str(k) for k in g["fact_node_keys"]]
+    rag = types.SimpleNamespace(
+        graph=graph, node_name_to_vertex_idx={n: i for i, n in enumerate(names)},     # HippoRAG.py:1301
+        passage_node_idxs=g["passage_node_idxs"].tolist(), fact_node_keys=keys,
+        fact_embedding_store=fake_hipporag._Store(keys, [str(c) for c in g["fact_contents"]]),
+        ent_node_to_chunk_ids={str(k): set(range(int(c))) for k, c in zip(g["ent_chunk_keys"], g["ent_chunk_counts"])})
     got = extract_tables(rag)
-    for k in ("n_nodes", "edge_src", "edge_dst", "edge_w", "passage_vid", "fact_subj_vid", "fact_obj_vid",
-              "ent_chunk_count"):
-        assert np.array_equal(np.asarray(got[k]), np.asarray(want[k])), k
-    assert [str(f) for f in got["facts"]] == want["fact_texts"]
+    assert got["n_nodes"] == int(g["want_n_nodes"])
+    for k in ("edge_src", "edge_dst", "edge_w", "passage_vid", "fact_subj_vid", "fact_obj_vid", "ent_chunk_count"):
+        assert np.array_equal(np.asarray(got[k]), g["want_" + k]), k
+    assert [str(f) for f in got["facts"]] == [str(t) for t in g["want_fact_texts"]]
     assert (got["fact_subj_vid"] >= 0).all() and (got["ent_chunk_count"][got["passage_vid"]] == 0).all()
 
 

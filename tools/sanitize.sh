@@ -1,6 +1,6 @@
 #!/bin/bash
 # compute-sanitizer passes over a small end-to-end run of every kernel family (SURVEY.md 5: race detection).
-# Usage (GPU box): bash tools/sanitize.sh [memcheck|racecheck|synccheck|initcheck]
+# Usage (on an H100): bash tools/sanitize.sh [memcheck|racecheck|synccheck|initcheck]
 set -u
 TOOL=${1:-memcheck}
 cat > /tmp/hrag_sanitize_driver.py <<'PY'
