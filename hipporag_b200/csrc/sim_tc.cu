@@ -21,7 +21,6 @@
 #include <cuda_bf16.h>
 
 #include <algorithm>
-#include <cstdlib>
 
 #include "common.cuh"
 #include "kernels.h"
@@ -135,7 +134,6 @@ struct TcParams {
     // fused epilogue (FUSE): per (query, n-tile) min/max and the 8 best rank keys instead of scores
     float2* part_mm;          // [Bq, num_n_tiles]
     uint64_t* part_keys;      // [Bq, num_n_tiles, 8]
-    int debug_mode;           // 0 = normal; 1 = TMA only (no MMAs issued); 2 = MMA only (no TMA loads) -- timing probes
     // threshold epilogue (FUSE == 2, index-time synonymy KNN): every score >= thr is appended to its query's
     // candidate list as a rank key; cand_count keeps counting past cand_cap so overflow is detectable
     float thr;
@@ -234,7 +232,6 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                 }
                 for (int kb = 0; kb < nkb; ++kb) {
                     mbar_wait(empty_bar(stage), phase ^ 1u);
-                    if (p.debug_mode == 2) { mbar_arrive(full_bar(stage)); if (++stage == STAGES) { stage = 0; phase ^= 1u; } continue; }
                     mbar_expect_tx(full_bar(stage), STAGE_BYTES);
                     const uint32_t sa = base + stage * STAGE_BYTES;
                     tma_load_2d(sa, &map_q_hi, full_bar(stage), kb * BKs, mt * BM);
@@ -266,28 +263,26 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
             const uint32_t sa = base + stage * STAGE_BYTES;
             const uint64_t a_hi = gmma_desc_kmajor<ROW_BYTES>(sa + wg * WG_A_OFF);
             const uint64_t b_hi = gmma_desc_kmajor<ROW_BYTES>(sa + OFF_B_HI);
-            if (p.debug_mode != 1) {
-                wgmma_fence();
-                if (SPLIT) {
-                    const uint64_t a_lo = gmma_desc_kmajor<ROW_BYTES>(sa + OFF_A_LO + wg * WG_A_OFF);
-                    const uint64_t b_lo = gmma_desc_kmajor<ROW_BYTES>(sa + OFF_B_LO);
-                    // smallest terms first: lo.lo, hi.lo, lo.hi, then hi.hi; +32 bytes (2 x 16-byte units) along K per step
+            wgmma_fence();
+            if (SPLIT) {
+                const uint64_t a_lo = gmma_desc_kmajor<ROW_BYTES>(sa + OFF_A_LO + wg * WG_A_OFF);
+                const uint64_t b_lo = gmma_desc_kmajor<ROW_BYTES>(sa + OFF_B_LO);
+                // smallest terms first: lo.lo, hi.lo, lo.hi, then hi.hi; +32 bytes (2 x 16-byte units) along K per step
 #pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k)
-                        wgmma_bf16(d, a_lo + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
+                for (int k = 0; k < BKs / UK; ++k)
+                    wgmma_bf16(d, a_lo + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
 #pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), 1u);
+                for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_lo + (uint64_t)(2 * k), 1u);
 #pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_lo + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), 1u);
+                for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_lo + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), 1u);
 #pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), 1u);
-                } else {
+                for (int k = 0; k < BKs / UK; ++k) wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), 1u);
+            } else {
 #pragma unroll
-                    for (int k = 0; k < BKs / UK; ++k)
-                        wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
-                }
-                wgmma_commit();
+                for (int k = 0; k < BKs / UK; ++k)
+                    wgmma_bf16(d, a_hi + (uint64_t)(2 * k), b_hi + (uint64_t)(2 * k), (kb > 0 || k > 0) ? 1u : 0u);
             }
+            wgmma_commit();
             // at most this k-block's MMAs are still in flight: the previous stage can be refilled
             wgmma_wait<1>();
             if (prev_stage >= 0 && lane == 0) mbar_arrive(empty_bar(prev_stage));
@@ -456,7 +451,6 @@ int sim_tc_threshold(const void* q_hi, const void* q_lo, int Bq, const void* e_h
     HRAG_TRY(make_map(&mel, e_lo, M, dim, bkc, BN));
     TcParams p;
     p.Bq = Bq; p.M = M; p.dim = dim; p.S = nullptr; p.ldS = 0; p.part_mm = nullptr; p.part_keys = nullptr;
-    p.debug_mode = 0;
     p.thr = thr; p.cand_keys = cand_keys; p.cand_count = cand_count; p.cand_cap = cand_cap;
     p.num_m_tiles = (int)ceil_div(Bq, BM);
     p.num_n_tiles = (int)ceil_div(M, BN);
@@ -490,15 +484,12 @@ int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const v
     TcParams p;
     p.Bq = Bq; p.M = M; p.dim = dim; p.S = S; p.ldS = ldS; p.part_mm = part_mm; p.part_keys = part_keys;
     const bool fuse = part_mm != nullptr;
-    p.debug_mode = 0;
     p.thr = 0.f; p.cand_keys = nullptr; p.cand_count = nullptr; p.cand_cap = 0;
-    if (const char* ed = getenv("HRAG_SIM_DEBUG")) p.debug_mode = atoi(ed);
     HRAG_CHECK(fuse || (S != nullptr && ldS % 4 == 0), "sim_tc: score buffer missing");
     p.num_m_tiles = (int)ceil_div(Bq, BM);
     p.num_n_tiles = (int)ceil_div(M, BN);
     const int64_t tiles = (int64_t)p.num_m_tiles * p.num_n_tiles;
-    int grid = (int)std::min<int64_t>(tiles, num_sms);
-    if (const char* eg = getenv("HRAG_SIM_GRID")) grid = std::max(1, std::min(grid, atoi(eg)));   // experiment knob
+    const int grid = (int)std::min<int64_t>(tiles, num_sms);
     if (n_seg == 4 && fuse) k_sim_tc<true, 1><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
     else if (n_seg == 4) k_sim_tc<true, 0><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
     else if (fuse) k_sim_tc<false, 1><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);

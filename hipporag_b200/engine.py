@@ -324,12 +324,6 @@ class Engine:
                                                 _ptr(scores), _ptr(found)))
         return ids, scores, found
 
-    def set_tuning(self, mixed_hint: int = -1, use_tma: int = -1, sorted_rows: int = -1, sweep_shape: int = -1,
-                   k5_debug: int = -1):
-        """Profiling switches: cache-policy variant of the fp16 sweep / TMA-gather sweep / by-length row
-        assignment / (gathers in flight, CTAs per SM)."""
-        _lib.check(self._lib.hrag_set_tuning(self._h, mixed_hint, use_tma, sorted_rows, sweep_shape, k5_debug))
-
     def bench_sweep(self, batch: int, sweeps: int = 20, method: int = PPR_POWER) -> float:
         ms = C.c_float()
         _lib.check(self._lib.hrag_bench_sweep(self._h, batch, sweeps, method, C.byref(ms)))

@@ -186,23 +186,6 @@ def test_ppr_sweep_counts_follow_damping(hb, damping, batch):
         assert np.max(np.abs(got2 - want) / scale) < RTOL
 
 
-def test_tma_gather_sweep_equals_ldg_sweep(hb):
-    """K1t (TMA gather4 into a shared-memory ring) computes the same sweep as k_sweep_h, bit for bit."""
-    from hipporag_b200 import synth
-    kg = synth.make_kg(30_000, 300_000, seed=6)
-    rng = np.random.default_rng(1)
-    R = np.zeros((33, kg.n_nodes), dtype=np.float32)
-    R[:, kg.passage_vid] = 0.05 * rng.random((33, kg.n_pass), dtype=np.float32)
-    for b in range(33):
-        R[b, rng.integers(0, kg.n_ent, 5)] = rng.random(5, dtype=np.float32)
-    e = _engine_for_graph(hb, kg.n_nodes, kg.edge_src, kg.edge_dst, kg.edge_w)
-    a = e.ppr(R)
-    e.set_tuning(use_tma=1)
-    b = e.ppr(R)
-    e.set_tuning(use_tma=0)
-    np.testing.assert_array_equal(a, b)
-
-
 def test_retrieve_musique1k_mixed_precision(hb, golden, c1):
     g = golden
     c1.engine.set_options(ppr_precision=hb.PPR_MIXED)

@@ -29,21 +29,11 @@ def main():
     e.p2p_import(handles)
     dist.barrier()
     ms_p2p = e.bench_sweep(32, 30, 2)
-    probes = []
-    for dbg in (1, 2, 3, 4):                       # timing probes (1-3: results invalid; 4: LSU stores instead of TMA bulk copies)
-        e.set_tuning(k5_debug=dbg)
-        dist.barrier()
-        probes.append(e.bench_sweep(32, 30, 2))
-    e.set_tuning(k5_debug=0)
-    t = torch.tensor([ms_nccl, ms_p2p] + probes, dtype=torch.float64)
+    t = torch.tensor([ms_nccl, ms_p2p], dtype=torch.float64)
     dist.all_reduce(t, op=dist.ReduceOp.MAX)
     if rank == 0:
         print(json.dumps({"workload": name, "gpus": world, "ms_per_sweep_nccl_allgather": round(float(t[0]), 4),
-                          "ms_per_sweep_fused_peer_stores": round(float(t[1]), 4),
-                          "probe_no_per_cta_system_fence": round(float(t[2]), 4),
-                          "probe_no_peer_stores": round(float(t[3]), 4),
-                          "probe_neither": round(float(t[4]), 4),
-                          "variant_lsu_stores_instead_of_tma_bulk": round(float(t[5]), 4)}), flush=True)
+                          "ms_per_sweep_fused_peer_stores": round(float(t[1]), 4)}), flush=True)
     dist.barrier()
     e.close()
     dist.destroy_process_group()
