@@ -134,6 +134,7 @@ struct hrag_handle {
     int mixed_m1 = 0, mixed_m2 = 0;   // 0 = derived from damping (8 / 7 at damping 0.5)
     double check_tol = 0.0, check_kappa = 0.0;   // > 0: this call's mixed solves are verified in resolve_spans
     float last_rho = 0.f;             // measured relative L1 residual of the fp16 first solve (last call)
+    bool rho_dirty = false;           // a mixed solve ran in this call: rho must be read / cleared in resolve_spans
     float last_bound = 0.f;           // a-posteriori bound on the relative L1 error of the last mixed call
 
     Buf V, XA, XC, partials, sums, S_fact, S_pass, mm_fact, mm_pass, mode;
@@ -208,21 +209,33 @@ int resolve_spans(hrag_t* h) {
         HRAG_CHECK(err == 0, "node-range sharding: a peer GPU never published its rows (fused exchange timed out); "
                              "the results of this call are invalid");
     }
-    if (h->check_tol > 0.0 && h->rho.p) {
-        // a-posteriori check of the mixed solver: rho = measured relative L1 residual of the fp16 first solve (max
-        // over every column solved in this call); the refinement round contracts it by kappa (plan_sweeps)
-        float rho = 0.f;
-        HRAG_CUDA(cudaMemcpy(&rho, h->rho.p, sizeof(float), cudaMemcpyDeviceToHost));
-        HRAG_CUDA(cudaMemset(h->rho.p, 0, sizeof(float)));
+    if ((h->rho_dirty || h->check_tol > 0.0) && h->rho.p) {
+        // every mixed solve of this call (a fresh capture or a replayed graph) raised rho[0] = the running maximum of
+        // the measured relative L1 residual of its fp16 first solve, and rho[1] if an fp16 iterate left fp16's range.
+        // Both are cleared here, checked call or not, so the next call is judged by its own solves only.
+        float rho[2] = {0.f, 0.f};
+        HRAG_CUDA(cudaMemcpy(rho, h->rho.p, sizeof(rho), cudaMemcpyDeviceToHost));
+        HRAG_CUDA(cudaMemset(h->rho.p, 0, sizeof(rho)));
+        int overflow = 0;
+        memcpy(&overflow, &rho[1], sizeof(int));
         const double tol = h->check_tol, kappa = h->check_kappa;
         h->check_tol = h->check_kappa = 0.0;
-        h->last_rho = rho;
-        h->last_bound = (float)(rho * kappa);
-        if (!(rho * kappa <= 10.0 * tol)) {
-            set_error("PPR (mixed solver): measured relative residual " + std::to_string(rho) + " x predicted contraction " +
-                      std::to_string(kappa) + " misses tol " + std::to_string(tol) +
-                      " -- pass more sweeps (iters) or use HRAG_PPR_FP32");
-            return 4;
+        h->rho_dirty = false;
+        if (overflow) {
+            set_error("PPR (mixed solver): an fp16 iterate reached 65520 in magnitude and would have been clamped, so "
+                      "the result is invalid -- pass more sweeps (iters) or use HRAG_PPR_FP32");
+            return 5;
+        }
+        if (tol > 0.0) {
+            // a-posteriori check of the mixed solver: the refinement round contracts rho by kappa (plan_sweeps)
+            h->last_rho = rho[0];
+            h->last_bound = (float)(rho[0] * kappa);
+            if (!(rho[0] * kappa <= 10.0 * tol)) {
+                set_error("PPR (mixed solver): measured relative residual " + std::to_string(rho[0]) +
+                          " x predicted contraction " + std::to_string(kappa) + " misses tol " + std::to_string(tol) +
+                          " -- pass more sweeps (iters) or use HRAG_PPR_FP32");
+                return 4;
+            }
         }
     }
     double* slots[ST_COUNT] = {&h->stats.ms_sim_fact, &h->stats.ms_select_fact, &h->stats.ms_sim_passage,
@@ -315,9 +328,9 @@ int ensure_state_mixed(hrag_t* h) {
     HRAG_TRY(h->partials.ensure((size_t)std::max(mixed_partial_rows(h->g), 1024) * 32 * sizeof(float)));
     HRAG_TRY(h->sums.ensure(192 * sizeof(double)));      // sums of x0, of d, of |r|, and of v (two sets)
     HRAG_TRY(h->mixed_aux.ensure(32 * sizeof(float)));   // column scales, set 0
-    if (h->rho.p == nullptr) {
-        HRAG_TRY(h->rho.ensure(sizeof(float)));
-        HRAG_CUDA(cudaMemset(h->rho.p, 0, sizeof(float)));
+    if (h->rho.p == nullptr) {       // [0] running max of the measured residual (float), [1] fp16 overflow flag (int)
+        HRAG_TRY(h->rho.ensure(2 * sizeof(float)));
+        HRAG_CUDA(cudaMemset(h->rho.p, 0, 2 * sizeof(float)));
     }
     return 0;
 }
@@ -414,8 +427,9 @@ int p2p_signal(hrag_t* h) {
 int mixed_sweep_x(hrag_t* h, int mode, const void* x, const int* slot_map, const void* rhs, const float* v32,
                   const float* scale, const void* prev, void* y, float alpha, float w, float t, float* part,
                   int* n_part) {
-    HRAG_TRY(mixed_sweep(h->g, mode, x, slot_map, rhs, v32, scale, prev, y, alpha, w, t, part, n_part, peers_for(h, y),
-                         sync_for_sweep(h), h->stream));
+    int* overflow = h->rho.p ? h->rho.as<int>() + 1 : nullptr;
+    HRAG_TRY(mixed_sweep(h->g, mode, x, slot_map, rhs, v32, scale, prev, y, alpha, w, t, part, n_part, overflow,
+                         peers_for(h, y), sync_for_sweep(h), h->stream));
     if (!h->p2p) HRAG_TRY(exchange_rows_bytes(h, y, 32 * 2));
     return 0;
 }
@@ -537,6 +551,7 @@ int dev_ppr_mixed_body(hrag_t* h, const SweepPlan& plan, float alpha, const int*
 int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot_map, const float* Vexact,
                   const void* rhs16, void* x0_dense, const float* scale, const double* vsum, void** X0, void** D) {
     StageTimer tm(h, ST_PPR);
+    h->rho_dirty = true;     // set here, not in the body: the body runs on the host only while a graph is captured
     if (h->world > 1) {
         HRAG_TRY(dev_ppr_mixed_body(h, plan, alpha, slot_map, Vexact, rhs16, x0_dense, scale, vsum, X0, D));
         return p2p_wait(h);     // the consumers of X0 / D (gather kernels) need every peer's last rows

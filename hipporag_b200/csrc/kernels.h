@@ -64,10 +64,11 @@ struct SweepSync {
 // mode 0: yh = w * (alpha * P xh + rhs) + (1 - w) * prevh ;  mode 1 (residual):
 // yh = t * (col_scale * v32 - xh + alpha * P xh), partials (if given) = column sums of |yh|.
 // rhs_h / v32 are [n_slots, 32] arrays addressed through slot_map[node] (-1 = zero row); slot_map == null
-// means dense [N, 32].  partials as in ppr_sweep ([rows, 32] floats).
+// means dense [N, 32].  partials as in ppr_sweep ([rows, 32] floats).  *overflow (if not null) is set to 1 when a
+// value to be stored is >= 65520 in magnitude (fp16 would round it to inf; it is clamped to 65504 instead).
 int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map, const void* rhs_h,
                 const float* v32, const float* col_scale, const void* prevh, void* yh, float alpha, float w,
-                float t, float* partials, int* n_partials, const PeerOut& peers, const SweepSync& sync,
+                float t, float* partials, int* n_partials, int* overflow, const PeerOut& peers, const SweepSync& sync,
                 cudaStream_t stream);
 int mixed_partial_rows(const PprGraph& g);
 // vsum[32] <- column sums of V32 [n_rows, 32] (>= 0; `partials` = scratch of >= 1024*32 floats);

@@ -152,7 +152,7 @@ __device__ __forceinline__ void row_epilogue_h(float (&acc)[8], int row, int lan
                                                const uint4* __restrict__ rhs_h, const float4* __restrict__ v32,
                                                const float* __restrict__ col_scale, const uint4* x0h,
                                                const uint4* prevh, uint4* yh, float alpha, float w, float t,
-                                               const PeerOut& peers, float (&out)[8], uint4& packed_out) {
+                                               const PeerOut& peers, int* overflow, float (&out)[8], uint4& packed_out) {
     const size_t o = (size_t)row * kLPR + lane;
     const int slot = slot_map ? __ldg(slot_map + row) : row;
     if (MODE == 0) {
@@ -191,6 +191,12 @@ __device__ __forceinline__ void row_epilogue_h(float (&acc)[8], int row, int lan
             out[j] = t * (fmaf(alpha, acc[j], fmaf(sc, v[j], -x0[j])));
         }
     }
+    // fp16 rounds |x| >= 65520 to inf, so sat_h would clamp such a value and change the answer: flag it (pinned small
+    // sweep counts on a concentrated seed can push the scaled residual that far; the host turns the flag into an error)
+    float mx = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) mx = fmaxf(mx, fabsf(out[j]));
+    if (mx >= 65520.f && overflow) *overflow = 1;
     const uint4 packed = f_to_h8(out);
     packed_out = packed;
     st_y(yh + o, packed);
@@ -240,6 +246,7 @@ struct SweepArgs {
     uint4* yh;
     float alpha, w, t;
     float* partials;
+    int* overflow;             // set to 1 when a stored value would leave fp16's range (null = not reported)
 };
 
 // Single-GPU sweep: one block of 64 rows per CTA.  (Kept free of the exchange code of k_sweep_h_push below: a block
@@ -260,7 +267,7 @@ k_sweep_h(const SweepArgs a) {
             uint4 packed;
             group_row_dot_h(a.cv, s, e, a.xh + l, acc);
             row_epilogue_h<CHEB, MODE>(acc, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh, a.prevh,
-                                       a.yh, a.alpha, a.w, a.t, PeerOut(), out, packed);
+                                       a.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out, packed);
         }
     }
     if (FINAL) block_colsum_h(out, a.partials + (size_t)blockIdx.x * kB);
@@ -303,7 +310,7 @@ k_sweep_h_push(const SweepArgs a, const PeerOut peers, const SweepSync sy) {
                 uint4 packed;
                 group_row_dot_h(a.cv, s, e, a.xh + l, acc);
                 row_epilogue_h<CHEB, MODE>(acc, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh,
-                                           a.prevh, a.yh, a.alpha, a.w, a.t, PeerOut(), out, packed);
+                                           a.prevh, a.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out, packed);
                 if (push) {
                     const int rl = r - blk * kGPB;       // row_order permutes rows inside their own 64-row block only
                     s_out[buf][rl * kLPR + l] = packed;
@@ -390,7 +397,7 @@ k_sweep_long_finalize_h(int n_long, const int* __restrict__ long_rows, const int
             for (int j = 0; j < 8; ++j) acc[j] += seg_partial[(size_t)s * kB + l * 8 + j];
         uint4 packed;
         row_epilogue_h<CHEB, MODE>(acc, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh, a.prevh,
-                                   a.yh, a.alpha, a.w, a.t, peers, out, packed);
+                                   a.yh, a.alpha, a.w, a.t, peers, a.overflow, out, packed);
     }
     if (FINAL) block_colsum_h(out, a.partials + (size_t)blockIdx.x * kB);
     sync_signal(sy);
@@ -635,7 +642,7 @@ int epoch_signal(const SweepSync& sync, cudaStream_t st) {
 // One fp16 sweep (mode 0) or the residual sweep (mode 1) over the owned rows.
 int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map, const void* rhs_h, const float* v32,
                 const float* col_scale, const void* prevh, void* yh, float alpha, float w, float t, float* partials,
-                int* n_partials, const PeerOut& peers, const SweepSync& sync, cudaStream_t st) {
+                int* n_partials, int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t st) {
     HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep: graph not loaded");
     const bool cheb = prevh != nullptr, fin = partials != nullptr;
     const int nb_rows = (int)ceil_div(g.n_rows, kGPB);
@@ -653,6 +660,7 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
     a.yh = reinterpret_cast<uint4*>(yh);
     a.alpha = alpha; a.w = w; a.t = t;
     a.partials = partials;
+    a.overflow = overflow;
     SweepSync sy = sync;
     // sharded (fused exchange): a persistent grid of 6 CTAs per SM, so each CTA pays one system-scope fence per sweep
     // and the epoch is published by the last CTA of the sweep itself, with no extra launch (see k_sweep_h_push).  The
