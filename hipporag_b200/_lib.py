@@ -48,6 +48,7 @@ SIGNATURES = {
     "hrag_p2p_export": (C.c_int, [_p, _p]),
     "hrag_p2p_import": (C.c_int, [_p, _p, C.c_int]),
     "hrag_load_graph_csr": (C.c_int, [_p, _i64, _i64, _i64, _i64, _p, _p, _p]),
+    "hrag_load_graph_csr_f64": (C.c_int, [_p, _i64, _i64, _i64, _i64, _p, _p, _p]),
     "hrag_load_graph_coo": (C.c_int, [_p, _i64, _i64, _p, _p, _p]),
     "hrag_load_tables": (C.c_int, [_p, _i64, _p, _i64, _p, _p, _p]),
     "hrag_load_embeddings": (C.c_int, [_p, C.c_int, _i64, _i32, _p, C.c_int]),
@@ -60,6 +61,7 @@ SIGNATURES = {
     "hrag_plan_sweeps": (C.c_int, [_f32, _f32, _i32, _i32, _p, _p, _p, _p, _p]),
     "hrag_retrieve_resident": (C.c_int, [_p, _i32, _p, _p, _f32, _f32, _i32, _i32, _i32, _f32, _p, _p]),
     "hrag_ppr": (C.c_int, [_p, _i32, _p, _f32, _i32, _f32, _p]),
+    "hrag_ppr_f64": (C.c_int, [_p, _i32, _p, C.c_double, C.c_double, _p]),
     "hrag_similarity": (C.c_int, [_p, C.c_int, _i32, _p, _p]),
     "hrag_topk_similarity": (C.c_int, [_p, C.c_int, _i32, _p, _i32, _p, _p]),
     "hrag_knn_threshold": (C.c_int, [_p, C.c_int, _i32, _p, _f32, _i32, _p, _p, _p]),

@@ -16,7 +16,8 @@ What is rebound (all paths under the reference's ``src/hipporag/``):
   stage B for all queries; timers ``ppr_time`` / ``rerank_time`` / ``all_retrieval_time`` and the
   optional Recall@k evaluation behave as in the reference;
 * ``run_ppr`` (``:1709-1749``), ``dense_passage_retrieval`` (``:1467-1502``), ``get_fact_scores``
-  (``:1427-1465``) -- single-call forms for code that uses them directly;
+  (``:1427-1465``) -- single-call forms for code that uses them directly; ``run_ppr`` in float64 to PRPACK's
+  1e-10 with ``run_ppr_fp64=True``;
 * ``index`` / ``delete`` (``:262``, ``:337``) -- additionally invalidate the device state
   (``index`` forgets to clear ``ready_to_retrieve`` in the reference);
 * ``add_synonymy_edges`` (``:959-1020``) -- runs unchanged, but the ``retrieve_knn`` it calls
@@ -72,7 +73,8 @@ def extract_tables(rag) -> dict:
 
 
 def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_workers: int = 1,
-               filter_chunk: int = 256, ppr_tol: float = 0.0, cache: bool = True, **engine_opts):
+               filter_chunk: int = 256, ppr_tol: float = 0.0, cache: bool = True, run_ppr_fp64: bool = False,
+               **engine_opts):
     """Rebinds the hot-path methods of ``rag`` (a reference ``HippoRAG`` instance) in place.
 
     ``filter_workers > 1`` (SURVEY.md 8(f)-1) runs the per-query recognition-memory filter calls (LLM HTTP
@@ -83,6 +85,10 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     of every PPR vector (0 = the library default 1e-6; PRPACK's own target is 1e-10 in float64).
     ``cache`` (SURVEY.md 8(f)-3): keep the CSR of P and the integer tables as ``b200_index_cache.npz/.json`` next to
     the reference's ``graph.pickle`` and reuse them while the index fingerprint is unchanged (``hipporag_b200/cache.py``).
+    ``run_ppr_fp64=True`` serves ``run_ppr`` (and so the reference's own ``graph_search_with_fact_entities``, which
+    calls it) at PRPACK's accuracy: the float64 P is uploaded, and every call solves in float64 to ``ppr_tol``
+    (0 = 1e-10) and returns float64 scores (``Engine.ppr_f64``).  ``retrieve`` is unaffected: its reset vectors come
+    from fp32 similarity scores.
     ``engine_opts`` go to ``Engine.set_options``.
     """
     from hipporag.utils.misc_utils import QuerySolution
@@ -111,11 +117,15 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         tb = fp = None
         if wd:
             fp = _cache.fingerprint(self)
-            tb = _cache.load(wd, fp)
+            tb = _cache.load(wd, fp, fp64=True) if run_ppr_fp64 else _cache.load(wd, fp)
         state["cache_hit"] = tb is not None
         if tb is None:
             tb = extract_tables(self)
-            csr = build_transition_csr(tb["n_nodes"], tb["edge_src"], tb["edge_dst"], tb["edge_w"])
+            if run_ppr_fp64:
+                csr = build_transition_csr(tb["n_nodes"], tb["edge_src"], tb["edge_dst"], tb["edge_w"],
+                                           dtype=np.float64)
+            else:
+                csr = build_transition_csr(tb["n_nodes"], tb["edge_src"], tb["edge_dst"], tb["edge_w"])
             tb["row_ptr"], tb["col"], tb["val"] = csr
             if wd:
                 try:
@@ -328,7 +338,10 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         if damping is None:
             damping = 0.5
         _ensure_ready(self)
-        pi = _engine().ppr(np.asarray(reset_prob, dtype=np.float32), damping, tol=ppr_tol)
+        if run_ppr_fp64:
+            pi = _engine().ppr_f64(np.asarray(reset_prob, dtype=np.float64), damping, tol=ppr_tol)
+        else:
+            pi = _engine().ppr(np.asarray(reset_prob, dtype=np.float32), damping, tol=ppr_tol)
         doc_scores = pi[np.asarray(self.passage_node_idxs, dtype=np.int64)].astype(np.float64)
         order = np.lexsort((np.arange(doc_scores.shape[0]), -doc_scores))
         return order, doc_scores[order]

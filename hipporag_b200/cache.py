@@ -7,7 +7,9 @@ of that is ``accelerate.extract_tables``: one ``eval`` + two md5 lookups per fac
 O(F + E) Python.  This module stores its result next to ``graph.pickle``:
 
     <working_dir>/b200_index_cache.npz    CSR of P = W D^-1 (row_ptr int64, col int32, val float32), the integer
-                                          tables (passage_vid, fact_subj_vid, fact_obj_vid, ent_chunk_count)
+                                          tables (passage_vid, fact_subj_vid, fact_obj_vid, ent_chunk_count);
+                                          with a float64 P also val_lo float32 = P - val (val + val_lo = P to
+                                          ~2^-48 relative, the operator of ``accelerate(run_ppr_fp64=True)``)
     <working_dir>/b200_index_cache.json   fingerprint + the fact triples (the filter needs them as Python tuples)
 
 keyed by a fingerprint of the index (vertex / edge / fact / passage counts, md5 of the vertex names, fact keys and
@@ -60,15 +62,20 @@ def fingerprint(rag) -> dict:
 
 
 def save(working_dir: str, fp: dict, tables: dict, csr) -> None:
-    """tables = accelerate.extract_tables(rag); csr = (row_ptr, col, val) of P."""
+    """tables = accelerate.extract_tables(rag); csr = (row_ptr, col, val) of P.  A float64 ``val`` is stored as
+    the float32 ``val`` plus ``val_lo``, so a float64 load (``load(..., fp64=True)``) gets P back to ~2^-48."""
     os.makedirs(working_dir, exist_ok=True)
     row_ptr, col, val = csr
+    extra = {}
+    if np.asarray(val).dtype == np.float64:
+        hi = np.asarray(val, np.float32)
+        extra["val_lo"] = (np.asarray(val, np.float64) - hi.astype(np.float64)).astype(np.float32)
     tmp = os.path.join(working_dir, NPZ_NAME + ".tmp.npz")
     np.savez(tmp, row_ptr=np.asarray(row_ptr, np.int64), col=np.asarray(col, np.int32), val=np.asarray(val, np.float32),
              passage_vid=np.asarray(tables["passage_vid"], np.int32),
              fact_subj_vid=np.asarray(tables["fact_subj_vid"], np.int32),
              fact_obj_vid=np.asarray(tables["fact_obj_vid"], np.int32),
-             ent_chunk_count=np.asarray(tables["ent_chunk_count"], np.int32))
+             ent_chunk_count=np.asarray(tables["ent_chunk_count"], np.int32), **extra)
     os.replace(tmp, os.path.join(working_dir, NPZ_NAME))
     meta = {"fingerprint": fp, "facts": [list(f) for f in tables["facts"]]}
     tmpj = os.path.join(working_dir, META_NAME + ".tmp")
@@ -77,8 +84,9 @@ def save(working_dir: str, fp: dict, tables: dict, csr) -> None:
     os.replace(tmpj, os.path.join(working_dir, META_NAME))
 
 
-def load(working_dir: str, fp: dict) -> Optional[dict]:
-    """The cached arrays if they were derived from exactly this index state, else None."""
+def load(working_dir: str, fp: dict, fp64: bool = False) -> Optional[dict]:
+    """The cached arrays if they were derived from exactly this index state, else None.  ``fp64``: ``val`` comes
+    back as float64 ``val + val_lo``, and a cache without ``val_lo`` (written in the default mode) is a miss."""
     npz, meta = os.path.join(working_dir, NPZ_NAME), os.path.join(working_dir, META_NAME)
     if not (os.path.exists(npz) and os.path.exists(meta)):
         return None
@@ -90,6 +98,10 @@ def load(working_dir: str, fp: dict) -> Optional[dict]:
         z = np.load(npz)
         out = {k: z[k] for k in ("row_ptr", "col", "val", "passage_vid", "fact_subj_vid", "fact_obj_vid",
                                  "ent_chunk_count")}
+        if fp64:
+            if "val_lo" not in z.files:
+                return None
+            out["val"] = out["val"].astype(np.float64) + z["val_lo"].astype(np.float64)
     except Exception:
         return None
     if out["row_ptr"].shape[0] != fp["n_nodes"] + 1 or out["fact_subj_vid"].shape[0] != fp["n_facts"]:

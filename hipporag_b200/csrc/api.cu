@@ -4,6 +4,7 @@
 //
 // HBM layout per handle (N nodes, P passages, F facts, d dims; DESIGN.md section 3):
 //   graph     row_ptr int32[n_rows+1], cv int2[nnz] {col, fp32 bits of P[i,j]}, row_order int32[n_rows]   (resident)
+//             + val_lo fp32[nnz] = fp32(P64 - hi) when loaded from float64 values (the fp64 solver's operator)
 //   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N], slot_map[2][N] (node -> rhs slot)       (resident)
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
 //   state     mixed solver: H0..H3, H0b [N, 32] fp16 in one IPC-exportable slab; fp32 solver: V, XA, XC [N, B] fp32
@@ -133,14 +134,18 @@ struct hrag_handle {
     int ppr_precision = HRAG_PPR_MIXED;   // applies to batches of > 16 queries; smaller ones run fp32
     int mixed_m1 = 0, mixed_m2 = 0;   // 0 = derived from damping (8 / 7 at damping 0.5)
     double check_tol = 0.0, check_kappa = 0.0;   // > 0: this call's mixed solves are verified in resolve_spans
-    float last_rho = 0.f;             // measured relative L1 residual of the fp16 first solve (last call)
+    double last_rho = 0.0;            // measured relative L1 residual: of the fp16 first solve (last mixed call), of
+                                      // the final refinement round (last hrag_ppr_f64 call)
     bool rho_dirty = false;           // a mixed solve ran in this call: rho must be read / cleared in resolve_spans
-    float last_bound = 0.f;           // a-posteriori bound on the relative L1 error of the last mixed call
+    double last_bound = 0.0;          // a-posteriori bound on the relative L1 error of the last mixed / fp64 call
 
     Buf V, XA, XC, partials, sums, S_fact, S_pass, mm_fact, mm_pass, mode;
     Buf d_q, d_q2, d_top_idx, d_top_score, d_nvalid, d_kept_idx, d_kept_score, d_dpr, d_out_ids, d_out_scores;
     Buf d_reset, d_scores, q_hi, q_lo, seed_vid, seed_w, H[4], mixed_aux, part_mm, part_keys;
     Buf xr_mm, xr_keys;             // fact-sharded stage A: [world, Bq] min/max and [world, Bq, 8] best keys
+    // fp64 solver (hrag_ppr_f64): iterate X64 and reset V64 [N, B] fp64, host-layout staging io64 [B, N] fp64 (reset
+    // in, probabilities out), column-sum partials part64, sums64 = [vsum | rsum | xsum] x 16
+    Buf X64, V64, io64, part64, sums64;
     // mixed solver, double-buffered per-sub-batch inputs (set s: x0 = H[0] / H0b, scales mixed_aux / mixed_aux1,
     // compact rhs Vc[s] / R16[s] addressed through slot_map[s]): stream2 prepares sub-batch i+1 while `stream`
     // sweeps sub-batch i
@@ -901,10 +906,12 @@ void hrag_destroy(hrag_t* h) {
                          &h->d_reset, &h->d_scores, &h->q_hi, &h->q_lo, &h->seed_vid, &h->seed_w, &h->H[0], &h->H[1],
                          &h->H[2], &h->H[3], &h->mixed_aux, &h->part_mm, &h->part_keys, &h->H0b,
                          &h->mixed_aux1, &h->prep_scratch, &h->slot_map[0], &h->slot_map[1], &h->slot_vid[0],
-                         &h->slot_vid[1], &h->Vc[0], &h->Vc[1], &h->R16[0], &h->R16[1], &h->rho, &h->xr_mm, &h->xr_keys})
+                         &h->slot_vid[1], &h->Vc[0], &h->Vc[1], &h->R16[0], &h->R16[1], &h->rho, &h->xr_mm, &h->xr_keys,
+                         &h->X64, &h->V64, &h->io64, &h->part64, &h->sums64})
         b->release();
     cudaFree(h->g.row_ptr); cudaFree(h->g.cv); cudaFree(h->g.long_rows); cudaFree(h->g.long_seg_ptr);
     cudaFree(h->g.segs); cudaFree(h->g.seg_partial); cudaFree(h->g.row_order);
+    cudaFree(h->g.val_lo); cudaFree(h->g.seg_partial64);
     cudaFree(h->t.passage_vid); cudaFree(h->t.fact_subj_vid); cudaFree(h->t.fact_obj_vid);
     cudaFree(h->t.ent_chunk_count);
     for (int i = 0; i < 2; ++i) {
@@ -983,18 +990,21 @@ int hrag_p2p_import(hrag_t* h, const void* handles, int world) {
     return 0;
 }
 
-int hrag_load_graph_csr(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, int64_t nnz,
-                        const int64_t* row_ptr, const int32_t* col, const float* val) {
-    HRAG_CHECK(h && row_ptr && (nnz == 0 || (col && val)), "hrag_load_graph_csr: null argument");
-    HRAG_CHECK(n_nodes > 0 && n_nodes < (int64_t)1 << 30, "hrag_load_graph_csr: n_nodes out of range");
-    HRAG_CHECK(nnz >= 0 && nnz < ((int64_t)1 << 31) - 8, "hrag_load_graph_csr: nnz must fit int32");
-    HRAG_CHECK(0 <= row_lo && row_lo <= row_hi && row_hi <= n_nodes, "hrag_load_graph_csr: bad row range");
+// The two CSR entries share this: exactly one of val (fp32) / val64 is given.  From val64 the fp32 plane cv stores
+// fp32(val64) -- bitwise what the fp32 entry stores for that rounding -- and the lo plane fp32(val64 - hi).
+static int load_graph_csr_impl(hrag_t* h, const std::string& who, int64_t n_nodes, int64_t row_lo, int64_t row_hi,
+                               int64_t nnz, const int64_t* row_ptr, const int32_t* col, const float* val,
+                               const double* val64) {
+    HRAG_CHECK(h && row_ptr && (nnz == 0 || (col && (val || val64))), who + ": null argument");
+    HRAG_CHECK(n_nodes > 0 && n_nodes < (int64_t)1 << 30, who + ": n_nodes out of range");
+    HRAG_CHECK(nnz >= 0 && nnz < ((int64_t)1 << 31) - 8, who + ": nnz must fit int32");
+    HRAG_CHECK(0 <= row_lo && row_lo <= row_hi && row_hi <= n_nodes, who + ": bad row range");
     HRAG_CUDA(cudaSetDevice(h->device));
     const int n_rows = (int)(row_hi - row_lo);
-    HRAG_CHECK(row_ptr[0] == 0 && row_ptr[n_rows] == nnz, "hrag_load_graph_csr: row_ptr does not span nnz");
+    HRAG_CHECK(row_ptr[0] == 0 && row_ptr[n_rows] == nnz, who + ": row_ptr does not span nnz");
     PprGraph& g = h->g;
     cudaFree(g.row_ptr); cudaFree(g.cv); cudaFree(g.long_rows); cudaFree(g.long_seg_ptr); cudaFree(g.segs);
-    cudaFree(g.seg_partial); cudaFree(g.row_order);
+    cudaFree(g.seg_partial); cudaFree(g.row_order); cudaFree(g.val_lo); cudaFree(g.seg_partial64);
     g = PprGraph();
     g.num_sms = h->num_sms;
     g.n_global = (int)n_nodes;
@@ -1006,21 +1016,22 @@ int hrag_load_graph_csr(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_
     h->chunk_rows = h->world > 1 ? ceil_div(n_nodes, h->world) : n_nodes;
     if (h->world > 1) {
         HRAG_CHECK(h->row_bounds.empty() || h->row_bounds.back() == n_nodes,
-                   "hrag_load_graph_csr: hrag_comm_set_row_bounds was given bounds for a different vertex count");
+                   who + ": hrag_comm_set_row_bounds was given bounds for a different vertex count");
         int64_t lo = 0, hi = 0;
         owned_rows(h, n_nodes, &lo, &hi);
         HRAG_CHECK(row_lo == lo && row_hi == hi,
-                   "hrag_load_graph_csr: sharded ranks own rows [rank*ceil(N/world), (rank+1)*ceil(N/world)), or the range "
+                   who + ": sharded ranks own rows [rank*ceil(N/world), (rank+1)*ceil(N/world)), or the range "
                    "given by hrag_comm_set_row_bounds");
     }
     std::vector<int> rp(n_rows + 1);
     std::vector<int2> cv((size_t)nnz);
+    std::vector<float> lo(val64 ? (size_t)nnz : 0);
     std::vector<int> long_rows, long_seg_ptr;
     std::vector<int4> segs;
     const int seg_len = 256;
     for (int r = 0; r < n_rows; ++r) {
         const int64_t s = row_ptr[r], e = row_ptr[r + 1];
-        HRAG_CHECK(s <= e && e <= nnz, "hrag_load_graph_csr: row_ptr not monotone");
+        HRAG_CHECK(s <= e && e <= nnz, who + ": row_ptr not monotone");
         rp[r] = (int)s;
         if (e - s > g.long_thresh) {
             long_rows.push_back(r);
@@ -1032,15 +1043,21 @@ int hrag_load_graph_csr(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_
     rp[n_rows] = (int)nnz;
     long_seg_ptr.push_back((int)segs.size());
     for (int64_t i = 0; i < nnz; ++i) {
-        HRAG_CHECK(col[i] >= 0 && col[i] < n_nodes, "hrag_load_graph_csr: column index out of range");
+        HRAG_CHECK(col[i] >= 0 && col[i] < n_nodes, who + ": column index out of range");
+        const float hi = val64 ? (float)val64[i] : val[i];
         int bits;
-        memcpy(&bits, &val[i], 4);
+        memcpy(&bits, &hi, 4);
         cv[(size_t)i] = make_int2(col[i], bits);
+        if (val64) lo[(size_t)i] = (float)(val64[i] - (double)hi);
     }
     HRAG_CUDA(cudaMalloc(&g.row_ptr, (size_t)(n_rows + 1) * sizeof(int)));
     HRAG_CUDA(cudaMalloc(&g.cv, std::max<size_t>(1, (size_t)nnz) * sizeof(int2)));   // non-null: marks a loaded graph
     HRAG_CUDA(cudaMemcpy(g.row_ptr, rp.data(), (size_t)(n_rows + 1) * sizeof(int), cudaMemcpyHostToDevice));
     if (nnz) HRAG_CUDA(cudaMemcpy(g.cv, cv.data(), (size_t)nnz * sizeof(int2), cudaMemcpyHostToDevice));
+    if (val64) {   // non-null even when empty: marks an fp64 operator
+        HRAG_CUDA(cudaMalloc(&g.val_lo, std::max<size_t>(1, (size_t)nnz) * sizeof(float)));
+        if (nnz) HRAG_CUDA(cudaMemcpy(g.val_lo, lo.data(), (size_t)nnz * sizeof(float), cudaMemcpyHostToDevice));
+    }
     {   // fp16 sweep: within each block of 64 rows (one CTA) order the rows by length so a warp's 8 rows match
         std::vector<int> order(n_rows);
         for (int r = 0; r < n_rows; ++r) order[r] = r;
@@ -1063,11 +1080,22 @@ int hrag_load_graph_csr(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_
         HRAG_CUDA(cudaMemcpy(g.long_seg_ptr, long_seg_ptr.data(), long_seg_ptr.size() * sizeof(int),
                              cudaMemcpyHostToDevice));
         HRAG_CUDA(cudaMemcpy(g.segs, segs.data(), segs.size() * sizeof(int4), cudaMemcpyHostToDevice));
+        if (val64) HRAG_CUDA(cudaMalloc(&g.seg_partial64, segs.size() * 16 * sizeof(double)));
     }
     h->V.release(); h->XA.release(); h->XC.release(); h->partials.release();
     h->slot_maps_valid = false;
     h->graph_generation += 1;
     return 0;
+}
+
+int hrag_load_graph_csr(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, int64_t nnz,
+                        const int64_t* row_ptr, const int32_t* col, const float* val) {
+    return load_graph_csr_impl(h, "hrag_load_graph_csr", n_nodes, row_lo, row_hi, nnz, row_ptr, col, val, nullptr);
+}
+
+int hrag_load_graph_csr_f64(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, int64_t nnz,
+                            const int64_t* row_ptr, const int32_t* col, const double* val) {
+    return load_graph_csr_impl(h, "hrag_load_graph_csr_f64", n_nodes, row_lo, row_hi, nnz, row_ptr, col, nullptr, val);
 }
 
 int hrag_load_graph_coo(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32_t* src, const int32_t* dst,
@@ -1105,8 +1133,8 @@ int hrag_load_graph_coo(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32
     std::vector<double> strength((size_t)n_nodes, 0.0);    // W is symmetric: column sums = row sums
     for (int64_t r = 0; r < n_nodes; ++r)
         for (int64_t k = row_ptr[(size_t)r]; k < row_ptr[(size_t)r + 1]; ++k) strength[(size_t)r] += wsum[(size_t)k];
-    std::vector<float> val(col.size());
-    for (size_t k = 0; k < col.size(); ++k) val[k] = (float)(wsum[k] / strength[(size_t)col[k]]);
+    std::vector<double> val(col.size());
+    for (size_t k = 0; k < col.size(); ++k) val[k] = wsum[k] / strength[(size_t)col[k]];
     int64_t lo = 0, hi = n_nodes;
     if (h->world > 1) {
         // every rank sees the whole edge list here, so all of them derive the same work-balanced partition
@@ -1116,7 +1144,9 @@ int hrag_load_graph_coo(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32
     const int64_t a = row_ptr[(size_t)lo], b = row_ptr[(size_t)hi];
     std::vector<int64_t> rp((size_t)(hi - lo) + 1);
     for (int64_t r = lo; r <= hi; ++r) rp[(size_t)(r - lo)] = row_ptr[(size_t)r] - a;
-    return hrag_load_graph_csr(h, n_nodes, lo, hi, b - a, rp.data(), col.data() + a, val.data() + a);
+    // fp64 values: the same fp32 plane as before, plus the lo plane hrag_ppr_f64 needs
+    return load_graph_csr_impl(h, "hrag_load_graph_csr", n_nodes, lo, hi, b - a, rp.data(), col.data() + a, nullptr,
+                               val.data() + a);
 }
 
 static int upload_i32(int** dst, const int32_t* src, int64_t n) {
@@ -1422,6 +1452,106 @@ int hrag_ppr(hrag_t* h, int32_t B, const float* reset, float damping, int32_t it
         HRAG_CUDA(cudaStreamSynchronize(h->stream));
     }
     return resolve_spans(h);
+}
+
+// Float64 PPR by iterative refinement (DESIGN.md section 2): per sub-batch of <= 16 columns, x = 0, r = v; every
+// round solves (I - aP32) d = fp32(r) with the fp32 solver, x += d in fp64, and recomputes r = v - x + a(hi + lo)x
+// in fp64.  P is column-substochastic, so ||(I - aP)^-1||_1 <= 1 / (1 - a), and ||x||_1 >= ||v||_1; normalising at
+// most doubles the error, hence the rigorous bound ||pi - pi_hat||_1 <= 2 ||r||_1 / ((1 - a) ||v||_1) per column.
+constexpr double kF64DefaultTol = 1e-10;   // PRPACK's target (HippoRAG.py:1736-1743)
+constexpr double kF64MinTol = 1e-13;       // above the fp64 floor of the bound (~1e-14 at damping 0.5)
+constexpr int kF64MaxRounds = 4;
+
+int hrag_ppr_f64(hrag_t* h, int32_t B, const double* reset, double damping, double tol, double* out) {
+    HRAG_CHECK(h && reset && out, "hrag_ppr_f64: null argument");
+    HRAG_CHECK(B >= 0 && damping > 0.0 && damping < 1.0, "hrag_ppr_f64: bad arguments");
+    HRAG_CHECK(tol == 0.0 || tol >= kF64MinTol,
+               "hrag_ppr_f64: tol must be 0 (= 1e-10) or >= 1e-13; a smaller bound is below what the fp64 residual "
+               "can certify");
+    HRAG_CHECK(h->g.n_global > 0, "hrag_ppr_f64: graph not loaded");
+    HRAG_CHECK(h->world == 1, "hrag_ppr_f64: not available on a node-range-sharded handle (world > 1); solve on a "
+                              "handle that holds the whole graph");
+    HRAG_CHECK(h->g.val_lo != nullptr, "hrag_ppr_f64: the graph was loaded from fp32 values and has no fp64 operator; "
+                                       "load it with hrag_load_graph_csr_f64 or hrag_load_graph_coo");
+    HRAG_CUDA(cudaSetDevice(h->device));
+    const double target = tol > 0.0 ? tol : kF64DefaultTol;
+    const int N = h->g.n_global;
+    // the fp32 solves run at fp32(damping); the fp64 residual uses damping itself, so the refinement converges to
+    // the solution at the damping asked (float32(0.85) alone moves pi by ~1e-7)
+    const float damping32 = (float)damping;
+    const SweepPlan plan = plan_sweeps(h, damping32, 0, (float)kDefaultTol, false);   // fp32 solver at its own tol
+    const int Bp = round_batch(std::min(16, std::max(B, 1)));
+    const size_t cells = (size_t)N * Bp;
+    HRAG_TRY(ensure_state(h, Bp));
+    HRAG_TRY(h->X64.ensure(cells * sizeof(double)));
+    HRAG_TRY(h->V64.ensure(cells * sizeof(double)));
+    HRAG_TRY(h->io64.ensure(cells * sizeof(double)));
+    const int64_t rows_resid = resid_f64_partial_rows(h->g, Bp);
+    const int64_t part_rows = std::max<int64_t>(2 * rows_resid, ceil_div((int64_t)cells, 256));
+    HRAG_TRY(h->part64.ensure((size_t)part_rows * Bp * sizeof(double)));
+    HRAG_TRY(h->sums64.ensure(48 * sizeof(double)));
+    double* X = h->X64.as<double>();
+    double* V = h->V64.as<double>();
+    double* part_r = h->part64.as<double>();
+    double* part_x = part_r + (size_t)rows_resid * Bp;
+    double* vsum = h->sums64.as<double>();
+    double* rsum = vsum + 16;
+    double* xsum = vsum + 32;
+    const double a = damping;
+    double call_resid = 0.0, call_bound = 0.0;
+    for (int q0 = 0; q0 < B; q0 += Bp) {
+        const int nb = std::min(Bp, B - q0);
+        int n_part = 0;
+        HRAG_TRY(h2d(h, h->io64.p, reset + (size_t)q0 * N, (size_t)nb * N * sizeof(double)));
+        HRAG_TRY(reset_to_state_f64(h->io64.as<double>(), nb, N, Bp, V, h->V.as<float>(), X, part_r, &n_part, h->stream));
+        HRAG_TRY(colsum_reduce_f64(part_r, n_part, Bp, vsum, h->stream));
+        // every column refines until its own bound meets the target and then keeps its iterate: a query's result
+        // does not depend on the queries it shares the sub-batch with
+        unsigned active = (1u << nb) - 1u;
+        double resid = 0.0, bound = 0.0;
+        for (int round = 0; round < kF64MaxRounds && active; ++round) {
+            float* D = nullptr;
+            HRAG_TRY(dev_ppr(h, Bp, plan.iters, damping32, &D));    // (I - aP32) d = fp32(r), r = h->V
+            {
+                StageTimer tm(h, ST_PPR);
+                HRAG_TRY(add_correction_f64(X, D, (int64_t)cells, Bp, active, h->stream));
+                HRAG_TRY(resid_sweep_f64(h->g, Bp, X, V, h->V.as<float>(), a, part_r, part_x, &n_part, h->stream));
+                HRAG_TRY(colsum_reduce_f64(part_r, n_part, Bp, rsum, h->stream));
+                HRAG_TRY(colsum_reduce_f64(part_x, n_part, Bp, xsum, h->stream));
+            }
+            h->stats.ppr_sweeps += 1;
+            h->stats.ppr_columns += Bp;
+            double s[32];
+            HRAG_CUDA(cudaMemcpyAsync(s, vsum, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+            HRAG_CUDA(cudaStreamSynchronize(h->stream));
+            resid = 0.0;
+            for (int b = 0; b < nb; ++b) {
+                const double rel = s[b] > 0.0 ? s[16 + b] / s[b] : 0.0;   // a reset without mass has nothing to bound
+                resid = std::max(resid, rel);
+                if (2.0 * rel / (1.0 - a) <= target) active &= ~(1u << b);
+            }
+            bound = 2.0 * resid / (1.0 - a);
+        }
+        call_resid = std::max(call_resid, resid);
+        call_bound = std::max(call_bound, bound);
+        if (active) {
+            HRAG_TRY(resolve_spans(h));
+            h->last_rho = call_resid;
+            h->last_bound = call_bound;
+            char msg[160];
+            snprintf(msg, sizeof(msg), "hrag_ppr_f64: after %d refinement rounds the error bound is %.3e, above tol %.3e",
+                     kF64MaxRounds, bound, target);
+            set_error(msg);
+            return 4;
+        }
+        HRAG_TRY(state_to_scores_f64(X, nb, N, Bp, xsum, h->io64.as<double>(), h->stream));
+        HRAG_TRY(d2h(h, out + (size_t)q0 * N, h->io64.p, (size_t)nb * N * sizeof(double)));
+        HRAG_CUDA(cudaStreamSynchronize(h->stream));
+    }
+    HRAG_TRY(resolve_spans(h));
+    h->last_rho = call_resid;
+    h->last_bound = call_bound;
+    return 0;
 }
 
 int hrag_similarity(hrag_t* h, int which, int32_t B, const float* q, float* out) {

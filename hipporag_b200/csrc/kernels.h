@@ -28,6 +28,9 @@ struct PprGraph {
     int max_batch = 0;
     int num_sms = 132;
     int* row_order = nullptr;     // [n_rows] fp16 sweep: rows of each 64-row CTA block sorted by length (desc)
+    // fp64 operator (graphs loaded from float64 values only; null otherwise): P = hi + lo to ~2^-48 relative
+    float* val_lo = nullptr;        // [nnz] fp32(P64 - hi), hi = the fp32 value in cv
+    double* seg_partial64 = nullptr; // [n_seg * 16] fp64 segment partials of the residual sweep
 };
 
 // One sweep  y[i,:] = w * (alpha * sum_j P[i,j] x[j,:] + v[i,:]) + (1 - w) * prev[i,:]
@@ -102,6 +105,22 @@ int state_to_scores_mixed(const void* X0, const void* D, float inv_t, int nb, in
 
 // sums[b] = sum over rows of partials[r, b], accumulated in fp64.
 int colsum_reduce(const float* partials, int n_partials, int B, double* sums, cudaStream_t stream);
+
+// ---- fp64 PPR by iterative refinement (ppr_f64.cu): fp64 state [N, B], B in {4, 8, 16} ---------
+// r = v - x + alpha (hi + lo) x in fp64; writes r32 = fp32(r) [N, B] and per-CTA column sums of |r| / of x into
+// part_r / part_x ([*n_partials, B] doubles each).  Needs g.val_lo.
+int resid_sweep_f64(const PprGraph& g, int B, const double* x, const double* v, float* r32, double alpha,
+                    double* part_r, double* part_x, int* n_partials, cudaStream_t stream);
+int resid_f64_partial_rows(const PprGraph& g, int B);  // rows of part_r / part_x a residual sweep writes
+// V[n, b] = sanitised R[b, n] (host layout [nb, N] -> [N, B], NaN / negative -> 0; columns >= nb zero), V32 = fp32(V),
+// X = 0; per-CTA column sums of V -> part_v ([*n_partials, B]).
+int reset_to_state_f64(const double* R, int nb, int N, int B, double* V, float* V32, double* X, double* part_v,
+                       int* n_partials, cudaStream_t stream);
+// X [n / B, B] += D on the columns b with bit b of `active` set
+int add_correction_f64(double* X, const float* D, int64_t n, int B, unsigned active, cudaStream_t stream);
+int colsum_reduce_f64(const double* partials, int n_partials, int B, double* sums, cudaStream_t stream);
+// out[b, n] = X[n, b] / sums[b]
+int state_to_scores_f64(const double* X, int nb, int N, int B, const double* sums, double* out, cudaStream_t stream);
 
 // ----------------------------------------------------------------------------- K2: similarity
 // S[b, m] = <Q[b, :], E[m, :]>  (fp32 FMA).  Q [Bq, dim], E [M, dim], S [Bq, ldS].

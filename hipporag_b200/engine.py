@@ -24,13 +24,15 @@ from ._lib import (HragError, PPR_CHEBYSHEV, PPR_FP32, PPR_MIXED, PPR_POWER, SIM
                    SIM_FP32)
 
 
-def build_transition_csr(n_nodes: int, edge_src, edge_dst, edge_w) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+def build_transition_csr(n_nodes: int, edge_src, edge_dst, edge_w,
+                         dtype=np.float32) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """CSR of P = W D^-1 from an igraph-style undirected multigraph edge list.
 
     Host-side ingest of the graph ``add_new_edges`` builds (``HippoRAG.py:1189-1223``): every
     edge (u, v, w) contributes w to W[u, v] and W[v, u]; parallel edges sum (the reference emits
     each fact as (s, o) and (o, s), ``:907-910``); edges with w <= 0 carry nothing; columns are
-    divided by the vertex strength.  Returns (row_ptr int64, col int32, val float32).
+    divided by the vertex strength.  Returns (row_ptr int64, col int32, val ``dtype``): float32 by
+    default, ``np.float64`` for the operator ``Engine.ppr_f64`` solves with.
     """
     import scipy.sparse as sp
     src = np.asarray(edge_src, dtype=np.int64)
@@ -50,7 +52,7 @@ def build_transition_csr(n_nodes: int, edge_src, edge_dst, edge_w) -> Tuple[np.n
     inv = np.zeros_like(strength)
     nz = strength > 0
     inv[nz] = 1.0 / strength[nz]
-    val = (W.data * inv[W.indices]).astype(np.float32)
+    val = (W.data * inv[W.indices]).astype(dtype)
     return W.indptr.astype(np.int64), W.indices.astype(np.int32), val
 
 
@@ -167,9 +169,13 @@ class Engine:
 
     def load_graph_csr(self, n_nodes: int, row_ptr, col, val, balanced: bool = True):
         """Full CSR of P; with node-range sharding this rank's row slice is cut out here -- by default along a
-        work-balanced partition (``balanced_row_bounds``), ``balanced=False`` = equal row counts (``shard_rows``)."""
+        work-balanced partition (``balanced_row_bounds``), ``balanced=False`` = equal row counts (``shard_rows``).
+        A float64 ``val`` also keeps the fp64 operator ``ppr_f64`` needs (``hrag_load_graph_csr_f64``; the fp32
+        plane every other solver sweeps is the same ``val.astype(float32)``); any other dtype is loaded as fp32."""
         row_ptr = np.ascontiguousarray(row_ptr, dtype=np.int64)
-        col, val = _i32(col), _f32(val)
+        f64 = np.asarray(val).dtype == np.float64
+        col = _i32(col)
+        val = np.ascontiguousarray(val, dtype=np.float64) if f64 else _f32(val)
         lo, hi = (0, n_nodes)
         if self.world > 1:
             if balanced:
@@ -179,8 +185,8 @@ class Engine:
             else:
                 lo, hi = shard_rows(n_nodes, self.rank, self.world)
             row_ptr, col, val = slice_csr_rows(row_ptr, col, val, lo, hi)
-        _lib.check(self._lib.hrag_load_graph_csr(self._h, n_nodes, lo, hi, int(col.shape[0]), _ptr(row_ptr),
-                                                 _ptr(col), _ptr(val)))
+        load = self._lib.hrag_load_graph_csr_f64 if f64 else self._lib.hrag_load_graph_csr
+        _lib.check(load(self._h, n_nodes, lo, hi, int(col.shape[0]), _ptr(row_ptr), _ptr(col), _ptr(val)))
         self.n_nodes = n_nodes
 
     def load_tables(self, passage_vid, fact_subj_vid, fact_obj_vid, ent_chunk_count):
@@ -295,6 +301,19 @@ class Engine:
             raise ValueError("reset must have one entry per vertex")
         out = np.empty_like(r)
         _lib.check(self._lib.hrag_ppr(self._h, r.shape[0], _ptr(r), damping, int(iters), float(tol), _ptr(out)))
+        return out[0] if single else out
+
+    def ppr_f64(self, reset, damping: float = 0.5, tol: float = 0.0) -> np.ndarray:
+        """``run_ppr`` at PRPACK's accuracy: reset [B, N] (or [N]) -> float64 probabilities, same shape, each column
+        within ``tol`` relative L1 error (0 = 1e-10) by a rigorous a-posteriori bound (``hrag_ppr_f64``).  Needs a
+        graph loaded from float64 values (``load_graph``, or ``load_graph_csr`` with a float64 ``val``)."""
+        r = np.ascontiguousarray(reset, dtype=np.float64)
+        single = r.ndim == 1
+        r = r.reshape(1, -1) if single else r
+        if r.shape[1] != self.n_nodes:
+            raise ValueError("reset must have one entry per vertex")
+        out = np.empty_like(r)
+        _lib.check(self._lib.hrag_ppr_f64(self._h, r.shape[0], _ptr(r), damping, float(tol), _ptr(out)))
         return out[0] if single else out
 
     def similarity(self, which: int, q) -> np.ndarray:

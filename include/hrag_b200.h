@@ -52,9 +52,12 @@ typedef struct hrag_stats {
     int64_t kernel_launches; /* kernels of this library launched since the last reset  */
     int64_t h2d_bytes;
     int64_t d2h_bytes;
-    double ppr_residual;     /* mixed solver, last call: measured relative L1 residual of the fp16 first solve */
-    double ppr_error_bound;  /* ... times the predicted contraction of the refinement round (a-posteriori    */
-                             /* bound on the relative L1 error of the PPR vectors of that call)              */
+    double ppr_residual;     /* last mixed-solver call: measured relative L1 residual of the fp16 first solve; */
+                             /* last hrag_ppr_f64 call: max over its columns of ||r||_1 / ||v||_1 after the    */
+                             /* final refinement round (r = v - (I - damping P) x, fp64)                       */
+    double ppr_error_bound;  /* a-posteriori bound on the relative L1 error of the PPR vectors of that call:   */
+                             /* mixed solver: ppr_residual x the predicted contraction of the refinement round; */
+                             /* hrag_ppr_f64: 2 ppr_residual / (1 - damping), rigorous (no model constant)     */
 } hrag_stats_t;
 
 const char* hrag_last_error(void);
@@ -91,6 +94,14 @@ int hrag_p2p_import(hrag_t* h, const void* handles, int world);
  * replicas pass row_lo = 0, row_hi = n_nodes. */
 int hrag_load_graph_csr(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, int64_t nnz,
                         const int64_t* row_ptr, const int32_t* col, const float* val);
+
+/* Same as hrag_load_graph_csr from float64 values of P (the graph of HippoRAG.py:1189-1223 as run_ppr's
+ * PRPACK call sees it, :1736-1743): the fp32 plane every solver sweeps is fp32(val), bitwise what
+ * hrag_load_graph_csr stores for those values, and a second plane lo = fp32(val - fp32(val)) keeps P to
+ * ~2^-48 relative for hrag_ppr_f64 (4 more bytes per non-zero of HBM).  hrag_load_graph_coo keeps the lo
+ * plane as well; a graph loaded through hrag_load_graph_csr has none. */
+int hrag_load_graph_csr_f64(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, int64_t nnz,
+                            const int64_t* row_ptr, const int32_t* col, const double* val);
 
 /* Same graph from the igraph-style undirected multigraph edge list itself
  * (graph.get_edgelist() + graph.es["weight"]): every edge (src, dst, w) contributes w to W[src,dst]
@@ -175,6 +186,15 @@ int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const fl
 /* run_ppr's numeric core (HippoRAG.py:1735-1743) for B reset vectors: reset is [B, N]
  * (host), NaN/negative entries count as 0; out is [B, N] probabilities.  iters / tol as in hrag_stage_b. */
 int hrag_ppr(hrag_t* h, int32_t B, const float* reset, float damping, int32_t iters, float tol, float* out);
+
+/* run_ppr at PRPACK's accuracy (HippoRAG.py:1735-1743: float64 reset, float64 scores, tolerance 1e-10) for B
+ * reset vectors: reset is [B, N] float64 (host), NaN/negative entries count as 0; out is [B, N] float64
+ * probabilities; damping is taken in float64 as PRPACK takes it.  Iterative refinement: fp32 sweeps solve each correction, the residual is recomputed in fp64
+ * against the fp64 operator, until the rigorous bound 2 ||r||_1 / ((1 - damping) ||v||_1) on the relative L1
+ * error of every column is <= tol (0 = 1e-10; below 1e-13 is rejected).  Status 4 when 4 rounds do not reach
+ * tol.  ppr_residual / ppr_error_bound of hrag_get_stats report the call.  Needs a graph loaded through
+ * hrag_load_graph_csr_f64 or hrag_load_graph_coo; fails on a node-range-sharded handle (world > 1). */
+int hrag_ppr_f64(hrag_t* h, int32_t B, const double* reset, double damping, double tol, double* out);
 
 /* Full score vectors for code that calls get_fact_scores (which = 0, HippoRAG.py:1427-1465)
  * or dense_passage_retrieval (which = 1, :1467-1502) directly: out[b, :] = min-max-normalised
