@@ -1,0 +1,239 @@
+// The handle behind the C ABI of libhrag_b200.so and what the host sources share: api.cu (lifecycle, options, stages
+// A/B, similarity, stats), ingest.cu (graph, tables, embeddings), solve.cu (the PPR solvers) and comm.cu (NCCL, peers).
+//
+// HBM layout per handle (N nodes, P passages, F facts, d dims; DESIGN.md section 3):
+//   graph     row_ptr int32[n_rows+1], cv int2[nnz] {col, fp32 bits of P[i,j]}, row_order int32[n_rows]   (resident)
+//             + val_lo fp32[nnz] = fp32(P64 - hi) when loaded from float64 values (the fp64 solver's operator)
+//   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N], slot_map[2][N] (node -> rhs slot)       (resident)
+//   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
+//   state     mixed solver: H0..H3, H0b [N, 32] fp16 in one IPC-exportable slab; fp32 solver: V, XA, XC [N, B] fp32
+//   rhs       compact: Vc [P + 2048, 32] fp32 (exact v) + R16 [P + 2048, 32] fp16 (scaled), two sets (double-buffered)
+//   scores    S_pass [chunk, P] fp32; fact scores are never materialised in the fused modes (72 B per query x tile)
+// Streams: `stream` runs the similarity, the solves and the selection; `stream2` builds the compact right-hand side of
+// sub-batch i + 1 while sub-batch i is being solved.  On one GPU a sub-batch's solve is replayed as a CUDA graph.
+#pragma once
+#include <nccl.h>
+
+#include <atomic>
+#include <utility>
+#include <vector>
+
+#include "../../include/hrag_b200.h"
+#include "common.cuh"
+#include "kernels.h"
+
+namespace hrag {
+
+struct NcclApi {
+    void* lib = nullptr;
+    ncclResult_t (*GetUniqueId)(ncclUniqueId*) = nullptr;
+    ncclResult_t (*CommInitRank)(ncclComm_t*, int, ncclUniqueId, int) = nullptr;
+    ncclResult_t (*CommDestroy)(ncclComm_t) = nullptr;
+    ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
+    ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t,
+                              cudaStream_t) = nullptr;
+    ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
+    ncclResult_t (*GroupStart)() = nullptr;
+    ncclResult_t (*GroupEnd)() = nullptr;
+    const char* (*GetErrorString)(ncclResult_t) = nullptr;
+};
+inline NcclApi g_nccl;   // filled in by load_nccl (comm.cu): only sharded runs need NCCL
+#define HRAG_NCCL(expr)                                                                        \
+    do {                                                                                       \
+        ncclResult_t _r = (expr);                                                              \
+        if (_r != ncclSuccess) {                                                               \
+            ::hrag::set_error(std::string(#expr) + " -> " + g_nccl.GetErrorString(_r));        \
+            return 3;                                                                          \
+        }                                                                                      \
+    } while (0)
+
+// Bumped whenever device storage is freed, so also by every reallocation (any handle, any thread): the captured CUDA
+// graphs of the mixed solve hold raw pointers, so they are replayed only under the generation they were captured in.
+inline std::atomic<int64_t> g_buf_generation{0};
+
+// One device allocation, owned: move-only, freed by its destructor.
+struct Buf {
+    void* p = nullptr;
+    size_t cap = 0;
+    Buf() = default;
+    Buf(Buf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }   // o frees ours
+    ~Buf() { reset(); }
+    int ensure(size_t bytes) {    // grow-only; the contents are not kept
+        if (bytes <= cap) return 0;
+        reset();
+        HRAG_CUDA(cudaMalloc(&p, bytes));
+        cap = bytes;
+        return 0;
+    }
+    template <class T, class V> int upload(const T* src, size_t n, V** view) {   // n elements; *view = the device copy
+        HRAG_TRY(ensure(n ? n * sizeof(T) : 1));                          // non-null even when empty
+        if (n) HRAG_CUDA(cudaMemcpy(p, src, n * sizeof(T), cudaMemcpyHostToDevice));
+        *view = as<T>();
+        return 0;
+    }
+    int zeros(size_t bytes) {     // ensure + clear
+        HRAG_TRY(ensure(bytes));
+        HRAG_CUDA(cudaMemset(p, 0, bytes));
+        return 0;
+    }
+    void reset() {
+        if (p) { g_buf_generation += 1; cudaFree(p); }
+        p = nullptr; cap = 0;
+    }
+    template <class T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+enum Stage { ST_SIM_FACT = 0, ST_SEL_FACT, ST_SIM_PASS, ST_SEED, ST_PPR, ST_TOPK, ST_COMM, ST_COUNT };
+struct Span { int stage; cudaEvent_t a, b; };
+
+// Storage behind the views the kernel launchers take (PprGraph g, SeedTables t), filled in by ingest.cu
+struct GraphMem { Buf row_ptr, cv, row_order, long_rows, long_seg_ptr, segs, seg_partial, val_lo, seg_partial64; };
+struct TableMem { Buf passage_vid, fact_subj_vid, fact_obj_vid, ent_chunk_count; };
+struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passages)
+    const float* f32 = nullptr;   // fp32 rows: borrowed from the caller (device upload, caller keeps it alive) or own
+    Buf own, hi, lo;              // hi / lo: bf16 split for the tensor-core path (dim % 8 == 0)
+    int64_t rows = 0;             // rows held by THIS handle (node-range sharding: the rank's slice of the facts)
+};
+
+}  // namespace hrag
+
+struct hrag_handle {
+    int device = 0;
+    int shard_mode = 0;
+    int rank = 0, world = 1;
+    ncclComm_t comm = nullptr;
+    cudaStream_t stream = nullptr;
+
+    hrag::PprGraph g;                  // view of `graph`
+    hrag::GraphMem graph;
+    int64_t chunk_rows = 0;      // rows per rank (sharded) = ceil(N / world)
+    std::vector<int64_t> row_bounds;   // optional [world + 1]: rank r owns rows [row_bounds[r], row_bounds[r + 1]) -- a
+                                       // work-balanced partition (non-zeros + 4 per row) instead of equal row counts
+    hrag::SeedTables t;                // view of `tables`
+    hrag::TableMem tables;
+    hrag::EmbMem emb[2];
+    int num_sms = 132;
+    int64_t fact_row_lo = 0;        // first global fact row of the local slice
+    int64_t n_facts_global = 0;
+    int dim = 0;
+
+    int ppr_method = HRAG_PPR_CHEBYSHEV;
+    int ppr_iters = 0;    // 0 = derived from damping / tol (plan_sweeps): 14 Chebyshev sweeps at damping 0.5
+    int ppr_batch = 16;
+    int sim_mode = HRAG_SIM_BF16X3;
+    bool keep_fact_scores = false;   // debugging: materialise S_fact even in tensor-core modes
+    int ppr_precision = HRAG_PPR_MIXED;   // applies to batches of > 16 queries; smaller ones run fp32
+    int mixed_m1 = 0, mixed_m2 = 0;   // 0 = derived from damping (8 / 7 at damping 0.5)
+    double check_tol = 0.0, check_kappa = 0.0;   // > 0: this call's mixed solves are verified in resolve_spans
+    double last_rho = 0.0;            // measured relative L1 residual: of the fp16 first solve (last mixed call), of
+                                      // the final refinement round (last hrag_ppr_f64 call)
+    bool rho_dirty = false;           // a mixed solve ran in this call: rho must be read / cleared in resolve_spans
+    double last_bound = 0.0;          // a-posteriori bound on the relative L1 error of the last mixed / fp64 call
+
+    // fp32 solver state [N, B]; column-sum partials and sums, shared with the mixed solver
+    hrag::Buf V, XA, XC, partials, sums;
+    // fp64 solver (hrag_ppr_f64): iterate X64 and reset V64 [N, B] fp64, host-layout staging io64 [B, N] fp64 (reset
+    // in, probabilities out), column-sum partials part64, sums64 = [vsum | rsum | xsum] x 16
+    hrag::Buf X64, V64, io64, part64, sums64;
+    // mixed solver: one allocation [H0 | H1 | H2 | H3 | H0b | flags] so a single IPC handle exposes every buffer a
+    // peer sweep may have to write into (K5, fused exchange for node-range sharding); H / H0b point into it
+    hrag::Buf slab;
+    size_t slab_hb = 0;                       // bytes of one fp16 state buffer inside the slab
+    void* H[4] = {nullptr, nullptr, nullptr, nullptr};
+    void* H0b = nullptr;
+    hrag::Buf mixed_aux, rho, p2p_err, done_ctr;
+    // double-buffered per-sub-batch inputs (set s: x0 = H[0] / H0b, scales mixed_aux / mixed_aux1, compact rhs
+    // Vc[s] / R16[s] addressed through slot_map[s]): stream2 prepares sub-batch i+1 while `stream` sweeps sub-batch i
+    hrag::Buf mixed_aux1, prep_scratch;
+    hrag::Buf slot_map[2], slot_vid[2], Vc[2], R16[2];
+    bool slot_maps_valid = false;
+    // scratch and I/O staging
+    hrag::Buf S_fact, S_pass, mm_fact, mm_pass, mode, seed_vid, seed_w, q_hi, q_lo, part_mm, part_keys;
+    hrag::Buf xr_mm, xr_keys;             // fact-sharded stage A: [world, Bq] min/max and [world, Bq, 8] best keys
+    hrag::Buf d_q, d_q2, d_top_idx, d_top_score, d_nvalid, d_kept_idx, d_kept_score, d_dpr, d_out_ids, d_out_scores;
+    hrag::Buf d_reset, d_scores;
+    // CUDA graphs of the mixed solve, one per (buffer set, sweep plan, g_buf_generation)
+    struct SolveGraph {
+        const void *x0 = nullptr, *slot_map = nullptr, *rhs16 = nullptr, *vexact = nullptr;
+        int m1 = 0, m2 = 0;
+        float alpha = 0.f;
+        int64_t generation = 0;
+        cudaGraphExec_t exec = nullptr;
+        void *X0 = nullptr, *D = nullptr;
+        int64_t sweeps = 0, columns = 0, launches = 0;
+    };
+    std::vector<SolveGraph> solve_graphs;
+    bool p2p = false;
+    void* peer_slab[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+    unsigned long long epoch = 0;             // exchange epochs signalled so far (same sequence on every rank)
+    cudaStream_t stream2 = nullptr;
+    cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_released[2] = {nullptr, nullptr}, ev_inputs = nullptr;
+    int64_t last_fact_rows = 0, last_pass_rows = 0;
+
+    hrag_stats_t stats{};
+    std::vector<hrag::Span> spans;
+    std::vector<cudaEvent_t> pool;
+};
+
+namespace hrag {
+
+inline cudaEvent_t get_event(hrag_t* h) {
+    if (!h->pool.empty()) { cudaEvent_t e = h->pool.back(); h->pool.pop_back(); return e; }
+    cudaEvent_t e;
+    cudaEventCreate(&e);
+    return e;
+}
+struct StageTimer {
+    hrag_t* h; int idx;
+    StageTimer(hrag_t* h_, int stage) : h(h_) {
+        Span s{stage, get_event(h), get_event(h)};
+        cudaEventRecord(s.a, h->stream);
+        h->spans.push_back(s);
+        idx = (int)h->spans.size() - 1;
+    }
+    ~StageTimer() { cudaEventRecord(h->spans[idx].b, h->stream); }
+};
+
+inline int h2d(hrag_t* h, void* dst, const void* src, size_t bytes) {
+    HRAG_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, h->stream));
+    h->stats.h2d_bytes += (int64_t)bytes;
+    return 0;
+}
+inline int d2h(hrag_t* h, void* dst, const void* src, size_t bytes) {
+    HRAG_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, h->stream));
+    h->stats.d2h_bytes += (int64_t)bytes;
+    return 0;
+}
+
+constexpr int kSeedSlots = kSeedSlotsPerQuery;   // 2 phrases per kept fact, <= 32 kept facts
+constexpr float kMixedT = 64.f;    // residual scale: r ~ 5e-4 x, keeps it in fp16's normal range
+// sums layout (doubles): [0, 32) column sums of x0, [32, 64) of d, [64, 96) of |r|, [96, 160) of v (two buffer sets)
+constexpr int kSumX0 = 0, kSumD = 32, kSumR = 64, kSumV = 96;
+constexpr double kDefaultTol = 1e-6;     // relative L1 accuracy of the PPR vector when the caller passes tol <= 0
+struct SweepPlan {
+    bool mixed = false;
+    int iters = 14;          // fp32 solver
+    int m1 = 8, m2 = 7;      // mixed solver
+    double kappa = 0.0;      // predicted contraction of the refinement round (mixed)
+    double tol = kDefaultTol;
+    bool check = false;      // verify the measured residual bound at the end of the call
+};
+SweepPlan plan_sweeps(const hrag_t* h, float alpha, int iters_arg, float tol_arg, bool want_mixed);
+int round_batch(int b);
+int ensure_state(hrag_t* h, int B);
+int ensure_state_mixed(hrag_t* h);
+int ensure_compact_rhs(hrag_t* h);
+int resolve_spans(hrag_t* h);   // end of a call: checks the mixed solves, accumulates the stage times
+int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot_map, const float* Vexact,
+                  const void* rhs16, void* x0_dense, const float* scale, const double* vsum, void** X0, void** D);
+int dev_ppr(hrag_t* h, int B, int iters, float alpha, float** result);
+
+int exchange_rows(hrag_t* h, float* y, int B);
+int p2p_wait(hrag_t* h);
+int p2p_signal(hrag_t* h);
+int mixed_sweep_x(hrag_t* h, int mode, const void* x, const int* slot_map, const void* rhs, const float* v32,
+                  const float* scale, const void* prev, void* y, float alpha, float w, float t, float* part,
+                  int* n_part);
+
+}  // namespace hrag

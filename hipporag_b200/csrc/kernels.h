@@ -1,5 +1,5 @@
 // Launchers of the hand-written sm_90a kernels (K1..K4).  Host-callable C++; the C ABI in
-// api.cu composes them.  All pointers are device pointers; all launches go to `stream`.
+// api.cu / solve.cu / ingest.cu / comm.cu composes them.  All pointers are device pointers; all launches go to `stream`.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -10,7 +10,7 @@
 //     3. d   ~ solve(r)          m2 Chebyshev sweeps in fp16 (r scaled by t)
 //     4. x   = x0 + d            only where it is consumed (passage rows) + the column sums
 // (when one round cannot reach the requested tolerance -- large damping -- the caller takes the fp32
-// solver instead, api.cu plan_sweeps).  Every product is accumulated in fp32; only the STORED
+// solver instead, solve.cu plan_sweeps).  Every product is accumulated in fp32; only the STORED
 // iterate is rounded, and step 2 measures exactly what that rounding (and the truncated step 1)
 // left behind: its column sums give the residual check of the solve for free.
 //
@@ -403,7 +403,7 @@ k_sweep_long_finalize_h(int n_long, const int* __restrict__ long_rows, const int
     sync_signal(sy);
 }
 
-// stand-alone halves of the handshake, for the exchange points that are not sweeps (see api.cu)
+// stand-alone halves of the handshake, for the exchange points that are not sweeps (see comm.cu)
 __global__ void k_epoch_wait(const SweepSync sy) { sync_wait(sy); }
 __global__ void k_epoch_signal(const SweepSync sy) { sync_signal(sy); }
 
@@ -575,7 +575,7 @@ k_slot_map_passages(int P, const int* __restrict__ passage_vid, int* __restrict_
 }
 
 // relative L1 size of the refinement residual per column: rho[b] = (sum_i |r_i| / t) / (scale[b] * sum v);
-// keeps the running maximum over every solve since the last reset (checked on the host, api.cu)
+// keeps the running maximum over every solve since the last reset (checked on the host, solve.cu)
 __global__ void k_residual_check(const double* __restrict__ rsum, const double* __restrict__ vsum,
                                  const float* __restrict__ scale, float inv_t, float* __restrict__ rho_max) {
     const int b = threadIdx.x;

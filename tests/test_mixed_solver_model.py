@@ -1,4 +1,4 @@
-"""A numpy model of the mixed-precision PPR solver of csrc/ppr_mixed.cu / api.cu (fp16 STORAGE of every iterate and of
+"""A numpy model of the mixed-precision PPR solver of csrc/ppr_mixed.cu / solve.cu (fp16 STORAGE of every iterate and of
 the scaled right-hand side, fp32 arithmetic, Chebyshev semi-iteration, one refinement round through the fp32 residual),
 run with the sweep counts `hrag_plan_sweeps` derives, against the float64 oracle.  CPU only: it pins the NUMERICS of the
 design -- the fp16 noise constant behind the a-priori plan, the residual the a-posteriori check reads, the accuracy after

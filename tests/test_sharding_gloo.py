@@ -148,7 +148,7 @@ def test_balanced_row_bounds_split_work_not_rows():
 
 def _balanced_worker(rank, world, port, n, src, dst, w, R, out_path):
     """The sharded solve with the WORK-BALANCED partition (unequal row ranges): every rank sweeps rows
-    [bounds[rank], bounds[rank + 1]) and the exchange is one broadcast per owner (api.cu exchange_rows_bytes with
+    [bounds[rank], bounds[rank + 1]) and the exchange is one broadcast per owner (comm.cu exchange_rows_bytes with
     row_bounds set; on devices the fused kernel writes the same ranges into the peers' buffers)."""
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     dist.init_process_group("gloo", rank=rank, world_size=world)
