@@ -50,6 +50,7 @@ SIGNATURES = {
     "hrag_load_graph_csr": (C.c_int, [_p, _i64, _i64, _i64, _i64, _p, _p, _p]),
     "hrag_load_graph_csr_f64": (C.c_int, [_p, _i64, _i64, _i64, _i64, _p, _p, _p]),
     "hrag_load_graph_coo": (C.c_int, [_p, _i64, _i64, _p, _p, _p]),
+    "hrag_load_graph_coo_device": (C.c_int, [_p, _i64, _i64, _p, _p, _p]),
     "hrag_load_tables": (C.c_int, [_p, _i64, _p, _i64, _p, _p, _p]),
     "hrag_load_embeddings": (C.c_int, [_p, C.c_int, _i64, _i32, _p, C.c_int]),
     "hrag_load_embeddings_begin": (C.c_int, [_p, C.c_int, _i64, _i32]),
@@ -71,6 +72,7 @@ SIGNATURES = {
     "hrag_reset_stats": (C.c_int, [_p]),
     "hrag_debug_keep_scores": (C.c_int, [_p, C.c_int]),
     "hrag_debug_copy": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
+    "hrag_debug_graph": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
 }
 
 _lib = None

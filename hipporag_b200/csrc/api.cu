@@ -606,4 +606,21 @@ int hrag_debug_copy(hrag_t* h, int which, float* host_out, int64_t max_elems, in
     return 0;
 }
 
+int hrag_debug_graph(hrag_t* h, int plane, void* host_out, int64_t max_bytes, int64_t* n_written) {
+    HRAG_CHECK(h && n_written, "hrag_debug_graph: null argument");
+    HRAG_CHECK(h->g.cv, "hrag_debug_graph: no graph loaded");
+    HRAG_CHECK(plane >= 0 && plane <= 6, "hrag_debug_graph: plane must be in [0, 6]");
+    const hrag::PprGraph& g = h->g;
+    const void* src[7] = {g.row_ptr, g.cv, g.val_lo, g.row_order, g.long_rows, g.long_seg_ptr, g.segs};
+    const int64_t bytes[7] = {4 * (int64_t)(g.n_rows + 1), 8 * g.nnz, g.val_lo ? 4 * g.nnz : 0, 4 * (int64_t)g.n_rows,
+                              4 * (int64_t)g.n_long, g.n_long ? 4 * (int64_t)(g.n_long + 1) : 0, 16 * (int64_t)g.n_seg};
+    *n_written = bytes[plane];
+    if (!host_out) return 0;
+    HRAG_CHECK(bytes[plane] <= max_bytes, "hrag_debug_graph: host buffer too small");
+    HRAG_CUDA(cudaSetDevice(h->device));
+    HRAG_CUDA(cudaStreamSynchronize(h->stream));
+    if (bytes[plane]) HRAG_CUDA(cudaMemcpy(host_out, src[plane], (size_t)bytes[plane], cudaMemcpyDeviceToHost));
+    return 0;
+}
+
 }  // extern "C"

@@ -1,5 +1,6 @@
 // The handle behind the C ABI of libhrag_b200.so and what the host sources share: api.cu (lifecycle, options, stages
-// A/B, similarity, stats), ingest.cu (graph, tables, embeddings), solve.cu (the PPR solvers) and comm.cu (NCCL, peers).
+// A/B, similarity, stats), ingest.cu (graph, tables, embeddings), graph_build.cu (the graph planes, built on the
+// device), solve.cu (the PPR solvers) and comm.cu (NCCL, peers).
 //
 // HBM layout per handle (N nodes, P passages, F facts, d dims; DESIGN.md section 3):
 //   graph     row_ptr int32[n_rows+1], cv int2[nnz] {col, fp32 bits of P[i,j]}, row_order int32[n_rows]   (resident)
@@ -228,6 +229,18 @@ int resolve_spans(hrag_t* h);   // end of a call: checks the mixed solves, accum
 int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot_map, const float* Vexact,
                   const void* rhs16, void* x0_dense, const float* scale, const double* vsum, void** X0, void** D);
 int dev_ppr(hrag_t* h, int B, int iters, float alpha, float** result);
+
+// graph_build.cu: the graph built on the device, on `stream`; both return once the device work is done.
+struct DeviceCsr { Buf row_ptr, col, val; int64_t nnz = 0; };   // int64 [N + 1], int32 [nnz], fp64 [nnz]
+// CSR of P = W D^-1 from a device edge list with n_edges < 2^30 (device pointers); *bad_edges = an endpoint lies
+// outside [0, n_nodes), and then nothing was built.
+int coo_to_csr(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32_t* src, const int32_t* dst, const double* w,
+               DeviceCsr* out, bool* bad_edges);
+// Replaces the handle's graph by rows [row_lo, row_hi) of a validated device CSR: row_ptr[0 .. n_rows] (offsets minus
+// `base` index col / val), exactly one of val (fp32) / val64 given; bounds = the row partition to install.
+int install_graph(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, int64_t nnz, const int64_t* row_ptr,
+                  int64_t base, const int32_t* col, const float* val, const double* val64,
+                  const std::vector<int64_t>& bounds);
 
 int exchange_rows(hrag_t* h, float* y, int B);
 int p2p_wait(hrag_t* h);

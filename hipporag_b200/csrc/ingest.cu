@@ -1,8 +1,8 @@
-// Uploads: the graph (CSR or COO, fp32 or fp64 values), the seed tables and the embedding matrices.  The graph and
-// table loaders check every input on the host before they touch the handle, so a rejected load leaves the handle as
-// it was; an upload that fails after that leaves no graph (no tables) rather than a half-loaded one.
+// Uploads: the graph (CSR or COO, fp32 or fp64 values, COO from host or device arrays), the seed tables and the
+// embedding matrices.  The graph and table loaders check every input (a device edge list: on the device) before they
+// touch the handle, so a rejected load leaves the handle as it was; a load that fails after that leaves no graph (no
+// tables) rather than a half-loaded one.  The graph planes themselves are built on the device (graph_build.cu).
 #include <algorithm>
-#include <cstring>
 
 #include "handle.h"
 
@@ -25,19 +25,25 @@ std::vector<int64_t> balanced_bounds(const int64_t* row_ptr, int64_t n_nodes, in
     return b;
 }
 
-// The two CSR entries and the COO entry share this: exactly one of val (fp32) / val64 is given.  From val64 the fp32
-// plane cv stores fp32(val64) -- bitwise what the fp32 entry stores for that rounding -- and the lo plane
-// fp32(val64 - hi).  new_bounds: the row partition to install instead of the handle's (node-range sharding).
+template <class T> int upload_to(hrag_t* h, Buf& b, const T* src, size_t n) {   // ordered before h->stream's work
+    HRAG_TRY(b.ensure(n ? n * sizeof(T) : 1));
+    if (n) HRAG_CUDA(cudaMemcpyAsync(b.p, src, n * sizeof(T), cudaMemcpyHostToDevice, h->stream));
+    return 0;
+}
+
+// The two CSR entries share this: exactly one of val (fp32) / val64 is given.  Checks every input on the host, then
+// uploads it and builds the planes on the device (install_graph: from val64 the fp32 plane cv stores fp32(val64) --
+// bitwise what the fp32 entry stores for that rounding -- and the lo plane fp32(val64 - hi)).
 int load_graph_csr_impl(hrag_t* h, const std::string& who, int64_t n_nodes, int64_t row_lo, int64_t row_hi,
                         int64_t nnz, const int64_t* row_ptr, const int32_t* col, const float* val,
-                        const double* val64, const std::vector<int64_t>* new_bounds = nullptr) {
+                        const double* val64) {
     HRAG_CHECK(h && row_ptr && (nnz == 0 || (col && (val || val64))), who + ": null argument");
     HRAG_CHECK(n_nodes > 0 && n_nodes < (int64_t)1 << 30, who + ": n_nodes out of range");
     HRAG_CHECK(nnz >= 0 && nnz < ((int64_t)1 << 31) - 8, who + ": nnz must fit int32");
     HRAG_CHECK(0 <= row_lo && row_lo <= row_hi && row_hi <= n_nodes, who + ": bad row range");
     HRAG_CUDA(cudaSetDevice(h->device));
-    const std::vector<int64_t>& bounds = new_bounds ? *new_bounds : h->row_bounds;
-    const int n_rows = (int)(row_hi - row_lo);
+    const std::vector<int64_t>& bounds = h->row_bounds;
+    const int64_t n_rows = row_hi - row_lo;
     HRAG_CHECK(row_ptr[0] == 0 && row_ptr[n_rows] == nnz, who + ": row_ptr does not span nnz");
     if (h->world > 1) {
         HRAG_CHECK(bounds.empty() || bounds.back() == n_nodes,
@@ -49,76 +55,41 @@ int load_graph_csr_impl(hrag_t* h, const std::string& who, int64_t n_nodes, int6
                    who + ": sharded ranks own rows [rank*ceil(N/world), (rank+1)*ceil(N/world)), or the range "
                    "given by hrag_comm_set_row_bounds");
     }
-    PprGraph g;
-    g.num_sms = h->num_sms;
-    g.n_global = (int)n_nodes;
-    g.row_lo = (int)row_lo;
-    g.n_rows = n_rows;
-    g.nnz = nnz;
-    g.long_thresh = 256;
-    g.max_batch = 64;
-    std::vector<int> rp(n_rows + 1);
-    std::vector<int2> cv((size_t)nnz);
-    std::vector<float> lo(val64 ? (size_t)nnz : 0);
-    std::vector<int> long_rows, long_seg_ptr;
-    std::vector<int4> segs;
-    const int seg_len = 256;
-    for (int r = 0; r < n_rows; ++r) {
-        const int64_t s = row_ptr[r], e = row_ptr[r + 1];
-        HRAG_CHECK(s <= e && e <= nnz, who + ": row_ptr not monotone");
-        rp[r] = (int)s;
-        if (e - s > g.long_thresh) {
-            long_rows.push_back(r);
-            long_seg_ptr.push_back((int)segs.size());
-            for (int64_t a = s; a < e; a += seg_len)
-                segs.push_back(make_int4(r, (int)a, (int)std::min<int64_t>(e, a + seg_len), 0));
-        }
-    }
-    rp[n_rows] = (int)nnz;
-    long_seg_ptr.push_back((int)segs.size());
-    for (int64_t i = 0; i < nnz; ++i) {
+    for (int64_t r = 0; r < n_rows; ++r)
+        HRAG_CHECK(row_ptr[r] <= row_ptr[r + 1] && row_ptr[r + 1] <= nnz, who + ": row_ptr not monotone");
+    for (int64_t i = 0; i < nnz; ++i)
         HRAG_CHECK(col[i] >= 0 && col[i] < n_nodes, who + ": column index out of range");
-        const float hi = val64 ? (float)val64[i] : val[i];
-        int bits;
-        memcpy(&bits, &hi, 4);
-        cv[(size_t)i] = make_int2(col[i], bits);
-        if (val64) lo[(size_t)i] = (float)(val64[i] - (double)hi);
-    }
-    // fp16 sweep: within each block of 64 rows (one CTA) order the rows by length so a warp's 8 rows match
-    std::vector<int> order(n_rows);
-    for (int r = 0; r < n_rows; ++r) order[r] = r;
-    for (int b0 = 0; b0 < n_rows; b0 += 64) {
-        const int b1 = std::min(n_rows, b0 + 64);
-        std::stable_sort(order.begin() + b0, order.begin() + b1,
-                         [&](int x, int y) { return rp[x + 1] - rp[x] > rp[y + 1] - rp[y]; });
-    }
-    g.n_long = (int)long_rows.size();
-    g.n_seg = (int)segs.size();
+    Buf d_row_ptr, d_col, d_val;   // the old graph stays until all of the input is on the device
+    HRAG_TRY(upload_to(h, d_row_ptr, row_ptr, (size_t)n_rows + 1));
+    HRAG_TRY(upload_to(h, d_col, col, (size_t)nnz));
+    if (val64) HRAG_TRY(upload_to(h, d_val, val64, (size_t)nnz));
+    else HRAG_TRY(upload_to(h, d_val, val, (size_t)nnz));
+    return install_graph(h, n_nodes, row_lo, row_hi, nnz, d_row_ptr.as<int64_t>(), 0, d_col.as<int32_t>(),
+                         val64 ? nullptr : d_val.as<float>(), val64 ? d_val.as<double>() : nullptr, bounds);
+}
 
-    // every input is valid: the old graph and the fp32 state sized for it go first (a reload never holds two graphs;
-    // the frees bump g_buf_generation, which invalidates every captured solve); the new graph becomes the handle's
-    // only once all of it is uploaded (a failed upload leaves no graph; the next load frees what it allocated)
-    h->graph = GraphMem{};
-    h->g = PprGraph();
-    h->V.reset(); h->XA.reset(); h->XC.reset(); h->partials.reset();
-    h->slot_maps_valid = false;
-    h->row_bounds = bounds;
-    h->chunk_rows = h->world > 1 ? ceil_div(n_nodes, h->world) : n_nodes;
-    HRAG_TRY(h->graph.row_ptr.upload(rp.data(), rp.size(), &g.row_ptr));
-    HRAG_TRY(h->graph.cv.upload(cv.data(), cv.size(), &g.cv));                    // non-null: marks a loaded graph
-    HRAG_TRY(h->graph.row_order.upload(order.data(), order.size(), &g.row_order));
-    if (val64) HRAG_TRY(h->graph.val_lo.upload(lo.data(), lo.size(), &g.val_lo));   // non-null: marks an fp64 operator
-    if (g.n_long) {
-        HRAG_TRY(h->graph.long_rows.upload(long_rows.data(), long_rows.size(), &g.long_rows));
-        HRAG_TRY(h->graph.long_seg_ptr.upload(long_seg_ptr.data(), long_seg_ptr.size(), &g.long_seg_ptr));
-        HRAG_TRY(h->graph.segs.upload(segs.data(), segs.size(), &g.segs));
-        HRAG_TRY(h->graph.seg_partial.ensure(segs.size() * (size_t)g.max_batch * sizeof(float)));
-        g.seg_partial = h->graph.seg_partial.as<float>();
-        if (val64) HRAG_TRY(h->graph.seg_partial64.ensure(segs.size() * 16 * sizeof(double)));
-        g.seg_partial64 = h->graph.seg_partial64.as<double>();
+// The two COO entries share this: src / dst / w are device pointers, sizes checked.  The edge list is validated on
+// the device before the handle is touched; with node-range sharding every rank builds the whole CSR, derives the same
+// work-balanced partition from its row_ptr and keeps its own rows.
+int load_graph_coo_impl(hrag_t* h, const std::string& who, int64_t n_nodes, int64_t n_edges, const int32_t* src,
+                        const int32_t* dst, const double* w) {
+    DeviceCsr csr;
+    bool bad_edges = false;
+    HRAG_TRY(coo_to_csr(h, n_nodes, n_edges, src, dst, w, &csr, &bad_edges));
+    HRAG_CHECK(!bad_edges, who + ": edge endpoint out of range");
+    int64_t lo = 0, hi = n_nodes, a = 0, b = csr.nnz;
+    std::vector<int64_t> bounds = h->row_bounds;
+    if (h->world > 1) {
+        std::vector<int64_t> row_ptr((size_t)n_nodes + 1);
+        HRAG_CUDA(cudaMemcpy(row_ptr.data(), csr.row_ptr.p, row_ptr.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
+        bounds = balanced_bounds(row_ptr.data(), n_nodes, h->world);
+        lo = bounds[h->rank], hi = bounds[h->rank + 1];
+        a = row_ptr[(size_t)lo], b = row_ptr[(size_t)hi];
     }
-    h->g = g;
-    return 0;
+    HRAG_CHECK(b - a < ((int64_t)1 << 31) - 8, who + ": nnz must fit int32");
+    // fp64 values: the same fp32 plane as the fp64 CSR entry, plus the lo plane hrag_ppr_f64 needs
+    return install_graph(h, n_nodes, lo, hi, b - a, csr.row_ptr.as<int64_t>() + lo, a, csr.col.as<int32_t>() + a,
+                         nullptr, csr.val.as<double>() + a, bounds);
 }
 
 // Drops embedding matrix `which`, sets dim and the rows of a `rows`-row matrix that this handle keeps (node-range
@@ -159,51 +130,25 @@ int hrag_load_graph_coo(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32
     HRAG_CHECK(h && (n_edges == 0 || (src && dst && w)), "hrag_load_graph_coo: null argument");
     HRAG_CHECK(n_nodes > 0 && n_nodes < (int64_t)1 << 30 && n_edges >= 0 && n_edges < (int64_t)1 << 30,
                "hrag_load_graph_coo: sizes out of range");
-    // symmetrise: (row, col, w) for both directions, keyed row-major
-    struct Ent { uint64_t key; double w; };
-    std::vector<Ent> e;
-    e.reserve((size_t)n_edges * 2);
-    for (int64_t i = 0; i < n_edges; ++i) {
-        const int64_t a = src[i], b = dst[i];
-        HRAG_CHECK(a >= 0 && a < n_nodes && b >= 0 && b < n_nodes, "hrag_load_graph_coo: edge endpoint out of range");
-        if (!(w[i] > 0.0)) continue;                       // non-positive (and NaN) weights carry nothing
-        e.push_back({((uint64_t)a << 32) | (uint64_t)b, w[i]});
-        e.push_back({((uint64_t)b << 32) | (uint64_t)a, w[i]});
-    }
-    std::stable_sort(e.begin(), e.end(), [](const Ent& x, const Ent& y) { return x.key < y.key; });
-    std::vector<int64_t> row_ptr((size_t)n_nodes + 1, 0);
-    std::vector<int32_t> col;
-    std::vector<double> wsum;
-    col.reserve(e.size());
-    wsum.reserve(e.size());
-    for (size_t i = 0; i < e.size();) {                    // merge parallel edges in input order
-        size_t j = i;
-        double s = 0.0;
-        while (j < e.size() && e[j].key == e[i].key) s += e[j++].w;
-        col.push_back((int32_t)(e[i].key & 0xffffffffu));
-        wsum.push_back(s);
-        row_ptr[(size_t)(e[i].key >> 32) + 1] += 1;
-        i = j;
-    }
-    for (int64_t r = 0; r < n_nodes; ++r) row_ptr[(size_t)r + 1] += row_ptr[(size_t)r];
-    std::vector<double> strength((size_t)n_nodes, 0.0);    // W is symmetric: column sums = row sums
-    for (int64_t r = 0; r < n_nodes; ++r)
-        for (int64_t k = row_ptr[(size_t)r]; k < row_ptr[(size_t)r + 1]; ++k) strength[(size_t)r] += wsum[(size_t)k];
-    std::vector<double> val(col.size());
-    for (size_t k = 0; k < col.size(); ++k) val[k] = wsum[k] / strength[(size_t)col[k]];
-    int64_t lo = 0, hi = n_nodes;
-    std::vector<int64_t> bounds = h->row_bounds;
-    if (h->world > 1) {
-        // every rank sees the whole edge list here, so all of them derive the same work-balanced partition
-        bounds = balanced_bounds(row_ptr.data(), n_nodes, h->world);
-        lo = bounds[h->rank], hi = bounds[h->rank + 1];
-    }
-    const int64_t a = row_ptr[(size_t)lo], b = row_ptr[(size_t)hi];
-    std::vector<int64_t> rp((size_t)(hi - lo) + 1);
-    for (int64_t r = lo; r <= hi; ++r) rp[(size_t)(r - lo)] = row_ptr[(size_t)r] - a;
-    // fp64 values: the same fp32 plane as before, plus the lo plane hrag_ppr_f64 needs
-    return load_graph_csr_impl(h, "hrag_load_graph_csr", n_nodes, lo, hi, b - a, rp.data(), col.data() + a, nullptr,
-                               val.data() + a, &bounds);
+    for (int64_t i = 0; i < n_edges; ++i)
+        HRAG_CHECK(src[i] >= 0 && src[i] < n_nodes && dst[i] >= 0 && dst[i] < n_nodes,
+                   "hrag_load_graph_coo: edge endpoint out of range");
+    HRAG_CUDA(cudaSetDevice(h->device));
+    Buf d_src, d_dst, d_w;
+    HRAG_TRY(upload_to(h, d_src, src, (size_t)n_edges));
+    HRAG_TRY(upload_to(h, d_dst, dst, (size_t)n_edges));
+    HRAG_TRY(upload_to(h, d_w, w, (size_t)n_edges));
+    return load_graph_coo_impl(h, "hrag_load_graph_coo", n_nodes, n_edges, d_src.as<int32_t>(), d_dst.as<int32_t>(),
+                               d_w.as<double>());
+}
+
+int hrag_load_graph_coo_device(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32_t* d_src,
+                               const int32_t* d_dst, const double* d_w) {
+    HRAG_CHECK(h && (n_edges == 0 || (d_src && d_dst && d_w)), "hrag_load_graph_coo_device: null argument");
+    HRAG_CHECK(n_nodes > 0 && n_nodes < (int64_t)1 << 30 && n_edges >= 0 && n_edges < (int64_t)1 << 30,
+               "hrag_load_graph_coo_device: sizes out of range");
+    HRAG_CUDA(cudaSetDevice(h->device));
+    return load_graph_coo_impl(h, "hrag_load_graph_coo_device", n_nodes, n_edges, d_src, d_dst, d_w);
 }
 
 int hrag_load_tables(hrag_t* h, int64_t n_passages, const int32_t* passage_vid, int64_t n_facts,

@@ -159,7 +159,27 @@ class Engine:
 
     # ---------------------------------------------------------------- uploads
     def load_graph(self, n_nodes: int, edge_src, edge_dst, edge_w):
-        """igraph-style edge list -> device CSR of P (built by the library: hrag_load_graph_coo)."""
+        """igraph-style edge list -> device CSR of P (built by the library on the GPU: hrag_load_graph_coo).
+
+        The edge list may also be three contiguous 1-D CUDA torch tensors on this handle's device -- int32, int32 and
+        float64 -- which are read in place (hrag_load_graph_coo_device) and not kept after the call."""
+        tensors = [a for a in (edge_src, edge_dst, edge_w) if hasattr(a, "is_cuda")]
+        if tensors:
+            import torch
+            want = (torch.int32, torch.int32, torch.float64)
+            for a, dt in zip((edge_src, edge_dst, edge_w), want):
+                if not (hasattr(a, "is_cuda") and a.is_cuda and a.device.index == self.device and a.dtype == dt
+                        and a.dim() == 1 and a.is_contiguous()):
+                    raise ValueError("a device edge list is three contiguous 1-D CUDA tensors on the handle's device: "
+                                     "int32 edge_src, int32 edge_dst, float64 edge_w")
+            if not edge_src.shape == edge_dst.shape == edge_w.shape:
+                raise ValueError("edge_src, edge_dst, edge_w must have the same length")
+            torch.cuda.current_stream(self.device).synchronize()     # the library reads them on its own stream
+            _lib.check(self._lib.hrag_load_graph_coo_device(
+                self._h, n_nodes, int(edge_src.shape[0]), C.c_void_p(edge_src.data_ptr()),
+                C.c_void_p(edge_dst.data_ptr()), C.c_void_p(edge_w.data_ptr())))
+            self.n_nodes = n_nodes
+            return
         s, d = _i32(edge_src), _i32(edge_dst)
         w = np.ascontiguousarray(edge_w, dtype=np.float64)
         if s.shape != d.shape or s.shape != w.shape:
@@ -372,6 +392,20 @@ class Engine:
         n = C.c_int64()
         _lib.check(self._lib.hrag_debug_copy(self._h, which, _ptr(buf), buf.shape[0], C.byref(n)))
         return buf[:n.value].reshape(-1, cols) if cols else buf[:0]
+
+    GRAPH_PLANES = {"row_ptr": (0, np.int32, 1), "cv": (1, np.int32, 2), "val_lo": (2, np.float32, 1),
+                    "row_order": (3, np.int32, 1), "long_rows": (4, np.int32, 1), "long_seg_ptr": (5, np.int32, 1),
+                    "segs": (6, np.int32, 4)}
+
+    def debug_graph(self, plane: str) -> np.ndarray:
+        """A copy of one plane of the loaded graph (``hrag_debug_graph``): cv as [nnz, 2] int32 {col, fp32 bits},
+        segs as [n_seg, 4] int32, every other plane 1-D."""
+        which, dtype, width = self.GRAPH_PLANES[plane]
+        n = C.c_int64()
+        _lib.check(self._lib.hrag_debug_graph(self._h, which, None, 0, C.byref(n)))
+        buf = np.empty(n.value // np.dtype(dtype).itemsize, dtype=dtype)
+        _lib.check(self._lib.hrag_debug_graph(self._h, which, _ptr(buf), n.value, C.byref(n)))
+        return buf.reshape(-1, width) if width > 1 else buf
 
 
 FactFilter = Callable[[int, Sequence[int], Sequence[float]], Sequence[int]]

@@ -76,7 +76,7 @@ int hrag_comm_init(hrag_t* h, const void* id128, int rank, int world);
 
 /* Optional, before the graph load: rank r owns rows [bounds[r], bounds[r + 1]) (bounds[0] = 0, bounds[world] = N) instead
  * of equal row counts -- a partition balanced by work (non-zeros + 4 per row) keeps the ranks in step when some row
- * ranges are much denser than others (the passage rows).  hrag_load_graph_coo derives it by itself (every rank sees the
+ * ranges are much denser than others (the passage rows).  The COO loaders derive it by themselves (every rank sees the
  * whole edge list); a caller of hrag_load_graph_csr passes it explicitly. */
 int hrag_comm_set_row_bounds(hrag_t* h, const int64_t* bounds, int world);
 
@@ -106,11 +106,21 @@ int hrag_load_graph_csr_f64(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t 
 /* Same graph from the igraph-style undirected multigraph edge list itself
  * (graph.get_edgelist() + graph.es["weight"]): every edge (src, dst, w) contributes w to W[src,dst]
  * and W[dst,src]; parallel edges sum (add_fact_edges emits (s,o) and (o,s), HippoRAG.py:907-910);
- * edges with w <= 0 carry nothing; columns are divided by the vertex strength.  The library builds
- * the CSR on the host (no scipy needed by a C caller).  With node-range sharding every rank passes
- * the full edge list and keeps its own row range. */
+ * edges with w <= 0 carry nothing; columns are divided by the vertex strength.  The endpoints are
+ * checked on the host; the library then uploads the list and builds the CSR on the GPU (no scipy
+ * needed by a C caller), byte for byte what a sequential build gives: parallel edges summed in input
+ * order, strengths summed in column order, fp64 division.  The graph keeps the fp64 lo plane of
+ * hrag_load_graph_csr_f64.  With node-range sharding every rank passes the full edge list and keeps
+ * its own row range.  Scratch while it runs: about 100 bytes of device memory per edge. */
 int hrag_load_graph_coo(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32_t* src, const int32_t* dst,
                         const double* w);
+
+/* Same as hrag_load_graph_coo from an edge list already in this handle's GPU memory (device pointers,
+ * n_edges entries each, ready to read: the caller has synchronised the stream that wrote them).  The
+ * endpoints are checked on the device; a rejected list leaves the handle as it was.  Nothing is kept
+ * from the arrays once the call returns. */
+int hrag_load_graph_coo_device(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32_t* d_src,
+                               const int32_t* d_dst, const double* d_w);
 
 /* Integer tables equivalent to the dicts prepare_retrieval_objects builds
  * (HippoRAG.py:1287-1389): passage_vid[p] = passage_node_idxs[p] (:1333);
@@ -232,6 +242,11 @@ int hrag_reset_stats(hrag_t* h);
 /* Raw device buffers for tests/benchmarks: which = 0 fact scores of the last stage A
  * sub-batch, 1 passage scores of the last stage B sub-batch. */
 int hrag_debug_copy(hrag_t* h, int which, float* host_out, int64_t max_elems, int64_t* n_written);
+/* One plane of the loaded graph, byte for byte (tests compare the ingest planes): plane = 0 row_ptr int32[n_rows + 1],
+ * 1 cv int2[nnz], 2 val_lo fp32[nnz] (empty without the fp64 operator), 3 row_order int32[n_rows], 4 long_rows
+ * int32[n_long], 5 long_seg_ptr int32[n_long + 1] (empty when n_long = 0), 6 segs int4[n_seg].  *n_written = the
+ * plane's size in bytes; host_out = NULL only reports it. */
+int hrag_debug_graph(hrag_t* h, int plane, void* host_out, int64_t max_bytes, int64_t* n_written);
 /* keep != 0: stage A materialises the fact score matrix even in the tensor-core modes (whose
  * default epilogue selects min/max/top-k in registers and never writes scores). */
 int hrag_debug_keep_scores(hrag_t* h, int keep);
