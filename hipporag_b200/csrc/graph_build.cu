@@ -293,8 +293,6 @@ int install_graph(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, in
                                                                g.long_seg_ptr, g.segs);
         HRAG_TRY(m.seg_partial.ensure((size_t)g.n_seg * g.max_batch * sizeof(float)));
         g.seg_partial = m.seg_partial.as<float>();
-        if (val64) HRAG_TRY(m.seg_partial64.ensure((size_t)g.n_seg * 16 * sizeof(double)));
-        g.seg_partial64 = m.seg_partial64.as<double>();
     }
     HRAG_CUDA(cudaGetLastError());
     HRAG_CUDA(cudaStreamSynchronize(st));

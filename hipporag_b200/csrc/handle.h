@@ -89,7 +89,7 @@ enum Stage { ST_SIM_FACT = 0, ST_SEL_FACT, ST_SIM_PASS, ST_SEED, ST_PPR, ST_TOPK
 struct Span { int stage; cudaEvent_t a, b; };
 
 // Storage behind the views the kernel launchers take (PprGraph g, SeedTables t), filled in by ingest.cu
-struct GraphMem { Buf row_ptr, cv, row_order, long_rows, long_seg_ptr, segs, seg_partial, val_lo, seg_partial64; };
+struct GraphMem { Buf row_ptr, cv, row_order, long_rows, long_seg_ptr, segs, seg_partial, val_lo; };
 struct TableMem { Buf passage_vid, fact_subj_vid, fact_obj_vid, ent_chunk_count; };
 struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passages)
     const float* f32 = nullptr;   // fp32 rows: borrowed from the caller (device upload, caller keeps it alive) or own

@@ -1,5 +1,6 @@
 // Launchers of the hand-written sm_90a kernels (K1..K4).  Host-callable C++; the C ABI in
 // api.cu / solve.cu / ingest.cu / comm.cu composes them.  All pointers are device pointers; all launches go to `stream`.
+// The three PPR sweeps (K1 fp32, K1m fp16, K1d fp64) share one CSR sweep skeleton, sweep.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -24,13 +25,12 @@ struct PprGraph {
     int* long_seg_ptr = nullptr;  // [n_long + 1] offsets into segs
     int n_seg = 0;
     int4* segs = nullptr;         // [n_seg] {local row, begin, end, 0}
-    float* seg_partial = nullptr; // [n_seg * Bmax]
+    float* seg_partial = nullptr; // [n_seg * Bmax] segment partials of every sweep (fp16 and fp64 use part of a row)
     int max_batch = 0;
     int num_sms = 132;
     int* row_order = nullptr;     // [n_rows] fp16 sweep: rows of each 64-row CTA block sorted by length (desc)
     // fp64 operator (graphs loaded from float64 values only; null otherwise): P = hi + lo to ~2^-48 relative
     float* val_lo = nullptr;        // [nnz] fp32(P64 - hi), hi = the fp32 value in cv
-    double* seg_partial64 = nullptr; // [n_seg * 16] fp64 segment partials of the residual sweep
 };
 
 // One sweep  y[i,:] = w * (alpha * sum_j P[i,j] x[j,:] + v[i,:]) + (1 - w) * prev[i,:]

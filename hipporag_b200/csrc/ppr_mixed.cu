@@ -15,8 +15,8 @@
 // left behind: its column sums give the residual check of the solve for free.
 //
 // Layout: half state [N, 32] row-major (64 B per row); a group of 4 lanes owns a row, each lane
-// 8 columns (one 16-byte load per gathered row per lane).  Rows > long_thresh use the same
-// segment scheme as K1.
+// 8 columns (one 16-byte load per gathered row per lane; sweep.cuh LaneF16).  Rows > long_thresh
+// go through K1's segment kernel body and fixed-order finalize sum (sweep.cuh), 4 gathers in flight.
 //
 // Right-hand side.  The reset vector of graph_search_with_fact_entities (HippoRAG.py:1544-1656)
 // is non-zero only on the P passage vertices and on <= link_top_k phrase vertices per query, so
@@ -35,31 +35,18 @@
 // NVLink; the epoch handshake that replaces a collective is folded into the sweep itself: every
 // CTA starts by polling the local flag words (ld.relaxed.sys), the last CTA of the persistent
 // grid to finish publishes this rank's epoch to the peers (st.release.sys) -- no extra launches.
-#include <cuda_fp16.h>
-
 #include <algorithm>
 
-#include "common.cuh"
-#include "kernels.h"
+#include "sweep.cuh"
 
 namespace hrag {
 
 namespace {
 
-constexpr int kThreads = 256;
 constexpr int kLPR = 4;                 // lanes per row
 constexpr int kGPB = kThreads / kLPR;   // rows per CTA
 constexpr int kB = 32;                  // batch width of the mixed solver
 
-__device__ __forceinline__ void h8_to_f(const uint4& u, float (&f)[8]) {
-    const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const float2 a = __half22float2(h[j]);
-        f[2 * j] = a.x;
-        f[2 * j + 1] = a.y;
-    }
-}
 __device__ __forceinline__ float sat_h(float x) { return fminf(fmaxf(x, -65504.f), 65504.f); }
 __device__ __forceinline__ uint4 f_to_h8(const float (&f)[8]) {
     uint4 u;
@@ -67,12 +54,6 @@ __device__ __forceinline__ uint4 f_to_h8(const float (&f)[8]) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) h[j] = __floats2half2_rn(sat_h(f[2 * j]), sat_h(f[2 * j + 1]));
     return u;
-}
-__device__ __forceinline__ void fma8(float (&acc)[8], float a, const uint4& u) {
-    float f[8];
-    h8_to_f(u, f);
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = fmaf(a, f[j], acc[j]);
 }
 
 // predicated forms: `ok == false` yields zeros without touching memory (the ragged end of a row is a predicated batch)
@@ -212,6 +193,8 @@ __device__ __forceinline__ void row_epilogue_h(float (&acc)[8], int row, int lan
     }
 }
 
+// The same sums as sweep.cuh's block_colsum<LaneF16, 4>, kept here because nvcc schedules k_sweep_h / k_sweep_h_push
+// differently through the shared one; their code stays as it is measured.
 __device__ __forceinline__ void block_colsum_h(float (&v)[8], float* __restrict__ partial_row) {
     __shared__ float s_sum[kThreads / 32][kB];
 #pragma unroll
@@ -352,35 +335,15 @@ k_sweep_h_push(const SweepArgs a, const PeerOut peers, const SweepSync sy) {
 
 __global__ void __launch_bounds__(kThreads)
 k_sweep_long_segments_h(int n_seg, const int4* __restrict__ segs, const int2* __restrict__ cv,
-                        const uint4* __restrict__ xh, float* __restrict__ seg_partial /* [n_seg, 32] */,
-                        const SweepSync sy) {
+                        const uint4* __restrict__ xh, F8* __restrict__ seg_partial, const SweepSync sy) {
     sync_wait(sy);
-    constexpr int G = 32 / kLPR;
-    const int warp = (blockIdx.x * kThreads + threadIdx.x) >> 5;
-    if (warp >= n_seg) return;
-    const int lane = threadIdx.x & 31;
-    const int g = lane / kLPR, l = lane % kLPR;
-    const int4 sg = __ldg(segs + warp);
-    float acc[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-    for (int i = sg.y + g; i < sg.z; i += G) {
-        const int2 c = __ldg(cv + i);
-        fma8(acc, __int_as_float(c.y), __ldg(xh + (size_t)c.x * kLPR + l));
-    }
-#pragma unroll
-    for (int off = kLPR; off < 32; off <<= 1)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], off);
-    if (lane < kLPR)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) seg_partial[(size_t)warp * kB + lane * 8 + j] = acc[j];
+    segment_partial<LaneF16, kLPR>(n_seg, segs, cv, nullptr, xh, seg_partial);
 }
 
 template <bool CHEB, int MODE, bool FINAL>
 __global__ void __launch_bounds__(kThreads)
 k_sweep_long_finalize_h(int n_long, const int* __restrict__ long_rows, const int* __restrict__ long_seg_ptr,
-                        const float* __restrict__ seg_partial, const SweepArgs a, const PeerOut peers,
+                        const F8* __restrict__ seg_partial, const SweepArgs a, const PeerOut peers,
                         const SweepSync sy) {
     const int g = threadIdx.x / kLPR, l = threadIdx.x % kLPR;
     const int k = blockIdx.x * kGPB + g;
@@ -389,14 +352,9 @@ k_sweep_long_finalize_h(int n_long, const int* __restrict__ long_rows, const int
     for (int j = 0; j < 8; ++j) out[j] = 0.f;
     if (k < n_long) {
         const int r = __ldg(long_rows + k);
-        float acc[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-        for (int s = __ldg(long_seg_ptr + k); s < __ldg(long_seg_ptr + k + 1); ++s)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) acc[j] += seg_partial[(size_t)s * kB + l * 8 + j];
+        F8 acc = segment_sum<LaneF16, kLPR>(long_seg_ptr, k, seg_partial + l);
         uint4 packed;
-        row_epilogue_h<CHEB, MODE>(acc, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh, a.prevh,
+        row_epilogue_h<CHEB, MODE>(acc.v, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh, a.prevh,
                                    a.yh, a.alpha, a.w, a.t, peers, a.overflow, out, packed);
     }
     if (FINAL) block_colsum_h(out, a.partials + (size_t)blockIdx.x * kB);
@@ -620,9 +578,7 @@ k_state_to_scores_mixed(const __half* __restrict__ X0, const __half* __restrict_
 
 }  // namespace
 
-int mixed_partial_rows(const PprGraph& g) {
-    return (int)ceil_div(g.n_rows, kGPB) + (g.n_long ? (int)ceil_div(g.n_long, kGPB) : 0);
-}
+int mixed_partial_rows(const PprGraph& g) { return sweep_partial_rows(g, kGPB); }
 
 int epoch_wait(const SweepSync& sync, cudaStream_t st) {
     k_epoch_wait<<<1, 32, 0, st>>>(sync);
@@ -644,9 +600,8 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
                 const float* col_scale, const void* prevh, void* yh, float alpha, float w, float t, float* partials,
                 int* n_partials, int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t st) {
     HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep: graph not loaded");
-    const bool cheb = prevh != nullptr, fin = partials != nullptr;
-    const int nb_rows = (int)ceil_div(g.n_rows, kGPB);
-    const int nb_long = g.n_long ? (int)ceil_div(g.n_long, kGPB) : 0;
+    HRAG_CHECK(kB <= g.max_batch, "mixed_sweep: segment partials too small for 32 columns");
+    const SweepGrid grid(g, kGPB);
     SweepArgs a;
     a.n_rows = g.n_rows; a.row_base = g.row_lo; a.long_thresh = g.long_thresh;
     a.row_order = g.row_order;
@@ -667,37 +622,32 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
     // staging ring is double-buffered so a block's bulk copies overlap the next block's gathers: without the second
     // buffer a CTA would sit on its slot until the TMA engine has drained its copies into a congested link.
     const bool sharded = sync.flags != nullptr;
-    const int grid_rows = sharded ? std::min(nb_rows, g.num_sms * 6) : nb_rows;
-    sy.total_ctas = (unsigned)(grid_rows + nb_long);
+    const int grid_rows = sharded ? std::min(grid.nb_rows, g.num_sms * 6) : grid.nb_rows;
+    sy.total_ctas = (unsigned)(grid_rows + grid.nb_long);
+    F8* segp = reinterpret_cast<F8*>(g.seg_partial);
     if (g.n_long) {     // only waits: the segment kernel writes no exchanged rows
-        k_sweep_long_segments_h<<<(unsigned)ceil_div((int64_t)g.n_seg * 32, kThreads), kThreads, 0, st>>>(
-            g.n_seg, g.segs, g.cv, a.xh, g.seg_partial, sy);
+        k_sweep_long_segments_h<<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, a.xh, segp, sy);
         count_launch();
     }
     SweepArgs al = a;
-    al.partials = fin ? partials + (size_t)nb_rows * kB : nullptr;
-#define HRAG_LAUNCH_H(C, M, F)                                                                                    \
-    do {                                                                                                          \
-        if (nb_rows) {                                                                                            \
-            if (sharded) k_sweep_h_push<C, M, F><<<grid_rows, kThreads, 0, st>>>(a, peers, sy);                    \
-            else k_sweep_h<C, M, F><<<grid_rows, kThreads, 0, st>>>(a);                                           \
-            count_launch();                                                                                       \
-        }                                                                                                         \
-        if (nb_long) {                                                                                            \
-            k_sweep_long_finalize_h<C, M, F><<<nb_long, kThreads, 0, st>>>(                                        \
-                g.n_long, g.long_rows, g.long_seg_ptr, g.seg_partial, al, peers, sy);                             \
-            count_launch();                                                                                       \
-        }                                                                                                         \
-    } while (0)
-    if (mode == 1 && fin) HRAG_LAUNCH_H(false, 1, true);
-    else if (mode == 1) HRAG_LAUNCH_H(false, 1, false);
-    else if (cheb && fin) HRAG_LAUNCH_H(true, 0, true);
-    else if (cheb) HRAG_LAUNCH_H(true, 0, false);
-    else if (fin) HRAG_LAUNCH_H(false, 0, true);
-    else HRAG_LAUNCH_H(false, 0, false);
-#undef HRAG_LAUNCH_H
-    if (nb_rows + nb_long == 0 && sharded) HRAG_TRY(epoch_signal(sy, st));
-    if (n_partials) *n_partials = nb_rows + nb_long;
+    al.partials = partials ? partials + (size_t)grid.nb_rows * kB : nullptr;
+    with_bools([&](auto cheb, auto resid, auto fin) {
+        if constexpr (!(cheb && resid)) {                // the residual (mode 1) has no Chebyshev form
+            constexpr int M = resid ? 1 : 0;
+            if (grid.nb_rows) {
+                if (sharded) k_sweep_h_push<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a, peers, sy);
+                else k_sweep_h<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a);
+                count_launch();
+            }
+            if (grid.nb_long) {
+                k_sweep_long_finalize_h<cheb, M, fin><<<grid.nb_long, kThreads, 0, st>>>(
+                    g.n_long, g.long_rows, g.long_seg_ptr, segp, al, peers, sy);
+                count_launch();
+            }
+        }
+    }, mode == 0 && prevh != nullptr, mode == 1, partials != nullptr);
+    if (grid.nb_rows + grid.nb_long == 0 && sharded) HRAG_TRY(epoch_signal(sy, st));
+    if (n_partials) *n_partials = grid.nb_rows + grid.nb_long;
     HRAG_CUDA(cudaGetLastError());
     return 0;
 }
