@@ -2,6 +2,7 @@
 // that stands in for the body of HippoRAG.retrieve()'s per-query loop (reference HippoRAG.py:459-480) -- batched, on
 // one H100, all intermediate state in HBM.  The handle and its HBM layout: handle.h.
 #include <algorithm>
+#include <cmath>
 #include <memory>
 
 #include "handle.h"
@@ -14,22 +15,23 @@ void set_error(const std::string& msg) { g_error = msg; }
 int64_t pad4(int64_t x) { return (x + 3) & ~(int64_t)3; }
 
 // bf16 hi / lo split of Bq queries into q_hi / q_lo, the query operand of the tensor-core kernels
-int split_queries(hrag_t* h, const float* dQ, int Bq) {
+int split_queries(hrag_t* h, const float* dQ, int Bq, cudaStream_t s) {
     const size_t n = (size_t)Bq * h->dim;
     HRAG_TRY(h->q_hi.ensure(n * 2));
     HRAG_TRY(h->q_lo.ensure(n * 2));
-    return split_bf16(dQ, (int64_t)n, h->q_hi.p, h->q_lo.p, h->stream);
+    return split_bf16(dQ, (int64_t)n, h->q_hi.p, h->q_lo.p, s);
 }
 
-int sim_dispatch(hrag_t* h, const float* dQ, int Bq, int which, float* S, int64_t ldS) {
+// n_ctas: persistent CTAs of the tensor-core GEMM (h->num_sms unless it shares the GPU with PPR sweeps)
+int sim_dispatch(hrag_t* h, const float* dQ, int Bq, int which, float* S, int64_t ldS, cudaStream_t s, int n_ctas) {
     if (h->sim_mode == HRAG_SIM_FP32 || h->emb[which].hi.p == nullptr) {   // dim % 8 != 0 has no TMA layout
         HRAG_CHECK(h->emb[which].f32 != nullptr, "similarity: the fp32 embedding matrix was not kept (streamed upload); "
                                                  "only the tensor-core modes are available");
-        return sim_fp32(dQ, Bq, h->emb[which].f32, h->emb[which].rows, h->dim, S, ldS, h->stream);
+        return sim_fp32(dQ, Bq, h->emb[which].f32, h->emb[which].rows, h->dim, S, ldS, s);
     }
-    HRAG_TRY(split_queries(h, dQ, Bq));
+    HRAG_TRY(split_queries(h, dQ, Bq, s));
     return sim_tc(h->q_hi.p, h->q_lo.p, Bq, h->emb[which].hi.p, h->emb[which].lo.p, h->emb[which].rows, h->dim,
-                  h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, S, ldS, nullptr, nullptr, h->num_sms, h->stream);
+                  h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, S, ldS, nullptr, nullptr, n_ctas, s);
 }
 
 constexpr int kFusedTopK = 8;     // candidates the GEMM epilogue / row_minmax_topk keep in registers
@@ -49,13 +51,14 @@ int64_t chunk_b(hrag_t* h) {
     return std::max<int64_t>(1, std::min<int64_t>(c, 1024));
 }
 
-// Stage A on device pointers, Bq <= chunk_a.
-int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, float* d_top_score, int* d_nvalid) {
+// Stage A on device pointers, Bq <= chunk_a, on stream s (h->stream when world > 1: the all-gathers run there).
+int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, float* d_top_score, int* d_nvalid,
+                cudaStream_t s, int n_ctas) {
     const int64_t F = h->emb[0].rows;
     if ((h->world > 1 ? h->n_facts_global : F) == 0) {   // no facts: get_fact_scores returns an empty array (HippoRAG.py:1454-1456)
-        HRAG_CUDA(cudaMemsetAsync(d_top_idx, 0xff, (size_t)Bq * k * sizeof(int), h->stream));
-        HRAG_CUDA(cudaMemsetAsync(d_top_score, 0, (size_t)Bq * k * sizeof(float), h->stream));
-        HRAG_CUDA(cudaMemsetAsync(d_nvalid, 0, (size_t)Bq * sizeof(int), h->stream));
+        HRAG_CUDA(cudaMemsetAsync(d_top_idx, 0xff, (size_t)Bq * k * sizeof(int), s));
+        HRAG_CUDA(cudaMemsetAsync(d_top_score, 0, (size_t)Bq * k * sizeof(float), s));
+        HRAG_CUDA(cudaMemsetAsync(d_nvalid, 0, (size_t)Bq * sizeof(int), s));
         return 0;
     }
     const int64_t ld = pad4(F);
@@ -65,11 +68,11 @@ int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, flo
         HRAG_TRY(h->part_mm.ensure((size_t)Bq * nt * sizeof(float2)));
         HRAG_TRY(h->part_keys.ensure((size_t)Bq * nt * 8 * sizeof(uint64_t)));
         {
-            StageTimer tm(h, ST_SIM_FACT);
-            HRAG_TRY(split_queries(h, d_qf, Bq));
+            StageTimer tm(h, ST_SIM_FACT, s);
+            HRAG_TRY(split_queries(h, d_qf, Bq, s));
             HRAG_TRY(sim_tc(h->q_hi.p, h->q_lo.p, Bq, h->emb[0].hi.p, h->emb[0].lo.p, F, h->dim,
                             h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, nullptr, 0, h->part_mm.as<float2>(),
-                            h->part_keys.as<uint64_t>(), h->num_sms, h->stream));
+                            h->part_keys.as<uint64_t>(), n_ctas, s));
         }
         if (h->world > 1) {
             // facts are sharded by row range (SURVEY.md 8(e)): local GEMM + local top-8 -> all-gather of 8 candidates
@@ -79,25 +82,25 @@ int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, flo
             float2* mm_all = h->xr_mm.as<float2>();
             uint64_t* keys_all = h->xr_keys.as<uint64_t>();
             {
-                StageTimer tm(h, ST_SEL_FACT);
+                StageTimer tm(h, ST_SEL_FACT, s);
                 HRAG_TRY(merge_minmax_topk_ex(h->part_mm.as<float2>(), h->part_keys.as<uint64_t>(), Bq, nt, nt, 1,
                                               h->fact_row_lo, F, 8, mm_all + (size_t)h->rank * Bq, nullptr, nullptr,
-                                              nullptr, keys_all + (size_t)h->rank * Bq * 8, h->stream));
+                                              nullptr, keys_all + (size_t)h->rank * Bq * 8, s));
             }
             {
-                StageTimer tc(h, ST_COMM);
+                StageTimer tc(h, ST_COMM, s);
                 HRAG_NCCL(g_nccl.AllGather(mm_all + (size_t)h->rank * Bq, mm_all, (size_t)Bq * sizeof(float2), ncclInt8,
-                                           h->comm, h->stream));
+                                           h->comm, s));
                 HRAG_NCCL(g_nccl.AllGather(keys_all + (size_t)h->rank * Bq * 8, keys_all, (size_t)Bq * 8 * sizeof(uint64_t),
-                                           ncclInt8, h->comm, h->stream));
+                                           ncclInt8, h->comm, s));
             }
-            StageTimer tm(h, ST_SEL_FACT);
+            StageTimer tm(h, ST_SEL_FACT, s);
             HRAG_TRY(merge_minmax_topk_ex(mm_all, keys_all, Bq, h->world, 1, Bq, 0, h->n_facts_global, k,
-                                          h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, nullptr, h->stream));
+                                          h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, nullptr, s));
         } else {
-            StageTimer tm(h, ST_SEL_FACT);
+            StageTimer tm(h, ST_SEL_FACT, s);
             HRAG_TRY(merge_minmax_topk(h->part_mm.as<float2>(), h->part_keys.as<uint64_t>(), Bq, nt, F, k,
-                                       h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, h->stream));
+                                       h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, s));
         }
         h->last_fact_rows = 0;
         return 0;
@@ -106,41 +109,50 @@ int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, flo
                               "(the fact rows are sharded; the fp32 / materialised paths are single-GPU)");
     HRAG_TRY(h->S_fact.ensure((size_t)Bq * ld * sizeof(float)));
     {
-        StageTimer tm(h, ST_SIM_FACT);
-        HRAG_TRY(sim_dispatch(h, d_qf, Bq, 0, h->S_fact.as<float>(), ld));
+        StageTimer tm(h, ST_SIM_FACT, s);
+        HRAG_TRY(sim_dispatch(h, d_qf, Bq, 0, h->S_fact.as<float>(), ld, s, n_ctas));
     }
     {
-        StageTimer tm(h, ST_SEL_FACT);
+        StageTimer tm(h, ST_SEL_FACT, s);
         if (k <= kFusedTopK) {
             HRAG_TRY(row_minmax_topk(h->S_fact.as<float>(), Bq, F, ld, k, h->mm_fact.as<float2>(), d_top_idx,
-                                     d_top_score, d_nvalid, h->stream));
+                                     d_top_score, d_nvalid, s));
         } else {   // linking_top_k > 8 (config_utils.py:184): exact radix select on the materialised scores
             HRAG_TRY(row_minmax_topk(h->S_fact.as<float>(), Bq, F, ld, 0, h->mm_fact.as<float2>(), nullptr, nullptr,
-                                     nullptr, h->stream));
-            HRAG_TRY(row_topk(h->S_fact.as<float>(), Bq, F, ld, k, d_top_idx, d_top_score, h->stream));
-            HRAG_TRY(topk_normalize(Bq, k, F, h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, h->stream));
+                                     nullptr, s));
+            HRAG_TRY(row_topk(h->S_fact.as<float>(), Bq, F, ld, k, d_top_idx, d_top_score, s));
+            HRAG_TRY(topk_normalize(Bq, k, F, h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, s));
         }
     }
     h->last_fact_rows = Bq;
     return 0;
 }
 
-// Stage B on device pointers, Bq <= chunk_b.
-int dev_stage_b(hrag_t* h, int Bq, const float* d_qp, const int* d_kept_idx, const float* d_kept_score,
-                int k_facts, const uint8_t* d_dpr, float damping, float pnw, int link_top_k, int topk,
-                int iters_arg, float tol_arg, int* d_out_ids, float* d_out_scores) {
+// Stage B's similarity part on stream s, Bq <= chunk_b: passage scores into S_buf [Bq, pad4(P)] and their per-row
+// (min, max) into mm_buf.
+int dev_stage_b_sim(hrag_t* h, int Bq, const float* d_qp, hrag::Buf& S_buf, hrag::Buf& mm_buf, cudaStream_t s,
+                    int n_ctas) {
     const int P = h->t.n_passages;
     HRAG_CHECK(P > 0, "stage B: no passages loaded");
     const int64_t ld = pad4(P);
-    HRAG_TRY(h->S_pass.ensure((size_t)Bq * ld * sizeof(float)));
-    HRAG_TRY(h->mm_pass.ensure((size_t)Bq * sizeof(float2)));
+    HRAG_TRY(S_buf.ensure((size_t)Bq * ld * sizeof(float)));
+    HRAG_TRY(mm_buf.ensure((size_t)Bq * sizeof(float2)));
+    StageTimer tm(h, ST_SIM_PASS, s);
+    HRAG_TRY(sim_dispatch(h, d_qp, Bq, 1, S_buf.as<float>(), ld, s, n_ctas));
+    HRAG_TRY(row_minmax_topk(S_buf.as<float>(), Bq, P, ld, 0, mm_buf.as<float2>(), nullptr, nullptr, nullptr, s));
+    h->last_pass_S = &S_buf;
+    h->last_pass_rows = Bq;
+    return 0;
+}
+
+// Stage B's solve part on `stream`: seeds -> PPR -> top-k over the scores S / mm_pass of dev_stage_b_sim (the PPR
+// scores are gathered into S in place).
+int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d_kept_idx, const float* d_kept_score,
+                      int k_facts, const uint8_t* d_dpr, float damping, float pnw, int link_top_k, int topk,
+                      int iters_arg, float tol_arg, int* d_out_ids, float* d_out_scores) {
+    const int P = h->t.n_passages;
+    const int64_t ld = pad4(P);
     HRAG_TRY(h->mode.ensure((size_t)Bq * sizeof(int)));
-    float* S = h->S_pass.as<float>();
-    {
-        StageTimer tm(h, ST_SIM_PASS);
-        HRAG_TRY(sim_dispatch(h, d_qp, Bq, 1, S, ld));
-        HRAG_TRY(row_minmax_topk(S, Bq, P, ld, 0, h->mm_pass.as<float2>(), nullptr, nullptr, nullptr, h->stream));
-    }
     const SweepPlan plan = plan_sweeps(h, damping, iters_arg, tol_arg, h->ppr_precision == HRAG_PPR_MIXED && Bq > 16);
     const bool mixed = plan.mixed;
     const int Bp = mixed ? 32 : round_batch(std::min(h->ppr_batch, Bq));
@@ -155,7 +167,7 @@ int dev_stage_b(hrag_t* h, int Bq, const float* d_qp, const int* d_kept_idx, con
     }
     if (k_facts == 0) {   // retrieve_dpr (HippoRAG.py:665-732): every query is a DPR query, no PPR at all
         StageTimer tm(h, ST_TOPK);
-        HRAG_TRY(minmax_apply(S, Bq, P, ld, h->mm_pass.as<float2>(), h->stream));
+        HRAG_TRY(minmax_apply(S, Bq, P, ld, mm_pass, h->stream));
     }
     if (mixed && k_facts > 0) {
         // Two streams: stream2 builds sub-batch i+1's compact right-hand side (passage weights + phrase seeds on
@@ -173,7 +185,7 @@ int dev_stage_b(hrag_t* h, int Bq, const float* d_qp, const int* d_kept_idx, con
             double* vsum = h->sums.as<double>() + kSumV + 32 * set;
             int* slot_map = h->slot_map[set].as<int>();
             if (it >= 2) HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_released[set], 0));   // set is free again
-            HRAG_TRY(compact_prepare_rhs(h->t, nb, q0, S, ld, h->mm_pass.as<float2>(), pnw, kSeedSlots,
+            HRAG_TRY(compact_prepare_rhs(h->t, nb, q0, S, ld, mm_pass, pnw, kSeedSlots,
                                          h->seed_vid.as<int>(), h->seed_w.as<float>(), damping, slot_map,
                                          h->slot_vid[set].as<int>(), h->Vc[set].as<float>(), h->R16[set].p, x0,
                                          (int64_t)h->g.n_global, h->prep_scratch.as<float>(), vsum, scale, h->stream2));
@@ -186,7 +198,7 @@ int dev_stage_b(hrag_t* h, int Bq, const float* d_qp, const int* d_kept_idx, con
                 StageTimer tm(h, ST_TOPK);
                 HRAG_TRY(gather_passage_scores_mixed(h->t, nb, q0, X0, D, 1.f / kMixedT, h->sums.as<double>(),
                                                      h->sums.as<double>() + 32, h->mode.as<int>(),
-                                                     h->mm_pass.as<float2>(), S, ld, h->stream));
+                                                     mm_pass, S, ld, h->stream));
                 HRAG_TRY(compact_release_slots(P, nb, q0, kSeedSlots, h->seed_vid.as<int>(), slot_map, h->stream));
             }
             HRAG_TRY(p2p_signal(h));   // peers may overwrite this rank's state buffers from here on
@@ -199,7 +211,7 @@ int dev_stage_b(hrag_t* h, int Bq, const float* d_qp, const int* d_kept_idx, con
         {
             StageTimer tm(h, ST_SEED);
             HRAG_CUDA(cudaMemsetAsync(h->V.p, 0, (size_t)h->g.n_global * Bp * sizeof(float), h->stream));
-            HRAG_TRY(seed_passages(h->t, Bp, nb, S, ld, q0, h->mm_pass.as<float2>(), pnw, h->V.as<float>(), h->stream));
+            HRAG_TRY(seed_passages(h->t, Bp, nb, S, ld, q0, mm_pass, pnw, h->V.as<float>(), h->stream));
             HRAG_TRY(seed_scatter(Bp, nb, q0, h->seed_vid.as<int>(), h->seed_w.as<float>(), h->V.as<float>(),
                                   h->stream));
         }
@@ -207,14 +219,32 @@ int dev_stage_b(hrag_t* h, int Bq, const float* d_qp, const int* d_kept_idx, con
         HRAG_TRY(dev_ppr(h, Bp, plan.iters, damping, &Z));
         StageTimer tm(h, ST_TOPK);
         HRAG_TRY(gather_passage_scores(h->t, Bp, nb, q0, Z, h->sums.as<double>(), h->mode.as<int>(),
-                                       h->mm_pass.as<float2>(), S, ld, h->stream));
+                                       mm_pass, S, ld, h->stream));
     }
     {
         StageTimer tm(h, ST_TOPK);
         HRAG_TRY(row_topk(S, Bq, P, ld, topk, d_out_ids, d_out_scores, h->stream));
     }
-    h->last_pass_rows = Bq;
     return 0;
+}
+
+// Persistent CTAs of the similarity GEMMs of chunk c + 1 while they share the GPU with chunk c's PPR sweeps in
+// hrag_retrieve_resident: enough SMs that the GEMMs finish within the sweeps, the rest stay with the sweeps (which
+// are bound by DRAM latency, not by SMs: on 132 - 56 SMs a K1m sweep takes 0.488 ms instead of 0.422).
+// Work per chunk of Bq queries: GEMM 2 n_seg Bq (F + P) dim FLOP, sweeps (non-zeros x sweeps per sub-batch x
+// sub-batches).  Rates measured at C3 on an H100 SXM (132 SMs, 700 W): K1m alone 34.4 G non-zeros/s (14.5 M in
+// 0.422 ms per sweep); K2 next to the sweeps 1.56 TFLOP/s per SM -- half its rate alone (3.0), as its TMA operand
+// loads queue behind the sweeps' gathers.  At C3 the rule gives 54; 48 and 56 measured the same step time, 40 and
+// 66 slower.
+int overlap_ctas(const hrag_t* h, int Bq, const SweepPlan& plan) {
+    constexpr double kGemmFlopPerSmMs = 1.56e9, kSweepNnzPerMs = 3.44e7;
+    const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
+    const double gemm_flop = 2.0 * n_seg * Bq * (double)(h->emb[0].rows + h->emb[1].rows) * h->dim;
+    const int64_t sweeps = plan.mixed ? (int64_t)(plan.m1 + 1 + plan.m2) * ceil_div(Bq, 32)
+                                      : (int64_t)plan.iters * ceil_div(Bq, round_batch(std::min(h->ppr_batch, Bq)));
+    const double t_sweep = (double)sweeps * (double)h->g.nnz / kSweepNnzPerMs;
+    const int g = (int)std::ceil(gemm_flop / (kGemmFlopPerSmMs * std::max(t_sweep, 1e-9)));
+    return std::min(std::max(g, 1), h->num_sms / 2);
 }
 
 }  // namespace hrag
@@ -248,11 +278,19 @@ int hrag_create(const int* device_ids, int n_devices, int shard_mode, hrag_t** o
     h->num_sms = prop.multiProcessorCount;
     HRAG_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     HRAG_CUDA(cudaStreamCreateWithFlags(&h->stream2, cudaStreamNonBlocking));
+    // highest priority: the similarity GEMMs' persistent CTAs take their SMs as soon as a sweep grid drains, instead of
+    // queueing behind the next sweep's grid
+    int prio_least = 0, prio_greatest = 0;
+    HRAG_CUDA(cudaDeviceGetStreamPriorityRange(&prio_least, &prio_greatest));
+    HRAG_CUDA(cudaStreamCreateWithPriority(&h->stream_sim, cudaStreamNonBlocking, prio_greatest));
     for (int i = 0; i < 2; ++i) {
         HRAG_CUDA(cudaEventCreateWithFlags(&h->ev_ready[i], cudaEventDisableTiming));
         HRAG_CUDA(cudaEventCreateWithFlags(&h->ev_released[i], cudaEventDisableTiming));
+        HRAG_CUDA(cudaEventCreateWithFlags(&h->ev_sim_ready[i], cudaEventDisableTiming));
+        HRAG_CUDA(cudaEventCreateWithFlags(&h->ev_sim_consumed[i], cudaEventDisableTiming));
     }
     HRAG_CUDA(cudaEventCreateWithFlags(&h->ev_inputs, cudaEventDisableTiming));
+    HRAG_CUDA(cudaEventCreateWithFlags(&h->ev_sim_start, cudaEventDisableTiming));
     *out = h.release();
     return 0;
 }
@@ -261,13 +299,16 @@ void hrag_destroy(hrag_t* h) {
     if (!h) return;
     cudaSetDevice(h->device);
     cudaStreamSynchronize(h->stream);
+    if (h->stream_sim) cudaStreamSynchronize(h->stream_sim);
     if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
     for (auto& c : h->solve_graphs) cudaGraphExecDestroy(c.exec);
     for (auto e : h->pool) cudaEventDestroy(e);
     for (void* p : h->peer_slab) if (p) cudaIpcCloseMemHandle(p);
-    for (cudaEvent_t e : {h->ev_ready[0], h->ev_ready[1], h->ev_released[0], h->ev_released[1], h->ev_inputs})
+    for (cudaEvent_t e : {h->ev_ready[0], h->ev_ready[1], h->ev_released[0], h->ev_released[1], h->ev_inputs,
+                          h->ev_sim_ready[0], h->ev_sim_ready[1], h->ev_sim_consumed[0], h->ev_sim_consumed[1],
+                          h->ev_sim_start})
         if (e) cudaEventDestroy(e);
-    for (cudaStream_t s : {h->stream2, h->stream}) if (s) cudaStreamDestroy(s);
+    for (cudaStream_t s : {h->stream_sim, h->stream2, h->stream}) if (s) cudaStreamDestroy(s);
     delete h;   // the buffers free themselves
 }
 
@@ -316,7 +357,7 @@ int hrag_stage_a(hrag_t* h, int32_t B, const float* q_fact, int32_t k, int32_t* 
         const int nb = (int)std::min<int64_t>(chunk, B - q0);
         HRAG_TRY(h2d(h, h->d_q.p, q_fact + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
         HRAG_TRY(dev_stage_a(h, nb, h->d_q.as<float>(), k, h->d_top_idx.as<int>() + q0 * k,
-                             h->d_top_score.as<float>() + q0 * k, h->d_nvalid.as<int>() + q0));
+                             h->d_top_score.as<float>() + q0 * k, h->d_nvalid.as<int>() + q0, h->stream, h->num_sms));
     }
     if (B > 0) {
         HRAG_TRY(d2h(h, top_idx, h->d_top_idx.p, (size_t)B * k * sizeof(int)));
@@ -368,11 +409,12 @@ int hrag_stage_b(hrag_t* h, int32_t B, const float* q_pass, const int32_t* kept_
     for (int64_t q0 = 0; q0 < B; q0 += chunk) {
         const int nb = (int)std::min<int64_t>(chunk, B - q0);
         HRAG_TRY(h2d(h, h->d_q2.p, q_pass + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
-        HRAG_TRY(dev_stage_b(h, nb, h->d_q2.as<float>(), h->d_kept_idx.as<int>() + q0 * k_facts,
-                             h->d_kept_score.as<float>() + q0 * k_facts, k_facts,
-                             dpr_only ? h->d_dpr.as<uint8_t>() + q0 : nullptr, damping, passage_node_weight,
-                             link_top_k, topk, iters, tol, h->d_out_ids.as<int>() + q0 * topk,
-                             h->d_out_scores.as<float>() + q0 * topk));
+        HRAG_TRY(dev_stage_b_sim(h, nb, h->d_q2.as<float>(), h->S_pass, h->mm_pass, h->stream, h->num_sms));
+        HRAG_TRY(dev_stage_b_solve(h, nb, h->S_pass.as<float>(), h->mm_pass.as<float2>(),
+                                   h->d_kept_idx.as<int>() + q0 * k_facts, h->d_kept_score.as<float>() + q0 * k_facts,
+                                   k_facts, dpr_only ? h->d_dpr.as<uint8_t>() + q0 : nullptr, damping,
+                                   passage_node_weight, link_top_k, topk, iters, tol,
+                                   h->d_out_ids.as<int>() + q0 * topk, h->d_out_scores.as<float>() + q0 * topk));
     }
     HRAG_TRY(d2h(h, out_ids, h->d_out_ids.p, (size_t)B * topk * sizeof(int)));
     HRAG_TRY(d2h(h, out_scores, h->d_out_scores.p, (size_t)B * topk * sizeof(float)));
@@ -390,19 +432,65 @@ int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const fl
     HRAG_TRY(check_loaded(h, "hrag_retrieve_resident", true));
     HRAG_CUDA(cudaSetDevice(h->device));
     const int64_t chunk = std::min(chunk_a(h, link_top_k), chunk_b(h));
+    const int64_t n_chunks = (B + chunk - 1) / chunk;
     const int k = link_top_k;
-    HRAG_TRY(h->d_top_idx.ensure((size_t)chunk * k * sizeof(int)));
-    HRAG_TRY(h->d_top_score.ensure((size_t)chunk * k * sizeof(float)));
-    HRAG_TRY(h->d_nvalid.ensure((size_t)chunk * sizeof(int)));
-    for (int64_t q0 = 0; q0 < B; q0 += chunk) {
-        const int nb = (int)std::min<int64_t>(chunk, B - q0);
-        HRAG_TRY(dev_stage_a(h, nb, d_q_fact + (size_t)q0 * h->dim, k, h->d_top_idx.as<int>(),
-                             h->d_top_score.as<float>(), h->d_nvalid.as<int>()));
-        // identity recognition-memory filter: the candidates are the kept facts
-        HRAG_TRY(dev_stage_b(h, nb, d_q_pass + (size_t)q0 * h->dim, h->d_top_idx.as<int>(),
-                             h->d_top_score.as<float>(), k, nullptr, damping, passage_node_weight, link_top_k,
-                             topk, iters, tol, d_out_ids + q0 * topk, d_out_scores + q0 * topk));
+    // the per-chunk state the similarity part hands to the solve part: slot 0, and slot 1 when chunks overlap
+    const bool overlap = h->world == 1 && n_chunks >= 2;
+    hrag::Buf* top_idx[2] = {&h->d_top_idx, &h->pipe.top_idx};
+    hrag::Buf* top_score[2] = {&h->d_top_score, &h->pipe.top_score};
+    hrag::Buf* nvalid[2] = {&h->d_nvalid, &h->pipe.nvalid};
+    hrag::Buf* S_pass[2] = {&h->S_pass, &h->pipe.S_pass};
+    hrag::Buf* mm_pass[2] = {&h->mm_pass, &h->pipe.mm_pass};
+    for (int s = 0; s < (overlap ? 2 : 1); ++s) {
+        HRAG_TRY(top_idx[s]->ensure((size_t)chunk * k * sizeof(int)));
+        HRAG_TRY(top_score[s]->ensure((size_t)chunk * k * sizeof(float)));
+        HRAG_TRY(nvalid[s]->ensure((size_t)chunk * sizeof(int)));
     }
+    // chunk c's similarity part on stream sim_s into slot c % 2 (stage A, then the passage GEMM + min/max)
+    auto slot = [&](int64_t c) { return overlap ? (int)(c & 1) : 0; };
+    auto similarity = [&](int64_t c, cudaStream_t sim_s, int n_ctas) -> int {
+        const int64_t q0 = c * chunk;
+        const int nb = (int)std::min<int64_t>(chunk, B - q0), s = slot(c);
+        HRAG_TRY(dev_stage_a(h, nb, d_q_fact + (size_t)q0 * h->dim, k, top_idx[s]->as<int>(), top_score[s]->as<float>(),
+                             nvalid[s]->as<int>(), sim_s, n_ctas));
+        return dev_stage_b_sim(h, nb, d_q_pass + (size_t)q0 * h->dim, *S_pass[s], *mm_pass[s], sim_s, n_ctas);
+    };
+    // chunk c's solve part on `stream` (identity recognition-memory filter: the candidates are the kept facts)
+    auto solve = [&](int64_t c) -> int {
+        const int64_t q0 = c * chunk;
+        const int nb = (int)std::min<int64_t>(chunk, B - q0), s = slot(c);
+        return dev_stage_b_solve(h, nb, S_pass[s]->as<float>(), mm_pass[s]->as<float2>(), top_idx[s]->as<int>(),
+                                 top_score[s]->as<float>(), k, nullptr, damping, passage_node_weight, link_top_k, topk,
+                                 iters, tol, d_out_ids + q0 * topk, d_out_scores + q0 * topk);
+    };
+    if (!overlap) {   // one chunk, or node-range sharding (its all-gathers and spin-waiting sweeps must not share SMs)
+        for (int64_t c = 0; c < n_chunks; ++c) {
+            HRAG_TRY(similarity(c, h->stream, h->num_sms));
+            HRAG_TRY(solve(c));
+        }
+        return resolve_spans(h);
+    }
+    // Two streams: stream_sim runs chunk c + 1's similarity GEMMs on n_ctas SMs while `stream` runs chunk c's sweeps on
+    // the others.  Every kernel computes what it computes on one stream, so the results are bit-identical.
+    const SweepPlan plan = plan_sweeps(h, damping, iters, tol, h->ppr_precision == HRAG_PPR_MIXED && chunk > 16);
+    const int n_ctas = overlap_ctas(h, (int)chunk, plan);
+    HRAG_CUDA(cudaEventRecord(h->ev_sim_start, h->stream));   // the caller's queries, ordered on `stream`
+    HRAG_CUDA(cudaStreamWaitEvent(h->stream_sim, h->ev_sim_start, 0));
+    HRAG_TRY(similarity(0, h->stream_sim, h->num_sms));        // nothing to overlap with yet: the whole GPU
+    HRAG_CUDA(cudaEventRecord(h->ev_sim_ready[0], h->stream_sim));
+    for (int64_t c = 0; c < n_chunks; ++c) {
+        const int s = (int)(c & 1);
+        if (c + 1 < n_chunks) {
+            if (c + 1 >= 2) HRAG_CUDA(cudaStreamWaitEvent(h->stream_sim, h->ev_sim_consumed[s ^ 1], 0));   // chunk c - 1 is done
+            HRAG_TRY(similarity(c + 1, h->stream_sim, n_ctas));
+            HRAG_CUDA(cudaEventRecord(h->ev_sim_ready[s ^ 1], h->stream_sim));
+        }
+        HRAG_CUDA(cudaStreamWaitEvent(h->stream, h->ev_sim_ready[s], 0));
+        HRAG_TRY(solve(c));
+        HRAG_CUDA(cudaEventRecord(h->ev_sim_consumed[s], h->stream));
+    }
+    // (the last chunk's sim_ready was the last work on stream_sim, so `stream` has joined it: the caller's events on
+    // `stream`, and resolve_spans' synchronise, cover all of the call)
     return resolve_spans(h);
 }
 int hrag_similarity(hrag_t* h, int which, int32_t B, const float* q, float* out) {
@@ -419,7 +507,7 @@ int hrag_similarity(hrag_t* h, int which, int32_t B, const float* q, float* out)
     for (int64_t q0 = 0; q0 < B; q0 += chunk) {
         const int nb = (int)std::min<int64_t>(chunk, B - q0);
         HRAG_TRY(h2d(h, h->d_q.p, q + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
-        HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld));
+        HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld, h->stream, h->num_sms));
         HRAG_TRY(row_minmax_topk(Sb.as<float>(), nb, M, ld, 0, mm.as<float2>(), nullptr, nullptr, nullptr, h->stream));
         HRAG_TRY(minmax_apply(Sb.as<float>(), nb, M, ld, mm.as<float2>(), h->stream));
         HRAG_CUDA(cudaMemcpy2DAsync(out + (size_t)q0 * M, (size_t)M * sizeof(float), Sb.p, (size_t)ld * sizeof(float),
@@ -450,7 +538,7 @@ int hrag_topk_similarity(hrag_t* h, int which, int32_t B, const float* q, int32_
         HRAG_TRY(h2d(h, h->d_q.p, q + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
         {
             StageTimer tm(h, which == 0 ? ST_SIM_FACT : ST_SIM_PASS);
-            HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld));
+            HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld, h->stream, h->num_sms));
         }
         {
             StageTimer tm(h, ST_TOPK);
@@ -488,7 +576,7 @@ int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float mi
         HRAG_CUDA(cudaMemsetAsync(d_count, 0, (size_t)nb * sizeof(int), h->stream));
         {
             StageTimer tm(h, which == 0 ? ST_SIM_FACT : ST_SIM_PASS);
-            HRAG_TRY(split_queries(h, h->d_q.as<float>(), nb));
+            HRAG_TRY(split_queries(h, h->d_q.as<float>(), nb, h->stream));
             HRAG_TRY(sim_tc_threshold(h->q_hi.p, h->q_lo.p, nb, h->emb[which].hi.p, h->emb[which].lo.p, M, h->dim,
                                       h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, min_score, h->part_keys.as<uint64_t>(),
                                       d_count, kCandidateCap, h->num_sms, h->stream));
@@ -593,7 +681,7 @@ int hrag_debug_keep_scores(hrag_t* h, int keep) {
 int hrag_debug_copy(hrag_t* h, int which, float* host_out, int64_t max_elems, int64_t* n_written) {
     HRAG_CHECK(h && host_out && n_written, "hrag_debug_copy: null argument");
     HRAG_CUDA(cudaSetDevice(h->device));
-    const hrag::Buf& b = which == 0 ? h->S_fact : h->S_pass;
+    const hrag::Buf& b = which == 0 ? h->S_fact : *h->last_pass_S;
     const int64_t rows = which == 0 ? h->last_fact_rows : h->last_pass_rows;
     const int64_t cols = which == 0 ? h->emb[0].rows : h->t.n_passages;
     const int64_t ld = pad4(cols);

@@ -12,6 +12,8 @@
 //   scores    S_pass [chunk, P] fp32; fact scores are never materialised in the fused modes (72 B per query x tile)
 // Streams: `stream` runs the similarity, the solves and the selection; `stream2` builds the compact right-hand side of
 // sub-batch i + 1 while sub-batch i is being solved.  On one GPU a sub-batch's solve is replayed as a CUDA graph.
+// `stream_sim` (highest priority) runs the similarity GEMMs of chunk c + 1 of a multi-chunk hrag_retrieve_resident
+// call while `stream` runs chunk c's solves; what it hands over lives in two slots (slot 1: `pipe`).
 #pragma once
 #include <nccl.h>
 
@@ -154,6 +156,9 @@ struct hrag_handle {
     hrag::Buf xr_mm, xr_keys;             // fact-sharded stage A: [world, Bq] min/max and [world, Bq, 8] best keys
     hrag::Buf d_q, d_q2, d_top_idx, d_top_score, d_nvalid, d_kept_idx, d_kept_score, d_dpr, d_out_ids, d_out_scores;
     hrag::Buf d_reset, d_scores;
+    // second slot of what stream_sim hands to `stream` in hrag_retrieve_resident (slot 0: d_top_*, d_nvalid,
+    // S_pass, mm_pass); allocated by the first call with two or more chunks
+    struct { hrag::Buf top_idx, top_score, nvalid, S_pass, mm_pass; } pipe;
     // CUDA graphs of the mixed solve, one per (buffer set, sweep plan, g_buf_generation)
     struct SolveGraph {
         const void *x0 = nullptr, *slot_map = nullptr, *rhs16 = nullptr, *vexact = nullptr;
@@ -170,7 +175,11 @@ struct hrag_handle {
     unsigned long long epoch = 0;             // exchange epochs signalled so far (same sequence on every rank)
     cudaStream_t stream2 = nullptr;
     cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_released[2] = {nullptr, nullptr}, ev_inputs = nullptr;
+    cudaStream_t stream_sim = nullptr;
+    // sim_ready[s]: slot s holds a chunk's stage A and passage scores; sim_consumed[s]: its solves and top-k are done
+    cudaEvent_t ev_sim_ready[2] = {nullptr, nullptr}, ev_sim_consumed[2] = {nullptr, nullptr}, ev_sim_start = nullptr;
     int64_t last_fact_rows = 0, last_pass_rows = 0;
+    const hrag::Buf* last_pass_S = &S_pass;   // the passage scores hrag_debug_copy reads (last_pass_rows rows)
 
     hrag_stats_t stats{};
     std::vector<hrag::Span> spans;
@@ -185,15 +194,17 @@ inline cudaEvent_t get_event(hrag_t* h) {
     cudaEventCreate(&e);
     return e;
 }
+// Times the work enqueued on `s` during its lifetime as one span of `stage`.  Spans on different streams may overlap.
 struct StageTimer {
-    hrag_t* h; int idx;
-    StageTimer(hrag_t* h_, int stage) : h(h_) {
-        Span s{stage, get_event(h), get_event(h)};
-        cudaEventRecord(s.a, h->stream);
-        h->spans.push_back(s);
+    hrag_t* h; cudaStream_t s; int idx;
+    StageTimer(hrag_t* h_, int stage, cudaStream_t s_) : h(h_), s(s_) {
+        Span sp{stage, get_event(h), get_event(h)};
+        cudaEventRecord(sp.a, s);
+        h->spans.push_back(sp);
         idx = (int)h->spans.size() - 1;
     }
-    ~StageTimer() { cudaEventRecord(h->spans[idx].b, h->stream); }
+    StageTimer(hrag_t* h_, int stage) : StageTimer(h_, stage, h_->stream) {}
+    ~StageTimer() { cudaEventRecord(h->spans[idx].b, s); }
 };
 
 inline int h2d(hrag_t* h, void* dst, const void* src, size_t bytes) {

@@ -463,7 +463,7 @@ int sim_tc_threshold(const void* q_hi, const void* q_lo, int Bq, const void* e_h
 }
 
 int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const void* e_lo, int64_t M, int dim,
-           int n_seg, float* S, int64_t ldS, float2* part_mm, uint64_t* part_keys, int num_sms, cudaStream_t stream) {
+           int n_seg, float* S, int64_t ldS, float2* part_mm, uint64_t* part_keys, int n_ctas, cudaStream_t stream) {
     HRAG_CHECK(dim % 8 == 0, "sim_tc: embedding dim must be a multiple of 8 (TMA row pitch)");
     HRAG_CHECK(n_seg == 1 || n_seg == 4, "sim_tc: n_seg must be 1 (bf16) or 4 (split)");
     if (Bq == 0 || M == 0) return 0;
@@ -489,7 +489,7 @@ int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const v
     p.num_m_tiles = (int)ceil_div(Bq, BM);
     p.num_n_tiles = (int)ceil_div(M, BN);
     const int64_t tiles = (int64_t)p.num_m_tiles * p.num_n_tiles;
-    const int grid = (int)std::min<int64_t>(tiles, num_sms);
+    const int grid = (int)std::min<int64_t>(tiles, std::max(n_ctas, 1));
     if (n_seg == 4 && fuse) k_sim_tc<true, 1><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
     else if (n_seg == 4) k_sim_tc<true, 0><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
     else if (fuse) k_sim_tc<false, 1><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);

@@ -188,7 +188,9 @@ int hrag_plan_sweeps(float damping, float tol, int32_t iters, int32_t batch, int
                      int32_t* mixed_sweeps1, int32_t* mixed_sweeps2, double* predicted_error);
 
 /* Whole retrieve() loop body for B queries with the identity recognition-memory filter,
- * inputs and outputs resident in HBM (device pointers): the device-timed benchmark leg. */
+ * inputs and outputs resident in HBM (device pointers): the device-timed benchmark leg.  Runs in chunks of up to
+ * 1,024 queries; on one GPU the similarity GEMMs of chunk c + 1 run on a second stream while chunk c's PPR sweeps
+ * run, with the same results as one chunk per call. */
 int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const float* d_q_pass,
                            float damping, float passage_node_weight, int32_t link_top_k,
                            int32_t topk, int32_t iters, float tol, int32_t* d_out_ids, float* d_out_scores);
@@ -233,10 +235,14 @@ int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float mi
  * compact rhs of stage B (needs hrag_load_tables). */
 int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float* ms_per_sweep);
 
-/* The CUDA stream (cudaStream_t) every kernel and copy of this handle is issued on, so a
+/* The CUDA stream (cudaStream_t) every call of this handle is ordered on: a call starts after the work already on
+ * it, and the work it runs on the handle's other streams is joined back into it before the call returns, so a
  * caller can bracket calls with its own CUDA events. */
 void* hrag_stream(hrag_t* h);
 
+/* Stage times are summed CUDA-event spans per stream.  hrag_retrieve_resident overlaps the similarity stages of
+ * one chunk of queries with the PPR of the previous chunk, so there the stage times can add up to more than the
+ * call's elapsed time. */
 int hrag_get_stats(hrag_t* h, hrag_stats_t* out);
 int hrag_reset_stats(hrag_t* h);
 /* Raw device buffers for tests/benchmarks: which = 0 fact scores of the last stage A
