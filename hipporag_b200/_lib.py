@@ -59,6 +59,7 @@ SIGNATURES = {
     "hrag_set_ppr_precision": (C.c_int, [_p, C.c_int, C.c_int, C.c_int]),
     "hrag_stage_a": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p]),
     "hrag_stage_b": (C.c_int, [_p, _i32, _p, _p, _p, _i32, _p, _f32, _f32, _i32, _i32, _i32, _f32, _p, _p]),
+    "hrag_stage_b_f64": (C.c_int, [_p, _i32, _p, _p, _p, _i32, _p, C.c_double, _f32, _i32, _i32, C.c_double, _p, _p]),
     "hrag_plan_sweeps": (C.c_int, [_f32, _f32, _i32, _i32, _p, _p, _p, _p, _p]),
     "hrag_retrieve_resident": (C.c_int, [_p, _i32, _p, _p, _f32, _f32, _i32, _i32, _i32, _f32, _p, _p]),
     "hrag_ppr": (C.c_int, [_p, _i32, _p, _f32, _i32, _f32, _p]),

@@ -13,7 +13,7 @@ What is rebound (all paths under the reference's ``src/hipporag/``):
 * ``retrieve_ircot`` (``:509-558``) -- step-synchronous: each reasoning round is one batched retrieve;
 * ``retrieve`` (``:413-499``) -- batched: stage A for all queries -> the object's own
   ``rerank_filter`` per query, unchanged, on the host (the LLM call of ``rerank.py:108``) ->
-  stage B for all queries; timers ``ppr_time`` / ``rerank_time`` / ``all_retrieval_time`` and the
+  stage B for all queries (in float64 to PRPACK's 1e-10 with ``run_ppr_fp64=True``); timers ``ppr_time`` / ``rerank_time`` / ``all_retrieval_time`` and the
   optional Recall@k evaluation behave as in the reference;
 * ``run_ppr`` (``:1709-1749``), ``dense_passage_retrieval`` (``:1467-1502``), ``get_fact_scores``
   (``:1427-1465``) -- single-call forms for code that uses them directly; ``run_ppr`` in float64 to PRPACK's
@@ -87,8 +87,10 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     the reference's ``graph.pickle`` and reuse them while the index fingerprint is unchanged (``hipporag_b200/cache.py``).
     ``run_ppr_fp64=True`` serves ``run_ppr`` (and so the reference's own ``graph_search_with_fact_entities``, which
     calls it) at PRPACK's accuracy: the float64 P is uploaded, and every call solves in float64 to ``ppr_tol``
-    (0 = 1e-10) and returns float64 scores (``Engine.ppr_f64``).  ``retrieve`` is unaffected: its reset vectors come
-    from fp32 similarity scores.
+    (0 = 1e-10) and returns float64 scores (``Engine.ppr_f64``).  ``retrieve`` -- and so ``rag_qa`` and
+    ``retrieve_ircot``, which call it -- runs stage B the same way (``Engine.stage_b_f64``): the reset vector built
+    in the reference's dtypes, float64 PPR to ``ppr_tol``, float64 ``doc_scores`` as the reference returns them.
+    ``retrieve_dpr`` has no PPR and is the same in both modes.
     ``engine_opts`` go to ``Engine.set_options``.
     """
     from hipporag.utils.misc_utils import QuerySolution
@@ -225,9 +227,10 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         # ---- stage B on the GPU (DPR fallback per query where nothing was kept, :467-469)
         ppr_start = time.time()
         topk = int(min(num_to_retrieve, 2048, max(len(self.passage_node_keys), 1)))
-        ids, scores = eng.stage_b(_query_matrix(self, queries, "passage"), kept_idx, kept_score, None,
-                                  self.global_config.damping, self.global_config.passage_node_weight,
-                                  link_top_k, topk, tol=ppr_tol)
+        stage_b = eng.stage_b_f64 if run_ppr_fp64 else eng.stage_b
+        ids, scores = stage_b(_query_matrix(self, queries, "passage"), kept_idx, kept_score, None,
+                              self.global_config.damping, self.global_config.passage_node_weight,
+                              link_top_k, topk, tol=ppr_tol)
         self.ppr_time += time.time() - ppr_start
 
         retrieval_results = []

@@ -159,11 +159,11 @@ int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d
     if (mixed) { HRAG_TRY(ensure_state_mixed(h)); HRAG_TRY(ensure_compact_rhs(h)); }
     else HRAG_TRY(ensure_state(h, Bp));
     HRAG_TRY(h->seed_vid.ensure((size_t)Bq * kSeedSlots * sizeof(int)));     // [Bq, kSeedSlots] seed slots
-    HRAG_TRY(h->seed_w.ensure((size_t)Bq * kSeedSlots * sizeof(float)));
+    HRAG_TRY(h->seed_w.ensure((size_t)Bq * kSeedSlots * sizeof(double)));
     {
         StageTimer tm(h, ST_SEED);
         HRAG_TRY(seed_entities(h->t, Bq, d_kept_idx, d_kept_score, k_facts, d_dpr, link_top_k, h->seed_vid.as<int>(),
-                               h->seed_w.as<float>(), h->mode.as<int>(), h->stream));
+                               h->seed_w.as<double>(), h->mode.as<int>(), h->stream));
     }
     if (k_facts == 0) {   // retrieve_dpr (HippoRAG.py:665-732): every query is a DPR query, no PPR at all
         StageTimer tm(h, ST_TOPK);
@@ -186,7 +186,7 @@ int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d
             int* slot_map = h->slot_map[set].as<int>();
             if (it >= 2) HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_released[set], 0));   // set is free again
             HRAG_TRY(compact_prepare_rhs(h->t, nb, q0, S, ld, mm_pass, pnw, kSeedSlots,
-                                         h->seed_vid.as<int>(), h->seed_w.as<float>(), damping, slot_map,
+                                         h->seed_vid.as<int>(), h->seed_w.as<double>(), damping, slot_map,
                                          h->slot_vid[set].as<int>(), h->Vc[set].as<float>(), h->R16[set].p, x0,
                                          (int64_t)h->g.n_global, h->prep_scratch.as<float>(), vsum, scale, h->stream2));
             HRAG_CUDA(cudaEventRecord(h->ev_ready[set], h->stream2));
@@ -212,7 +212,7 @@ int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d
             StageTimer tm(h, ST_SEED);
             HRAG_CUDA(cudaMemsetAsync(h->V.p, 0, (size_t)h->g.n_global * Bp * sizeof(float), h->stream));
             HRAG_TRY(seed_passages(h->t, Bp, nb, S, ld, q0, mm_pass, pnw, h->V.as<float>(), h->stream));
-            HRAG_TRY(seed_scatter(Bp, nb, q0, h->seed_vid.as<int>(), h->seed_w.as<float>(), h->V.as<float>(),
+            HRAG_TRY(seed_scatter(Bp, nb, q0, h->seed_vid.as<int>(), h->seed_w.as<double>(), h->V.as<float>(),
                                   h->stream));
         }
         float* Z = nullptr;
@@ -224,6 +224,53 @@ int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d
     {
         StageTimer tm(h, ST_TOPK);
         HRAG_TRY(row_topk(S, Bq, P, ld, topk, d_out_ids, d_out_scores, h->stream));
+    }
+    return 0;
+}
+
+// Stage B at PRPACK accuracy on `stream`, Bq <= chunk_b: the same seeds, the reset in the reference's dtypes (float64
+// node_weights from fp32 scores), float64 PPR by iterative refinement per sub-batch of <= 16 queries, the passage
+// scores gathered in float64 into io64 [nb, pad4(P)] and their exact top-k.  S / mm_pass (dev_stage_b_sim) are only
+// read.  *worst accumulates the residual and bound of the sub-batches solved; status 4 when one misses `target`.
+int dev_stage_b_solve_f64(hrag_t* h, int Bq, const float* S, const float2* mm_pass, const int* d_kept_idx,
+                          const float* d_kept_score, int k_facts, const uint8_t* d_dpr, double damping, float pnw,
+                          int link_top_k, int topk, double target, int* d_out_ids, double* d_out_scores,
+                          F64Refined* worst) {
+    const int P = h->t.n_passages;
+    const int N = h->g.n_global;
+    const int64_t ld = pad4(P);
+    const int Bp = round_batch(std::min(16, Bq));
+    HRAG_TRY(h->mode.ensure((size_t)Bq * sizeof(int)));
+    HRAG_TRY(ensure_state_f64(h, Bp, ld));
+    HRAG_TRY(h->seed_vid.ensure((size_t)Bq * kSeedSlots * sizeof(int)));
+    HRAG_TRY(h->seed_w.ensure((size_t)Bq * kSeedSlots * sizeof(double)));
+    {
+        StageTimer tm(h, ST_SEED);
+        HRAG_TRY(seed_entities(h->t, Bq, d_kept_idx, d_kept_score, k_facts, d_dpr, link_top_k, h->seed_vid.as<int>(),
+                               h->seed_w.as<double>(), h->mode.as<int>(), h->stream));
+    }
+    double* io = h->io64.as<double>();
+    const double* xsum = h->sums64.as<double>() + 32;
+    for (int q0 = 0; q0 < Bq; q0 += Bp) {
+        const int nb = std::min(Bp, Bq - q0);
+        if (k_facts > 0) {   // k_facts == 0 is retrieve_dpr (HippoRAG.py:665-732): every row is a DPR row, no PPR
+            {
+                StageTimer tm(h, ST_SEED);
+                HRAG_TRY(seed_reset_f64(h->t, nb, N, q0, S, ld, mm_pass, pnw, h->seed_vid.as<int>(),
+                                        h->seed_w.as<double>(), io, h->stream));
+                HRAG_TRY(reset_f64(h, Bp, nb));
+            }
+            F64Refined r;
+            HRAG_TRY(refine_f64(h, Bp, nb, damping, target, &r));
+            if (r.active) return f64_missed(h, "hrag_stage_b_f64", r, target, worst->resid, worst->bound);
+            worst->resid = std::max(worst->resid, r.resid);
+            worst->bound = std::max(worst->bound, r.bound);
+        }
+        StageTimer tm(h, ST_TOPK);
+        HRAG_TRY(gather_passage_scores_f64(h->t, Bp, nb, q0, h->X64.as<double>(), xsum, h->mode.as<int>(), mm_pass,
+                                           S, ld, io, ld, h->stream));
+        HRAG_TRY(row_topk(io, nb, P, ld, topk, d_out_ids + (size_t)q0 * topk, d_out_scores + (size_t)q0 * topk,
+                          h->stream));
     }
     return 0;
 }
@@ -245,6 +292,54 @@ int overlap_ctas(const hrag_t* h, int Bq, const SweepPlan& plan) {
     const double t_sweep = (double)sweeps * (double)h->g.nnz / kSweepNnzPerMs;
     const int g = (int)std::ceil(gemm_flop / (kGemmFlopPerSmMs * std::max(t_sweep, 1e-9)));
     return std::min(std::max(g, 1), h->num_sms / 2);
+}
+
+// tables, graph and embeddings must describe the same index (a passage matrix with more rows than passage_vid
+// would make the similarity kernel write past the score buffer)
+static int check_loaded(hrag_t* h, const char* who, bool need_facts) {
+    HRAG_CHECK(h->dim > 0 && h->g.n_global > 0 && h->t.passage_vid, std::string(who) + ": graph/tables/embeddings not loaded");
+    HRAG_CHECK(h->emb[1].rows == h->t.n_passages,
+               std::string(who) + ": passage embeddings have " + std::to_string(h->emb[1].rows) + " rows but passage_vid has " +
+                   std::to_string(h->t.n_passages));
+    HRAG_CHECK(!need_facts || h->n_facts_global == 0 || h->n_facts_global == h->t.n_facts,
+               std::string(who) + ": fact embeddings have " + std::to_string(h->n_facts_global) + " rows but the fact tables have " +
+                   std::to_string(h->t.n_facts));
+    return 0;
+}
+
+// The host-buffer form of stage B: uploads the kept facts and flags, runs each chunk of chunk_b queries through the
+// passage similarity (into S_pass / mm_pass) and solve(q0, nb, that chunk's kept facts, flags), which writes its ids
+// and score_size-byte scores into d_out_ids / d_out_scores at row q0, and copies them back.
+template <class Solve>
+static int stage_b_host(hrag_t* h, const char* who, int B, const float* q_pass, const int32_t* kept_fact_idx,
+                        const float* kept_fact_score, int k_facts, const uint8_t* dpr_only, int topk, size_t score_size,
+                        int32_t* out_ids, void* out_scores, Solve solve) {
+    HRAG_TRY(check_loaded(h, who, k_facts > 0));
+    HRAG_CUDA(cudaSetDevice(h->device));
+    const int64_t chunk = chunk_b(h);
+    const int kf = std::max(k_facts, 1);
+    HRAG_TRY(h->d_q2.ensure((size_t)std::min<int64_t>(chunk, std::max(B, 1)) * h->dim * sizeof(float)));
+    HRAG_TRY(h->d_kept_idx.ensure((size_t)std::max(B, 1) * kf * sizeof(int)));
+    HRAG_TRY(h->d_kept_score.ensure((size_t)std::max(B, 1) * kf * sizeof(float)));
+    HRAG_TRY(h->d_dpr.ensure((size_t)std::max(B, 1)));
+    HRAG_TRY(h->d_out_ids.ensure((size_t)std::max(B, 1) * topk * sizeof(int)));
+    HRAG_TRY(h->d_out_scores.ensure((size_t)std::max(B, 1) * topk * score_size));
+    if (B == 0) return resolve_spans(h);
+    if (k_facts > 0) {
+        HRAG_TRY(h2d(h, h->d_kept_idx.p, kept_fact_idx, (size_t)B * k_facts * sizeof(int)));
+        HRAG_TRY(h2d(h, h->d_kept_score.p, kept_fact_score, (size_t)B * k_facts * sizeof(float)));
+    }
+    if (dpr_only) HRAG_TRY(h2d(h, h->d_dpr.p, dpr_only, (size_t)B));
+    for (int64_t q0 = 0; q0 < B; q0 += chunk) {
+        const int nb = (int)std::min<int64_t>(chunk, B - q0);
+        HRAG_TRY(h2d(h, h->d_q2.p, q_pass + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
+        HRAG_TRY(dev_stage_b_sim(h, nb, h->d_q2.as<float>(), h->S_pass, h->mm_pass, h->stream, h->num_sms));
+        HRAG_TRY(solve(q0, nb, h->d_kept_idx.as<int>() + q0 * k_facts, h->d_kept_score.as<float>() + q0 * k_facts,
+                       dpr_only ? h->d_dpr.as<uint8_t>() + q0 : nullptr));
+    }
+    HRAG_TRY(d2h(h, out_ids, h->d_out_ids.p, (size_t)B * topk * sizeof(int)));
+    HRAG_TRY(d2h(h, out_scores, h->d_out_scores.p, (size_t)B * topk * score_size));
+    return resolve_spans(h);
 }
 
 }  // namespace hrag
@@ -367,19 +462,6 @@ int hrag_stage_a(hrag_t* h, int32_t B, const float* q_fact, int32_t k, int32_t* 
     return resolve_spans(h);
 }
 
-// tables, graph and embeddings must describe the same index (a passage matrix with more rows than passage_vid
-// would make the similarity kernel write past the score buffer)
-static int check_loaded(hrag_t* h, const char* who, bool need_facts) {
-    HRAG_CHECK(h->dim > 0 && h->g.n_global > 0 && h->t.passage_vid, std::string(who) + ": graph/tables/embeddings not loaded");
-    HRAG_CHECK(h->emb[1].rows == h->t.n_passages,
-               std::string(who) + ": passage embeddings have " + std::to_string(h->emb[1].rows) + " rows but passage_vid has " +
-                   std::to_string(h->t.n_passages));
-    HRAG_CHECK(!need_facts || h->n_facts_global == 0 || h->n_facts_global == h->t.n_facts,
-               std::string(who) + ": fact embeddings have " + std::to_string(h->n_facts_global) + " rows but the fact tables have " +
-                   std::to_string(h->t.n_facts));
-    return 0;
-}
-
 int hrag_stage_b(hrag_t* h, int32_t B, const float* q_pass, const int32_t* kept_fact_idx,
                  const float* kept_fact_score, int32_t k_facts, const uint8_t* dpr_only, float damping,
                  float passage_node_weight, int32_t link_top_k, int32_t topk, int32_t iters, float tol,
@@ -390,35 +472,38 @@ int hrag_stage_b(hrag_t* h, int32_t B, const float* q_pass, const int32_t* kept_
                "hrag_stage_b: bad sizes (at most 32 kept facts per query, topk <= 2048)");
     HRAG_CHECK(damping > 0.f && damping < 1.f, "hrag_stage_b: damping must be in (0, 1)");
     HRAG_CHECK(iters >= 0 && tol >= 0.f, "hrag_stage_b: iters and tol must be >= 0 (0 = derive from damping)");
-    HRAG_TRY(check_loaded(h, "hrag_stage_b", k_facts > 0));
-    HRAG_CUDA(cudaSetDevice(h->device));
-    const int64_t chunk = chunk_b(h);
-    const int kf = std::max(k_facts, 1);
-    HRAG_TRY(h->d_q2.ensure((size_t)std::min<int64_t>(chunk, std::max(B, 1)) * h->dim * sizeof(float)));
-    HRAG_TRY(h->d_kept_idx.ensure((size_t)std::max(B, 1) * kf * sizeof(int)));
-    HRAG_TRY(h->d_kept_score.ensure((size_t)std::max(B, 1) * kf * sizeof(float)));
-    HRAG_TRY(h->d_dpr.ensure((size_t)std::max(B, 1)));
-    HRAG_TRY(h->d_out_ids.ensure((size_t)std::max(B, 1) * topk * sizeof(int)));
-    HRAG_TRY(h->d_out_scores.ensure((size_t)std::max(B, 1) * topk * sizeof(float)));
-    if (B == 0) return resolve_spans(h);
-    if (k_facts > 0) {
-        HRAG_TRY(h2d(h, h->d_kept_idx.p, kept_fact_idx, (size_t)B * k_facts * sizeof(int)));
-        HRAG_TRY(h2d(h, h->d_kept_score.p, kept_fact_score, (size_t)B * k_facts * sizeof(float)));
-    }
-    if (dpr_only) HRAG_TRY(h2d(h, h->d_dpr.p, dpr_only, (size_t)B));
-    for (int64_t q0 = 0; q0 < B; q0 += chunk) {
-        const int nb = (int)std::min<int64_t>(chunk, B - q0);
-        HRAG_TRY(h2d(h, h->d_q2.p, q_pass + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
-        HRAG_TRY(dev_stage_b_sim(h, nb, h->d_q2.as<float>(), h->S_pass, h->mm_pass, h->stream, h->num_sms));
-        HRAG_TRY(dev_stage_b_solve(h, nb, h->S_pass.as<float>(), h->mm_pass.as<float2>(),
-                                   h->d_kept_idx.as<int>() + q0 * k_facts, h->d_kept_score.as<float>() + q0 * k_facts,
-                                   k_facts, dpr_only ? h->d_dpr.as<uint8_t>() + q0 : nullptr, damping,
-                                   passage_node_weight, link_top_k, topk, iters, tol,
-                                   h->d_out_ids.as<int>() + q0 * topk, h->d_out_scores.as<float>() + q0 * topk));
-    }
-    HRAG_TRY(d2h(h, out_ids, h->d_out_ids.p, (size_t)B * topk * sizeof(int)));
-    HRAG_TRY(d2h(h, out_scores, h->d_out_scores.p, (size_t)B * topk * sizeof(float)));
-    return resolve_spans(h);
+    return stage_b_host(h, "hrag_stage_b", B, q_pass, kept_fact_idx, kept_fact_score, k_facts, dpr_only, topk,
+                        sizeof(float), out_ids, out_scores, [&](int64_t q0, int nb, const int* d_kept_idx,
+                                                                const float* d_kept_score, const uint8_t* d_dpr) {
+        return dev_stage_b_solve(h, nb, h->S_pass.as<float>(), h->mm_pass.as<float2>(), d_kept_idx, d_kept_score,
+                                 k_facts, d_dpr, damping, passage_node_weight, link_top_k, topk, iters, tol,
+                                 h->d_out_ids.as<int>() + q0 * topk, h->d_out_scores.as<float>() + q0 * topk);
+    });
+}
+
+int hrag_stage_b_f64(hrag_t* h, int32_t B, const float* q_pass, const int32_t* kept_fact_idx,
+                     const float* kept_fact_score, int32_t k_facts, const uint8_t* dpr_only, double damping,
+                     float passage_node_weight, int32_t link_top_k, int32_t topk, double tol, int32_t* out_ids,
+                     double* out_scores) {
+    HRAG_CHECK(h && q_pass && out_ids && out_scores, "hrag_stage_b_f64: null argument");
+    HRAG_CHECK(k_facts == 0 || (kept_fact_idx && kept_fact_score), "hrag_stage_b_f64: kept facts missing");
+    HRAG_CHECK(B >= 0 && k_facts >= 0 && k_facts <= kMaxKeptFacts && topk >= 1 && topk <= 2048,
+               "hrag_stage_b_f64: bad sizes (at most 32 kept facts per query, topk <= 2048)");
+    HRAG_TRY(check_f64_call(h, "hrag_stage_b_f64", damping, tol));
+    const double target = f64_target(tol);
+    F64Refined worst;
+    worst.resid = worst.bound = 0.0;
+    HRAG_TRY(stage_b_host(h, "hrag_stage_b_f64", B, q_pass, kept_fact_idx, kept_fact_score, k_facts, dpr_only, topk,
+                          sizeof(double), out_ids, out_scores, [&](int64_t q0, int nb, const int* d_kept_idx,
+                                                                   const float* d_kept_score, const uint8_t* d_dpr) {
+        return dev_stage_b_solve_f64(h, nb, h->S_pass.as<float>(), h->mm_pass.as<float2>(), d_kept_idx, d_kept_score,
+                                     k_facts, d_dpr, damping, passage_node_weight, link_top_k, topk, target,
+                                     h->d_out_ids.as<int>() + q0 * topk, h->d_out_scores.as<double>() + q0 * topk,
+                                     &worst);
+    }));
+    h->last_rho = worst.resid;
+    h->last_bound = worst.bound;
+    return 0;
 }
 
 int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const float* d_q_pass, float damping,

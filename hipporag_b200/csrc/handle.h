@@ -136,8 +136,9 @@ struct hrag_handle {
 
     // fp32 solver state [N, B]; column-sum partials and sums, shared with the mixed solver
     hrag::Buf V, XA, XC, partials, sums;
-    // fp64 solver (hrag_ppr_f64): iterate X64 and reset V64 [N, B] fp64, host-layout staging io64 [B, N] fp64 (reset
-    // in, probabilities out), column-sum partials part64, sums64 = [vsum | rsum | xsum] x 16
+    // fp64 solver (hrag_ppr_f64, hrag_stage_b_f64): iterate X64 and reset V64 [N, B] fp64, host-layout staging io64
+    // [B, max(N, pad4(P))] fp64 (reset in; probabilities, or stage B's passage scores, out), column-sum partials
+    // part64, sums64 = [vsum | rsum | xsum] x 16
     hrag::Buf X64, V64, io64, part64, sums64;
     // mixed solver: one allocation [H0 | H1 | H2 | H3 | H0b | flags] so a single IPC handle exposes every buffer a
     // peer sweep may have to write into (K5, fused exchange for node-range sharding); H / H0b point into it
@@ -240,6 +241,25 @@ int resolve_spans(hrag_t* h);   // end of a call: checks the mixed solves, accum
 int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot_map, const float* Vexact,
                   const void* rhs16, void* x0_dense, const float* scale, const double* vsum, void** X0, void** D);
 int dev_ppr(hrag_t* h, int B, int iters, float alpha, float** result);
+
+// Float64 PPR by iterative refinement (solve.cu), shared by hrag_ppr_f64 and hrag_stage_b_f64.
+// check_f64_call: the argument / handle checks of a float64 solve, messages prefixed by `who`.
+int check_f64_call(hrag_t* h, const char* who, double damping, double tol);
+double f64_target(double tol);                       // tol 0 = 1e-10
+// state of sub-batches Bp wide; io64 holds Bp rows of max(N, io_cols)
+int ensure_state_f64(hrag_t* h, int Bp, int64_t io_cols);
+// io64 [nb, N] (host-layout reset) -> V64, h->V = fp32(V64), X64 = 0, sums64[0, Bp) = column sums of v
+int reset_f64(hrag_t* h, int Bp, int nb);
+struct F64Refined {
+    double resid = 0.0;      // max over the columns of ||r||_1 / ||v||_1 after the last round
+    double bound = 0.0;      // 2 resid / (1 - damping)
+    unsigned active = 0;     // columns whose bound still misses the target (the solve failed if any)
+};
+// Up to 4 rounds of fp32 solve + fp64 correction + fp64 residual on the state reset_f64 prepared; every column stops
+// once its own bound meets `target`.  Leaves X64 and xsum = sums64 + 32 (its column sums).
+int refine_f64(hrag_t* h, int Bp, int nb, double damping, double target, F64Refined* out);
+// End of a call whose sub-batch missed the target: stats report the call so far, error message, status 4.
+int f64_missed(hrag_t* h, const char* who, const F64Refined& r, double target, double call_resid, double call_bound);
 
 // graph_build.cu: the graph built on the device, on `stream`; both return once the device work is done.
 struct DeviceCsr { Buf row_ptr, col, val; int64_t nnz = 0; };   // int64 [N + 1], int32 [nnz], fp64 [nnz]

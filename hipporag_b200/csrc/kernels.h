@@ -87,7 +87,7 @@ int compact_rhs_partial_rows(int P);
 // pnw * minmax(S) on the passage slots, phrase weights on freshly assigned seed slots), its column sums / fp16
 // scales, rhs16 = fp16(scale * Vc), and the dense first iterate x0_dense [n_nodes, 32] fp16.
 int compact_prepare_rhs(const SeedTables& t, int nb, int q0, const float* S, int64_t ldS, const float2* minmax,
-                        float pnw, int slots_per_query, const int* seed_vid, const float* seed_w, float alpha,
+                        float pnw, int slots_per_query, const int* seed_vid, const double* seed_w, float alpha,
                         int* slot_map, int* slot_vid, float* Vc, void* rhs16, void* x0_dense, int64_t n_nodes,
                         float* partials, double* vsum, float* scale, cudaStream_t stream);
 int compact_release_slots(int P, int nb, int q0, int slots_per_query, const int* seed_vid, int* slot_map,
@@ -175,6 +175,9 @@ int minmax_apply(float* S, int rows, int64_t M, int64_t ld, const float2* minmax
 // index asc), sorted.  out_ids / out_scores are [rows, k]; missing entries (k > M) = -1 / 0.
 int row_topk(const float* S, int rows, int64_t M, int64_t ld, int k, int* out_ids, float* out_scores,
              cudaStream_t stream);
+// The same on float64 scores.
+int row_topk(const double* S, int rows, int64_t M, int64_t ld, int k, int* out_ids, double* out_scores,
+             cudaStream_t stream);
 
 // ----------------------------------------------------------------------------- K3: seeds
 constexpr int kMaxKeptFacts = 32;                       // kept facts per query (linking_top_k, config_utils.py:184)
@@ -195,12 +198,17 @@ int seed_passages(const SeedTables& t, int B, int nb, const float* S, int64_t ld
                   const float2* minmax, float pnw, float* V, cudaStream_t stream);
 // Phrase seeds of graph_search_with_fact_entities for the nq queries of a chunk: the kept facts'
 // subject/object vertices get mean(score / chunk_count), the link_top_k best survive ->
-// seed_vid / seed_w [nq, kSeedSlotsPerQuery] (-1 = unused); mode[q] = 1 (PPR) or 0 (DPR fallback: no kept fact / flagged).
+// seed_vid / seed_w [nq, kSeedSlotsPerQuery] (-1 = unused; seed_w float64, as the reference's node_weights);
+// mode[q] = 1 (PPR) or 0 (DPR fallback: no kept fact / flagged).
 int seed_entities(const SeedTables& t, int nq, const int* kept_idx, const float* kept_score, int k_facts,
-                  const uint8_t* dpr_only, int link_top_k, int* seed_vid, float* seed_w, int* mode,
+                  const uint8_t* dpr_only, int link_top_k, int* seed_vid, double* seed_w, int* mode,
                   cudaStream_t stream);
-// V[seed_vid[q0 + b, :], b] += seed_w[q0 + b, :] for b < nb.
-int seed_scatter(int B, int nb, int q0, const int* seed_vid, const float* seed_w, float* V, cudaStream_t stream);
+// V[seed_vid[q0 + b, :], b] += fp32(seed_w[q0 + b, :]) for b < nb.
+int seed_scatter(int B, int nb, int q0, const int* seed_vid, const double* seed_w, float* V, cudaStream_t stream);
+// Float64 reset of the nb queries [q0, q0 + nb) in host layout R [nb, N] (the input of reset_to_state_f64): zeroed,
+// then R[b, passage_vid[p]] = double(fp32(minmax(S[q0 + b, p])) * pnw), then R[b, seed_vid] += seed_w in float64.
+int seed_reset_f64(const SeedTables& t, int nb, int N, int q0, const float* S, int64_t ldS, const float2* minmax,
+                   float pnw, const int* seed_vid, const double* seed_w, double* R, cudaStream_t stream);
 
 // ----------------------------------------------------------------------------- K4: gather
 // PPR rows: S[q0 + b, p] = Z[passage_vid[p], b] / sums[b]; DPR-fallback rows (mode == 0):
@@ -208,6 +216,12 @@ int seed_scatter(int B, int nb, int q0, const int* seed_vid, const float* seed_w
 int gather_passage_scores(const SeedTables& t, int B, int nb, int q0, const float* Z, const double* sums,
                           const int* mode, const float2* minmax, float* S, int64_t ldS,
                           cudaStream_t stream);
+
+// Float64 form for the nb queries [q0, q0 + nb) of a sub-batch into out [nb, ld]: PPR rows X[passage_vid[p], b] /
+// xsum[b] (X [N, B] fp64), DPR-fallback rows the fp32 minmax(S[q0 + b, p]) widened (S is read, not written).
+int gather_passage_scores_f64(const SeedTables& t, int B, int nb, int q0, const double* X, const double* xsum,
+                              const int* mode, const float2* minmax, const float* S, int64_t ldS, double* out,
+                              int64_t ld, cudaStream_t stream);
 
 // Sanitise + transpose host-layout reset vectors: V[n, b] = max(R[b, n], 0) (NaN -> 0).
 int reset_to_state(const float* R, int nb, int N, int B, float* V, cudaStream_t stream);

@@ -450,7 +450,7 @@ k_rhs_passages(int P, int nb, const float* __restrict__ S, int64_t ldS, int q0, 
 // fp16 column scales.  Item i = (query b = i / slots_per_query, seed r = i % slots_per_query) owns slot P + i.
 __global__ void __launch_bounds__(1024)
 k_rhs_seeds(int P, int nb, int q0, int slots_per_query, const int* __restrict__ seed_vid,
-            const float* __restrict__ seed_w, int* __restrict__ slot_map, int* __restrict__ slot_vid,
+            const double* __restrict__ seed_w, int* __restrict__ slot_map, int* __restrict__ slot_vid,
             float* __restrict__ Vc, const float* __restrict__ partial, int n_partial, float one_minus_alpha,
             double* __restrict__ vsum, float* __restrict__ scale) {
     __shared__ double s_sum[32][33];
@@ -465,7 +465,7 @@ k_rhs_seeds(int P, int nb, int q0, int slots_per_query, const int* __restrict__ 
         if (b < nb) {
             const int v = seed_vid[(size_t)(q0 + b) * slots_per_query + r];
             if (v >= 0) {
-                const float w = seed_w[(size_t)(q0 + b) * slots_per_query + r];
+                const float w = (float)seed_w[(size_t)(q0 + b) * slots_per_query + r];
                 const int old = atomicCAS(slot_map + v, -1, P + i);
                 const int slot = old < 0 ? P + i : old;
                 if (old < 0) created = v;
@@ -678,7 +678,7 @@ int slot_map_build(int N, int P, const int* passage_vid, int* slot_map, cudaStre
 int compact_rhs_partial_rows(int P) { return (int)ceil_div(std::max(P, 1), 32); }
 
 int compact_prepare_rhs(const SeedTables& t, int nb, int q0, const float* S, int64_t ldS, const float2* minmax,
-                        float pnw, int slots_per_query, const int* seed_vid, const float* seed_w, float alpha,
+                        float pnw, int slots_per_query, const int* seed_vid, const double* seed_w, float alpha,
                         int* slot_map, int* slot_vid, float* Vc, void* rhs16, void* x0_dense, int64_t n_nodes,
                         float* partials, double* vsum, float* scale, cudaStream_t st) {
     const int P = t.n_passages;

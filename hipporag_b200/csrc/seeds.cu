@@ -29,12 +29,13 @@ constexpr int kMaxFacts = kMaxKeptFacts;         // 32 (kernels.h): linking_top_
 constexpr int kSeedSlots = kSeedSlotsPerQuery;   // a query keeps at most 2 phrases per kept fact (link_top_k = 0 keeps all)
 
 // One thread per query of the chunk: phrase weights of the kept facts -> compact seed list
-// seed_vid / seed_w [q, kSeedSlots] (unused slots: vid = -1) and mode[q] (1 = PPR, 0 = DPR fallback).
+// seed_vid / seed_w [q, kSeedSlots] (unused slots: vid = -1) and mode[q] (1 = PPR, 0 = DPR fallback).  seed_w is the
+// float64 mean the reference stores in node_weights; the fp32 solvers round it where they read it.
 __global__ void __launch_bounds__(64)
 k_seed_entities(int nq, const int* __restrict__ fact_subj, const int* __restrict__ fact_obj,
                 const int* __restrict__ chunk_count, int64_t n_facts, const int* __restrict__ kept_idx,
                 const float* __restrict__ kept_score, int k_facts, const uint8_t* __restrict__ dpr_only,
-                int link_top_k, int* __restrict__ seed_vid, float* __restrict__ seed_w, int* __restrict__ mode) {
+                int link_top_k, int* __restrict__ seed_vid, double* __restrict__ seed_w, int* __restrict__ mode) {
     const int q = blockIdx.x * 64 + threadIdx.x;
     if (q >= nq) return;
     int vid[2 * kMaxFacts];
@@ -60,7 +61,7 @@ k_seed_entities(int nq, const int* __restrict__ fact_subj, const int* __restrict
         }
     }
     const bool flagged = dpr_only != nullptr && dpr_only[q] != 0;
-    for (int r = 0; r < kSeedSlots; ++r) { seed_vid[(size_t)q * kSeedSlots + r] = -1; seed_w[(size_t)q * kSeedSlots + r] = 0.f; }
+    for (int r = 0; r < kSeedSlots; ++r) { seed_vid[(size_t)q * kSeedSlots + r] = -1; seed_w[(size_t)q * kSeedSlots + r] = 0.0; }
     if (!flagged && n_kept > 0) {
         for (int j = 0; j < n; ++j) wsum[j] /= (double)occ[j];  // :1608 mean over occurrences
         int keep = (link_top_k > 0 && link_top_k < n) ? link_top_k : n;   // :1620, :1528
@@ -72,7 +73,7 @@ k_seed_entities(int nq, const int* __restrict__ fact_subj, const int* __restrict
             }
             if (best < 0) break;
             seed_vid[(size_t)q * kSeedSlots + r] = vid[best];
-            seed_w[(size_t)q * kSeedSlots + r] = (float)wsum[best];
+            seed_w[(size_t)q * kSeedSlots + r] = wsum[best];
             occ[best] = 0;
         }
     }
@@ -83,13 +84,62 @@ k_seed_entities(int nq, const int* __restrict__ fact_subj, const int* __restrict
 
 // V[seed_vid, b] += seed_w for the nb queries of one PPR sub-batch (:1638 phrase + passage weights)
 __global__ void __launch_bounds__(256)
-k_seed_scatter(int B, int nb, int q0, const int* __restrict__ seed_vid, const float* __restrict__ seed_w,
+k_seed_scatter(int B, int nb, int q0, const int* __restrict__ seed_vid, const double* __restrict__ seed_w,
                float* __restrict__ V) {
     const int t = blockIdx.x * 256 + threadIdx.x;
     const int b = t / kSeedSlots, r = t % kSeedSlots;
     if (b >= nb) return;
     const int v = seed_vid[(size_t)(q0 + b) * kSeedSlots + r];
-    if (v >= 0) V[(size_t)v * B + b] += seed_w[(size_t)(q0 + b) * kSeedSlots + r];   // distinct (v, b) per thread
+    if (v >= 0) V[(size_t)v * B + b] += (float)seed_w[(size_t)(q0 + b) * kSeedSlots + r];   // distinct (v, b) per thread
+}
+
+// ---- the float64 reset of stage B (hrag_stage_b_f64), in the reference's dtypes -------------------------------
+// R [nb, N] is the host-layout staging reset_to_state_f64 reads (zeroed by the caller).
+// R[b, passage_vid[p]] = double(fp32(minmax(S[q0+b, p])) * fp32(pnw)): k_seed_passages' fp32 product, stored into the
+// float64 passage_weights array (HippoRAG.py:1626-1633)
+__global__ void __launch_bounds__(256)
+k_seed_passages_f64(int P, int nb, int N, const int* __restrict__ passage_vid, const float* __restrict__ S,
+                    int64_t ldS, int q0, const float2* __restrict__ minmax, float pnw, double* __restrict__ R) {
+    const int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    const int p = (int)(t / nb), b = (int)(t % nb);
+    if (p >= P) return;
+    const float2 mm = __ldg(minmax + q0 + b);
+    const float range = mm.y - mm.x;
+    const float s = __ldg(S + (size_t)(q0 + b) * ldS + p);
+    const float nrm = range == 0.f ? 1.f : __fdiv_rn(s - mm.x, range);
+    R[(size_t)b * N + __ldg(passage_vid + p)] = (double)(nrm * pnw);
+}
+
+// R[b, seed_vid] += seed_w: phrase_weights + passage_weights in float64 (:1638)
+__global__ void __launch_bounds__(256)
+k_seed_scatter_f64(int nb, int N, int q0, const int* __restrict__ seed_vid, const double* __restrict__ seed_w,
+                   double* __restrict__ R) {
+    const int t = blockIdx.x * 256 + threadIdx.x;
+    const int b = t / kSeedSlots, r = t % kSeedSlots;
+    if (b >= nb) return;
+    const int v = seed_vid[(size_t)(q0 + b) * kSeedSlots + r];
+    if (v >= 0) R[(size_t)b * N + v] += seed_w[(size_t)(q0 + b) * kSeedSlots + r];   // distinct (v, b) per thread
+}
+
+// out[b, p] (row stride ld) for the nb queries [q0, q0 + nb) of a sub-batch: PPR rows pi = X[passage_vid[p], b] /
+// xsum[b] in float64 (:1745); DPR-fallback rows the fp32 min-maxed score of k_gather_passage_scores, widened.
+__global__ void __launch_bounds__(256)
+k_gather_passage_scores_f64(int P, int B, int nb, int q0, const int* __restrict__ passage_vid,
+                            const double* __restrict__ X, const double* __restrict__ xsum, const int* __restrict__ mode,
+                            const float2* __restrict__ minmax, const float* __restrict__ S, int64_t ldS,
+                            double* __restrict__ out, int64_t ld) {
+    const int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x;
+    const int p = (int)(t / nb), b = (int)(t % nb);
+    if (p >= P) return;
+    double v;
+    if (mode[q0 + b]) {
+        v = X[(size_t)__ldg(passage_vid + p) * B + b] / xsum[b];
+    } else {
+        const float2 mm = __ldg(minmax + q0 + b);
+        const float range = mm.y - mm.x;
+        v = range == 0.f ? 1.f : __fdiv_rn(__ldg(S + (size_t)(q0 + b) * ldS + p) - mm.x, range);
+    }
+    out[(size_t)b * ld + p] = v;
 }
 
 __global__ void __launch_bounds__(256)
@@ -147,7 +197,7 @@ int seed_passages(const SeedTables& t, int B, int nb, const float* S, int64_t ld
 }
 
 int seed_entities(const SeedTables& t, int nq, const int* kept_idx, const float* kept_score, int k_facts,
-                  const uint8_t* dpr_only, int link_top_k, int* seed_vid, float* seed_w, int* mode,
+                  const uint8_t* dpr_only, int link_top_k, int* seed_vid, double* seed_w, int* mode,
                   cudaStream_t stream) {
     HRAG_CHECK(k_facts >= 0 && k_facts <= kMaxFacts, "seed_entities: at most 32 kept facts per query");
     if (nq == 0) return 0;
@@ -160,9 +210,38 @@ int seed_entities(const SeedTables& t, int nq, const int* kept_idx, const float*
     return 0;
 }
 
-int seed_scatter(int B, int nb, int q0, const int* seed_vid, const float* seed_w, float* V, cudaStream_t stream) {
+int seed_scatter(int B, int nb, int q0, const int* seed_vid, const double* seed_w, float* V, cudaStream_t stream) {
     if (nb == 0) return 0;
     k_seed_scatter<<<(unsigned)ceil_div(nb * kSeedSlots, 256), 256, 0, stream>>>(B, nb, q0, seed_vid, seed_w, V);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int seed_reset_f64(const SeedTables& t, int nb, int N, int q0, const float* S, int64_t ldS, const float2* minmax,
+                   float pnw, const int* seed_vid, const double* seed_w, double* R, cudaStream_t stream) {
+    if (nb == 0) return 0;
+    HRAG_CUDA(cudaMemsetAsync(R, 0, (size_t)nb * N * sizeof(double), stream));
+    if (t.n_passages > 0) {
+        const int64_t total = (int64_t)t.n_passages * nb;
+        k_seed_passages_f64<<<(unsigned)ceil_div(total, 256), 256, 0, stream>>>(t.n_passages, nb, N, t.passage_vid, S,
+                                                                                 ldS, q0, minmax, pnw, R);
+        count_launch(1);
+    }
+    k_seed_scatter_f64<<<(unsigned)ceil_div(nb * kSeedSlots, 256), 256, 0, stream>>>(nb, N, q0, seed_vid, seed_w, R);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int gather_passage_scores_f64(const SeedTables& t, int B, int nb, int q0, const double* X, const double* xsum,
+                              const int* mode, const float2* minmax, const float* S, int64_t ldS, double* out,
+                              int64_t ld, cudaStream_t stream) {
+    if (t.n_passages == 0 || nb == 0) return 0;
+    const int64_t total = (int64_t)t.n_passages * nb;
+    k_gather_passage_scores_f64<<<(unsigned)ceil_div(total, 256), 256, 0, stream>>>(t.n_passages, B, nb, q0,
+                                                                                     t.passage_vid, X, xsum, mode,
+                                                                                     minmax, S, ldS, out, ld);
     count_launch(1);
     HRAG_CUDA(cudaGetLastError());
     return 0;

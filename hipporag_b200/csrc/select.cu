@@ -176,36 +176,96 @@ k_merge_minmax_topk(const float2* __restrict__ part_mm, const uint64_t* __restri
     if (threadIdx.x == 0 && n_valid) n_valid[row] = kk;
 }
 
-// ---- exact top-k (k <= 1024) of a row by 64-bit rank key: MSB radix select + bitonic sort ----
+// ---- exact top-k (k <= 2048) of a row by rank key: MSB radix select + bitonic sort ----
+// A key policy fixes the score type and how (score desc, index asc) is encoded as one unsigned key that is unique per
+// element, larger = better, and never 0 (0 pads the sort).  The select walks the key 8 bits at a time from the top.
 constexpr int kTopkThreads = 512;
 constexpr int kTopkMax = 2048;
 
+// fp32 scores: rank_key, the score and the index in 64 bits
+struct RankKeyF32 {
+    using Score = float;
+    using Key = uint64_t;
+    static constexpr int kBits = 64;
+    static constexpr int kUnroll = 4;   // of the histogram loop (what the compiler picks unasked)
+    __device__ static Key make(float s, uint32_t i) { return rank_key(s, i); }
+    __device__ static uint32_t digit(Key k, int shift) { return (uint32_t)(k >> shift) & 0xffu; }
+    __device__ static bool above_equal(Key k, Key prefix, int shift) {   // bits above shift + 8 agree
+        const uint64_t himask = shift == 56 ? 0ull : (~0ull << (shift + 8));
+        return (k & himask) == prefix;
+    }
+    __device__ static Key with_digit(Key prefix, uint32_t d, int shift) { return prefix | ((uint64_t)d << shift); }
+    __device__ static uint32_t index(Key k) { return key_index(k); }
+    __device__ static float score(Key k) { return key_score(k); }
+};
+
+// fp64 scores: an order-preserving 64-bit image of the double does not leave room for the index, so the key is 96 bits
+// wide, {ordered score, 0xffffffff - index}.  The select runs 4 more passes over the index bits: ties straddling the
+// cut resolve to the lower indices like any other key.
+struct Key96 {
+    uint64_t s;
+    uint64_t i;      // 0xffffffff - index (32 bits used)
+    __device__ bool operator<(const Key96& o) const { return s < o.s || (s == o.s && i < o.i); }
+    __device__ bool operator>=(const Key96& o) const { return !(*this < o); }
+};
+struct RankKeyF64 {
+    using Score = double;
+    using Key = Key96;
+    static constexpr int kBits = 96;
+    static constexpr int kUnroll = 1;   // unrolled, the loop spills its invariants to the stack
+    __device__ static Key make(double s, uint32_t i) {
+        const uint64_t u = (uint64_t)__double_as_longlong(s);
+        return Key96{(u >> 63) ? ~u : (u | (1ull << 63)), (uint64_t)(0xffffffffu - i)};
+    }
+    __device__ static uint32_t digit(Key k, int shift) {
+        return shift >= 32 ? (uint32_t)(k.s >> (shift - 32)) & 0xffu : (uint32_t)(k.i >> shift) & 0xffu;
+    }
+    __device__ static bool above_equal(Key k, Key prefix, int shift) {
+        const int top = shift + 8;
+        if (top >= 96) return true;
+        if (top >= 32) return (k.s >> (top - 32)) == (prefix.s >> (top - 32));
+        return k.s == prefix.s && (k.i >> top) == (prefix.i >> top);
+    }
+    __device__ static Key with_digit(Key p, uint32_t d, int shift) {
+        if (shift >= 32) p.s |= (uint64_t)d << (shift - 32);
+        else p.i |= (uint64_t)d << shift;
+        return p;
+    }
+    __device__ static uint32_t index(Key k) { return 0xffffffffu - (uint32_t)k.i; }
+    __device__ static double score(Key k) {
+        const uint64_t u = (k.s >> 63) ? (k.s & ~(1ull << 63)) : ~k.s;
+        return __longlong_as_double((long long)u);
+    }
+};
+
+template <class Pol>
 __global__ void __launch_bounds__(kTopkThreads)
-k_row_topk(const float* __restrict__ S, int64_t M, int64_t ld, int k, int* __restrict__ out_ids,
-           float* __restrict__ out_scores) {
+k_row_topk(const typename Pol::Score* __restrict__ S, int64_t M, int64_t ld, int k, int* __restrict__ out_ids,
+           typename Pol::Score* __restrict__ out_scores) {
+    using Key = typename Pol::Key;
     __shared__ unsigned int hist[256];
-    __shared__ uint64_t s_prefix;
+    __shared__ Key s_prefix;
     __shared__ int s_need;
     __shared__ int s_count;
-    __shared__ uint64_t keys[kTopkMax];
+    __shared__ Key keys[kTopkMax];
     const int row = blockIdx.x;
-    const float* s = S + (size_t)row * ld;
+    const typename Pol::Score* s = S + (size_t)row * ld;
     const int kk = (int)((int64_t)k < M ? k : M);   // number of real results
     int k2 = 1;
     while (k2 < k) k2 <<= 1;
-    for (int i = threadIdx.x; i < k2; i += kTopkThreads) keys[i] = 0ull;
-    if (threadIdx.x == 0) { s_prefix = 0ull; s_need = kk; s_count = 0; }
+    for (int i = threadIdx.x; i < k2; i += kTopkThreads) keys[i] = Key{};
+    if (threadIdx.x == 0) { s_prefix = Key{}; s_need = kk; s_count = 0; }
     __syncthreads();
     if (kk > 0) {
         // find the kk-th largest key, 8 bits at a time from the top
-        for (int shift = 56; shift >= 0; shift -= 8) {
+        for (int shift = Pol::kBits - 8; shift >= 0; shift -= 8) {
             for (int i = threadIdx.x; i < 256; i += kTopkThreads) hist[i] = 0u;
             __syncthreads();
-            const uint64_t prefix = s_prefix;
-            const uint64_t himask = shift == 56 ? 0ull : (~0ull << (shift + 8));
+            const Key prefix = s_prefix;
+#pragma unroll Pol::kUnroll
             for (int64_t i = threadIdx.x; i < M; i += kTopkThreads) {
-                const uint64_t key = rank_key(__ldg(s + i), (uint32_t)i);
-                if ((key & himask) == prefix) atomicAdd(&hist[(key >> shift) & 0xff], 1u);
+                const Key key = Pol::make(__ldg(s + i), (uint32_t)i);
+                if (Pol::above_equal(key, prefix, shift)) atomicAdd(&hist[Pol::digit(key, shift)], 1u);
             }
             __syncthreads();
             if (threadIdx.x == 0) {
@@ -215,14 +275,14 @@ k_row_topk(const float* __restrict__ S, int64_t M, int64_t ld, int k, int* __res
                     if ((int)hist[d] >= need) break;
                     need -= (int)hist[d];
                 }
-                s_prefix = prefix | ((uint64_t)d << shift);
+                s_prefix = Pol::with_digit(prefix, (uint32_t)d, shift);
                 s_need = need;
             }
             __syncthreads();
         }
-        const uint64_t kth = s_prefix;   // keys are unique, so exactly kk keys are >= kth
+        const Key kth = s_prefix;   // keys are unique, so exactly kk keys are >= kth
         for (int64_t i = threadIdx.x; i < M; i += kTopkThreads) {
-            const uint64_t key = rank_key(__ldg(s + i), (uint32_t)i);
+            const Key key = Pol::make(__ldg(s + i), (uint32_t)i);
             if (key >= kth) {
                 const int pos = atomicAdd(&s_count, 1);
                 if (pos < kTopkMax) keys[pos] = key;
@@ -236,7 +296,7 @@ k_row_topk(const float* __restrict__ S, int64_t M, int64_t ld, int k, int* __res
                     const int lo = 2 * i - (i & (stride - 1));
                     const int hi = lo + stride;
                     const bool desc = (lo & size) == 0;
-                    const uint64_t a = keys[lo], b = keys[hi];
+                    const Key a = keys[lo], b = keys[hi];
                     if ((a < b) == desc) { keys[lo] = b; keys[hi] = a; }
                 }
                 __syncthreads();
@@ -245,11 +305,11 @@ k_row_topk(const float* __restrict__ S, int64_t M, int64_t ld, int k, int* __res
     }
     for (int i = threadIdx.x; i < k; i += kTopkThreads) {
         if (i < kk) {
-            out_ids[(size_t)row * k + i] = (int)key_index(keys[i]);
-            out_scores[(size_t)row * k + i] = key_score(keys[i]);
+            out_ids[(size_t)row * k + i] = (int)Pol::index(keys[i]);
+            out_scores[(size_t)row * k + i] = Pol::score(keys[i]);
         } else {
             out_ids[(size_t)row * k + i] = -1;
-            out_scores[(size_t)row * k + i] = 0.f;
+            out_scores[(size_t)row * k + i] = 0;
         }
     }
 }
@@ -379,15 +439,26 @@ int merge_minmax_topk_ex(const float2* part_mm, const uint64_t* part_keys, int r
     return 0;
 }
 
-int row_topk(const float* S, int rows, int64_t M, int64_t ld, int k, int* out_ids, float* out_scores,
-             cudaStream_t stream) {
+template <class Pol>
+static int launch_row_topk(const typename Pol::Score* S, int rows, int64_t M, int64_t ld, int k, int* out_ids,
+                           typename Pol::Score* out_scores, cudaStream_t stream) {
     HRAG_CHECK(k >= 1 && k <= kTopkMax, "row_topk: k must be in [1, 2048]");
     HRAG_CHECK(M > 0 && M < (int64_t)0xffffffff, "row_topk: bad column count");
     if (rows == 0) return 0;
-    k_row_topk<<<rows, kTopkThreads, 0, stream>>>(S, M, ld, k, out_ids, out_scores);
+    k_row_topk<Pol><<<rows, kTopkThreads, 0, stream>>>(S, M, ld, k, out_ids, out_scores);
     count_launch(1);
     HRAG_CUDA(cudaGetLastError());
     return 0;
+}
+
+int row_topk(const float* S, int rows, int64_t M, int64_t ld, int k, int* out_ids, float* out_scores,
+             cudaStream_t stream) {
+    return launch_row_topk<RankKeyF32>(S, rows, M, ld, k, out_ids, out_scores, stream);
+}
+
+int row_topk(const double* S, int rows, int64_t M, int64_t ld, int k, int* out_ids, double* out_scores,
+             cudaStream_t stream) {
+    return launch_row_topk<RankKeyF64>(S, rows, M, ld, k, out_ids, out_scores, stream);
 }
 
 }  // namespace hrag

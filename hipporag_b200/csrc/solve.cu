@@ -303,10 +303,6 @@ int dev_ppr(hrag_t* h, int B, int iters, float alpha, float** result) {
     return 0;
 }
 
-}  // namespace hrag
-
-using namespace hrag;
-
 // Float64 PPR by iterative refinement (DESIGN.md section 2): per sub-batch of <= 16 columns, x = 0, r = v; every
 // round solves (I - aP32) d = fp32(r) with the fp32 solver, x += d in fp64, and recomputes r = v - x + a(hi + lo)x
 // in fp64.  P is column-substochastic, so ||(I - aP)^-1||_1 <= 1 / (1 - a), and ||x||_1 >= ||v||_1; normalising at
@@ -314,6 +310,107 @@ using namespace hrag;
 constexpr double kF64DefaultTol = 1e-10;   // PRPACK's target (HippoRAG.py:1736-1743)
 constexpr double kF64MinTol = 1e-13;       // above the fp64 floor of the bound (~1e-14 at damping 0.5)
 constexpr int kF64MaxRounds = 4;
+
+int check_f64_call(hrag_t* h, const char* who, double damping, double tol) {
+    const std::string w(who);
+    HRAG_CHECK(damping > 0.0 && damping < 1.0, w + ": damping must be in (0, 1)");
+    HRAG_CHECK(tol == 0.0 || tol >= kF64MinTol,
+               w + ": tol must be 0 (= 1e-10) or >= 1e-13; a smaller bound is below what the fp64 residual can certify");
+    HRAG_CHECK(h->g.n_global > 0, w + ": graph not loaded");
+    HRAG_CHECK(h->world == 1, w + ": not available on a node-range-sharded handle (world > 1); solve on a handle that "
+                                  "holds the whole graph");
+    HRAG_CHECK(h->g.val_lo != nullptr, w + ": the graph was loaded from fp32 values and has no fp64 operator; load it "
+                                           "with hrag_load_graph_csr_f64 or hrag_load_graph_coo");
+    return 0;
+}
+
+double f64_target(double tol) { return tol > 0.0 ? tol : kF64DefaultTol; }
+
+int ensure_state_f64(hrag_t* h, int Bp, int64_t io_cols) {
+    const size_t cells = (size_t)h->g.n_global * Bp;
+    HRAG_TRY(ensure_state(h, Bp));
+    HRAG_TRY(h->X64.ensure(cells * sizeof(double)));
+    HRAG_TRY(h->V64.ensure(cells * sizeof(double)));
+    HRAG_TRY(h->io64.ensure((size_t)std::max<int64_t>(io_cols, h->g.n_global) * Bp * sizeof(double)));
+    const int64_t rows_resid = resid_f64_partial_rows(h->g, Bp);
+    const int64_t part_rows = std::max<int64_t>(2 * rows_resid, ceil_div((int64_t)cells, 256));
+    HRAG_TRY(h->part64.ensure((size_t)part_rows * Bp * sizeof(double)));
+    HRAG_TRY(h->sums64.ensure(48 * sizeof(double)));
+    return 0;
+}
+
+int reset_f64(hrag_t* h, int Bp, int nb) {
+    int n_part = 0;
+    double* part_v = h->part64.as<double>();
+    HRAG_TRY(reset_to_state_f64(h->io64.as<double>(), nb, h->g.n_global, Bp, h->V64.as<double>(), h->V.as<float>(),
+                                h->X64.as<double>(), part_v, &n_part, h->stream));
+    return colsum_reduce_f64(part_v, n_part, Bp, h->sums64.as<double>(), h->stream);
+}
+
+int refine_f64(hrag_t* h, int Bp, int nb, double damping, double target, F64Refined* out) {
+    const int N = h->g.n_global;
+    const size_t cells = (size_t)N * Bp;
+    // the fp32 solves run at fp32(damping); the fp64 residual uses damping itself, so the refinement converges to
+    // the solution at the damping asked (float32(0.85) alone moves pi by ~1e-7)
+    const float damping32 = (float)damping;
+    const SweepPlan plan = plan_sweeps(h, damping32, 0, (float)kDefaultTol, false);   // fp32 solver at its own tol
+    const int64_t rows_resid = resid_f64_partial_rows(h->g, Bp);
+    double* X = h->X64.as<double>();
+    double* V = h->V64.as<double>();
+    double* part_r = h->part64.as<double>();
+    double* part_x = part_r + (size_t)rows_resid * Bp;
+    double* vsum = h->sums64.as<double>();
+    double* rsum = vsum + 16;
+    double* xsum = vsum + 32;
+    const double a = damping;
+    // every column refines until its own bound meets the target and then keeps its iterate: a query's result does
+    // not depend on the queries it shares the sub-batch with
+    unsigned active = (1u << nb) - 1u;
+    double resid = 0.0;
+    for (int round = 0; round < kF64MaxRounds && active; ++round) {
+        float* D = nullptr;
+        int n_part = 0;
+        HRAG_TRY(dev_ppr(h, Bp, plan.iters, damping32, &D));    // (I - aP32) d = fp32(r), r = h->V
+        {
+            StageTimer tm(h, ST_PPR);
+            HRAG_TRY(add_correction_f64(X, D, (int64_t)cells, Bp, active, h->stream));
+            HRAG_TRY(resid_sweep_f64(h->g, Bp, X, V, h->V.as<float>(), a, part_r, part_x, &n_part, h->stream));
+            HRAG_TRY(colsum_reduce_f64(part_r, n_part, Bp, rsum, h->stream));
+            HRAG_TRY(colsum_reduce_f64(part_x, n_part, Bp, xsum, h->stream));
+        }
+        h->stats.ppr_sweeps += 1;
+        h->stats.ppr_columns += Bp;
+        double s[32];
+        HRAG_CUDA(cudaMemcpyAsync(s, vsum, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
+        HRAG_CUDA(cudaStreamSynchronize(h->stream));
+        resid = 0.0;
+        for (int b = 0; b < nb; ++b) {
+            const double rel = s[b] > 0.0 ? s[16 + b] / s[b] : 0.0;   // a reset without mass has nothing to bound
+            resid = std::max(resid, rel);
+            if (2.0 * rel / (1.0 - a) <= target) active &= ~(1u << b);
+        }
+    }
+    out->resid = resid;
+    out->bound = 2.0 * resid / (1.0 - a);
+    out->active = active;
+    return 0;
+}
+
+// A call's end when a sub-batch missed the target: the stats report the call so far, status 4
+int f64_missed(hrag_t* h, const char* who, const F64Refined& r, double target, double call_resid, double call_bound) {
+    HRAG_TRY(resolve_spans(h));
+    h->last_rho = std::max(call_resid, r.resid);
+    h->last_bound = std::max(call_bound, r.bound);
+    char msg[200];
+    snprintf(msg, sizeof(msg), "%s: after %d refinement rounds the error bound is %.3e, above tol %.3e", who,
+             kF64MaxRounds, r.bound, target);
+    set_error(msg);
+    return 4;
+}
+
+}  // namespace hrag
+
+using namespace hrag;
 
 extern "C" {
 
@@ -360,87 +457,25 @@ int hrag_ppr(hrag_t* h, int32_t B, const float* reset, float damping, int32_t it
 
 int hrag_ppr_f64(hrag_t* h, int32_t B, const double* reset, double damping, double tol, double* out) {
     HRAG_CHECK(h && reset && out, "hrag_ppr_f64: null argument");
-    HRAG_CHECK(B >= 0 && damping > 0.0 && damping < 1.0, "hrag_ppr_f64: bad arguments");
-    HRAG_CHECK(tol == 0.0 || tol >= kF64MinTol,
-               "hrag_ppr_f64: tol must be 0 (= 1e-10) or >= 1e-13; a smaller bound is below what the fp64 residual "
-               "can certify");
-    HRAG_CHECK(h->g.n_global > 0, "hrag_ppr_f64: graph not loaded");
-    HRAG_CHECK(h->world == 1, "hrag_ppr_f64: not available on a node-range-sharded handle (world > 1); solve on a "
-                              "handle that holds the whole graph");
-    HRAG_CHECK(h->g.val_lo != nullptr, "hrag_ppr_f64: the graph was loaded from fp32 values and has no fp64 operator; "
-                                       "load it with hrag_load_graph_csr_f64 or hrag_load_graph_coo");
+    HRAG_CHECK(B >= 0, "hrag_ppr_f64: bad arguments");
+    HRAG_TRY(check_f64_call(h, "hrag_ppr_f64", damping, tol));
     HRAG_CUDA(cudaSetDevice(h->device));
-    const double target = tol > 0.0 ? tol : kF64DefaultTol;
+    const double target = f64_target(tol);
     const int N = h->g.n_global;
-    // the fp32 solves run at fp32(damping); the fp64 residual uses damping itself, so the refinement converges to
-    // the solution at the damping asked (float32(0.85) alone moves pi by ~1e-7)
-    const float damping32 = (float)damping;
-    const SweepPlan plan = plan_sweeps(h, damping32, 0, (float)kDefaultTol, false);   // fp32 solver at its own tol
     const int Bp = round_batch(std::min(16, std::max(B, 1)));
-    const size_t cells = (size_t)N * Bp;
-    HRAG_TRY(ensure_state(h, Bp));
-    HRAG_TRY(h->X64.ensure(cells * sizeof(double)));
-    HRAG_TRY(h->V64.ensure(cells * sizeof(double)));
-    HRAG_TRY(h->io64.ensure(cells * sizeof(double)));
-    const int64_t rows_resid = resid_f64_partial_rows(h->g, Bp);
-    const int64_t part_rows = std::max<int64_t>(2 * rows_resid, ceil_div((int64_t)cells, 256));
-    HRAG_TRY(h->part64.ensure((size_t)part_rows * Bp * sizeof(double)));
-    HRAG_TRY(h->sums64.ensure(48 * sizeof(double)));
-    double* X = h->X64.as<double>();
-    double* V = h->V64.as<double>();
-    double* part_r = h->part64.as<double>();
-    double* part_x = part_r + (size_t)rows_resid * Bp;
-    double* vsum = h->sums64.as<double>();
-    double* rsum = vsum + 16;
-    double* xsum = vsum + 32;
-    const double a = damping;
+    HRAG_TRY(ensure_state_f64(h, Bp, N));
+    double* xsum = h->sums64.as<double>() + 32;
     double call_resid = 0.0, call_bound = 0.0;
     for (int q0 = 0; q0 < B; q0 += Bp) {
         const int nb = std::min(Bp, B - q0);
-        int n_part = 0;
         HRAG_TRY(h2d(h, h->io64.p, reset + (size_t)q0 * N, (size_t)nb * N * sizeof(double)));
-        HRAG_TRY(reset_to_state_f64(h->io64.as<double>(), nb, N, Bp, V, h->V.as<float>(), X, part_r, &n_part, h->stream));
-        HRAG_TRY(colsum_reduce_f64(part_r, n_part, Bp, vsum, h->stream));
-        // every column refines until its own bound meets the target and then keeps its iterate: a query's result
-        // does not depend on the queries it shares the sub-batch with
-        unsigned active = (1u << nb) - 1u;
-        double resid = 0.0, bound = 0.0;
-        for (int round = 0; round < kF64MaxRounds && active; ++round) {
-            float* D = nullptr;
-            HRAG_TRY(dev_ppr(h, Bp, plan.iters, damping32, &D));    // (I - aP32) d = fp32(r), r = h->V
-            {
-                StageTimer tm(h, ST_PPR);
-                HRAG_TRY(add_correction_f64(X, D, (int64_t)cells, Bp, active, h->stream));
-                HRAG_TRY(resid_sweep_f64(h->g, Bp, X, V, h->V.as<float>(), a, part_r, part_x, &n_part, h->stream));
-                HRAG_TRY(colsum_reduce_f64(part_r, n_part, Bp, rsum, h->stream));
-                HRAG_TRY(colsum_reduce_f64(part_x, n_part, Bp, xsum, h->stream));
-            }
-            h->stats.ppr_sweeps += 1;
-            h->stats.ppr_columns += Bp;
-            double s[32];
-            HRAG_CUDA(cudaMemcpyAsync(s, vsum, sizeof(s), cudaMemcpyDeviceToHost, h->stream));
-            HRAG_CUDA(cudaStreamSynchronize(h->stream));
-            resid = 0.0;
-            for (int b = 0; b < nb; ++b) {
-                const double rel = s[b] > 0.0 ? s[16 + b] / s[b] : 0.0;   // a reset without mass has nothing to bound
-                resid = std::max(resid, rel);
-                if (2.0 * rel / (1.0 - a) <= target) active &= ~(1u << b);
-            }
-            bound = 2.0 * resid / (1.0 - a);
-        }
-        call_resid = std::max(call_resid, resid);
-        call_bound = std::max(call_bound, bound);
-        if (active) {
-            HRAG_TRY(resolve_spans(h));
-            h->last_rho = call_resid;
-            h->last_bound = call_bound;
-            char msg[160];
-            snprintf(msg, sizeof(msg), "hrag_ppr_f64: after %d refinement rounds the error bound is %.3e, above tol %.3e",
-                     kF64MaxRounds, bound, target);
-            set_error(msg);
-            return 4;
-        }
-        HRAG_TRY(state_to_scores_f64(X, nb, N, Bp, xsum, h->io64.as<double>(), h->stream));
+        HRAG_TRY(reset_f64(h, Bp, nb));
+        F64Refined r;
+        HRAG_TRY(refine_f64(h, Bp, nb, damping, target, &r));
+        if (r.active) return f64_missed(h, "hrag_ppr_f64", r, target, call_resid, call_bound);
+        call_resid = std::max(call_resid, r.resid);
+        call_bound = std::max(call_bound, r.bound);
+        HRAG_TRY(state_to_scores_f64(h->X64.as<double>(), nb, N, Bp, xsum, h->io64.as<double>(), h->stream));
         HRAG_TRY(d2h(h, out + (size_t)q0 * N, h->io64.p, (size_t)nb * N * sizeof(double)));
         HRAG_CUDA(cudaStreamSynchronize(h->stream));
     }

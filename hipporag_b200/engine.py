@@ -106,6 +106,20 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else C.c_void_p(a.ctypes.data)
 
 
+def _stage_b_inputs(q_pass, kept_idx, kept_score, dpr_only):
+    """The host arrays of a stage B call: (queries, kept_idx, kept_score (None when no facts), k, dpr flags)."""
+    q = _f32(q_pass)
+    B = q.shape[0]
+    kept_idx, kept_score = _i32(kept_idx), _f32(kept_score)
+    kf = kept_idx.shape[1] if kept_idx.ndim == 2 else (kept_idx.size // B if B else 0)
+    if kf == 0:
+        kept_idx = kept_score = None
+    if kf and (kept_idx.size != B * kf or kept_score.size != B * kf):
+        raise ValueError("kept_idx / kept_score must be [B, k]")
+    flags = None if dpr_only is None else np.ascontiguousarray(dpr_only, dtype=np.uint8)
+    return q, kept_idx, kept_score, kf, flags
+
+
 class Engine:
     """One handle = one H100.  Not thread-safe (like the reference's ``HippoRAG`` object)."""
 
@@ -286,20 +300,28 @@ class Engine:
 
         ``tol`` = relative L1 accuracy of each PPR vector (0 = 1e-6); the sweep counts follow from
         ``damping`` and ``tol`` unless ``iters`` pins them (``include/hrag_b200.h``)."""
-        q = _f32(q_pass)
+        q, kept_idx, kept_score, kf, flags = _stage_b_inputs(q_pass, kept_idx, kept_score, dpr_only)
         B = q.shape[0]
-        kept_idx, kept_score = _i32(kept_idx), _f32(kept_score)
-        kf = kept_idx.shape[1] if kept_idx.ndim == 2 else (kept_idx.size // B if B else 0)
-        if kf == 0:
-            kept_idx = kept_score = None
-        if kf and (kept_idx.size != B * kf or kept_score.size != B * kf):
-            raise ValueError("kept_idx / kept_score must be [B, k]")
-        flags = None if dpr_only is None else np.ascontiguousarray(dpr_only, dtype=np.uint8)
         ids = np.empty((B, topk), dtype=np.int32)
         scores = np.empty((B, topk), dtype=np.float32)
         _lib.check(self._lib.hrag_stage_b(self._h, B, _ptr(q), _ptr(kept_idx), _ptr(kept_score), kf, _ptr(flags),
                                           damping, passage_node_weight, link_top_k or 0, topk, int(iters),
                                           float(tol), _ptr(ids), _ptr(scores)))
+        return ids, scores
+
+    def stage_b_f64(self, q_pass, kept_idx, kept_score, dpr_only=None, damping: float = 0.5,
+                    passage_node_weight: float = 0.05, link_top_k: int = 5, topk: int = 200, tol: float = 0.0):
+        """``stage_b`` at PRPACK's accuracy (``hrag_stage_b_f64``): the reset in the reference's dtypes, float64 PPR
+        with every vector within ``tol`` relative L1 error (0 = 1e-10) by a rigorous bound, float64 gather and exact
+        top-k -> (ids [B,topk] int32, scores [B,topk] float64), best first.  Needs a graph loaded from float64 values
+        (``load_graph``, or ``load_graph_csr`` with a float64 ``val``)."""
+        q, kept_idx, kept_score, kf, flags = _stage_b_inputs(q_pass, kept_idx, kept_score, dpr_only)
+        B = q.shape[0]
+        ids = np.empty((B, topk), dtype=np.int32)
+        scores = np.empty((B, topk), dtype=np.float64)
+        _lib.check(self._lib.hrag_stage_b_f64(self._h, B, _ptr(q), _ptr(kept_idx), _ptr(kept_score), kf, _ptr(flags),
+                                              float(damping), passage_node_weight, link_top_k or 0, topk, float(tol),
+                                              _ptr(ids), _ptr(scores)))
         return ids, scores
 
     def retrieve_resident(self, d_q_fact, d_q_pass, d_out_ids, d_out_scores, damping: float = 0.5,

@@ -180,6 +180,21 @@ int hrag_stage_b(hrag_t* h, int32_t B, const float* q_pass, const int32_t* kept_
                  float damping, float passage_node_weight, int32_t link_top_k, int32_t topk,
                  int32_t iters, float tol, int32_t* out_ids, float* out_scores);
 
+/* hrag_stage_b at PRPACK's accuracy: what the reference's retrieve() computes (graph_search_with_fact_entities ->
+ * run_ppr, HippoRAG.py:1544-1656, 1709-1749), float64 to 1e-10.  The reset vector is built on the device in the
+ * reference's dtypes (phrase weights fp32(score) / fp32(chunk count), averaged in float64; passage weights
+ * fp32(minmax(dpr)) x fp32(passage_node_weight); summed in float64), solved as hrag_ppr_f64 solves (per sub-batch of
+ * <= 16 queries), and the passage scores are gathered and ranked in float64: out_scores [B, topk] float64, sorted by
+ * (score desc, id asc) exactly, -1 / 0 padded when topk > passages.  DPR-fallback rows are stage B's fp32 min-maxed
+ * scores, widened.  Arguments as in hrag_stage_b, except: damping is float64; tol is the relative L1 error bound of
+ * every PPR vector (0 = 1e-10, below 1e-13 is rejected); status 4 when 4 refinement rounds do not reach tol (the
+ * outputs are then unspecified); ppr_residual / ppr_error_bound of hrag_get_stats report the call.  Needs a graph
+ * loaded through hrag_load_graph_csr_f64 or hrag_load_graph_coo; fails on a node-range-sharded handle (world > 1). */
+int hrag_stage_b_f64(hrag_t* h, int32_t B, const float* q_pass, const int32_t* kept_fact_idx,
+                     const float* kept_fact_score, int32_t k_facts, const uint8_t* dpr_only, double damping,
+                     float passage_node_weight, int32_t link_top_k, int32_t topk, double tol, int32_t* out_ids,
+                     double* out_scores);
+
 /* The rule hrag_stage_b / hrag_ppr apply to (damping, tol, iters) for a batch of `batch` columns with the default engine
  * options, as a pure host function (no device needed): which solver runs (use_mixed: fp16 state + refinement, batches > 16
  * whose single refinement round reaches tol), the fp32 solver's sweep count, the mixed solver's two counts, and the
