@@ -14,6 +14,7 @@ LIB_PATH = os.path.join(_HERE, "libhrag_b200.so")
 PPR_POWER, PPR_CHEBYSHEV = 0, 1
 SIM_FP32, SIM_BF16X3, SIM_BF16 = 0, 1, 2
 PPR_FP32, PPR_MIXED = 0, 1
+DEVICE_EDGES, DEVICE_FACT_EMB, DEVICE_PASSAGE_EMB = 1, 2, 4     # hrag_index_append's on_device bits
 
 
 class HragError(RuntimeError):
@@ -55,6 +56,10 @@ SIGNATURES = {
     "hrag_load_embeddings": (C.c_int, [_p, C.c_int, _i64, _i32, _p, C.c_int]),
     "hrag_load_embeddings_begin": (C.c_int, [_p, C.c_int, _i64, _i32]),
     "hrag_load_embeddings_chunk": (C.c_int, [_p, C.c_int, _i64, _i64, _p, C.c_int]),
+    "hrag_set_mutable": (C.c_int, [_p, C.c_int]),
+    "hrag_index_reserve": (C.c_int, [_p, _i64, _i64, _i64, _i64]),
+    "hrag_index_append": (C.c_int, [_p, _i64, _i64, _p, _p, _p, _i64, _p, _i64, _p, _p, _p, _i32, _p, _p, C.c_int]),
+    "hrag_index_delete": (C.c_int, [_p, _i64, _p, _i64, _p, _p]),
     "hrag_set_options": (C.c_int, [_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "hrag_set_ppr_precision": (C.c_int, [_p, C.c_int, C.c_int, C.c_int]),
     "hrag_stage_a": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p]),
@@ -74,6 +79,7 @@ SIGNATURES = {
     "hrag_debug_keep_scores": (C.c_int, [_p, C.c_int]),
     "hrag_debug_copy": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
     "hrag_debug_graph": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
+    "hrag_debug_index": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
 }
 
 _lib = None

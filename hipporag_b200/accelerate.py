@@ -19,7 +19,8 @@ What is rebound (all paths under the reference's ``src/hipporag/``):
   (``:1427-1465``) -- single-call forms for code that uses them directly; ``run_ppr`` in float64 to PRPACK's
   1e-10 with ``run_ppr_fp64=True``;
 * ``index`` / ``delete`` (``:262``, ``:337``) -- additionally invalidate the device state
-  (``index`` forgets to clear ``ready_to_retrieve`` in the reference);
+  (``index`` forgets to clear ``ready_to_retrieve`` in the reference); with ``incremental=True`` the next prepare
+  applies the change to the device in place when it is an append or an ordered delete;
 * ``add_synonymy_edges`` (``:959-1020``) -- runs unchanged, but the ``retrieve_knn`` it calls
   (``utils/embed_utils.py:6-94``, imported into ``HippoRAG.py:35``) is the engine's fused
   threshold KNN for the duration of the call (``hipporag_b200/knn.py``).
@@ -38,6 +39,7 @@ from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 
+from ._lib import HragError
 from .engine import Engine
 
 logger = logging.getLogger(__name__)
@@ -72,9 +74,93 @@ def extract_tables(rag) -> dict:
                 fact_subj_vid=subj, fact_obj_vid=obj, ent_chunk_count=cnt, facts=facts)
 
 
+def index_view(rag) -> dict:
+    """What the engine mirrors of ``rag``'s index that is cheap to read (no ``eval``, no md5): vertex names, the
+    igraph edge list with its weights, fact keys, passage keys and passage vertices."""
+    edges = np.asarray(rag.graph.get_edgelist(), dtype=np.int32).reshape(-1, 2)
+    weights = np.asarray(rag.graph.es["weight"], dtype=np.float64) if len(edges) else np.zeros(0)
+    return dict(names=list(rag.graph.vs["name"]) if rag.graph.vcount() else [],
+                edge_src=np.ascontiguousarray(edges[:, 0]), edge_dst=np.ascontiguousarray(edges[:, 1]),
+                edge_w=weights, fact_keys=list(rag.fact_node_keys), passage_keys=list(rag.passage_node_keys),
+                passage_vid=np.asarray(rag.passage_node_idxs, dtype=np.int32))
+
+
+def _same_bits(a, b) -> bool:
+    return a.shape == b.shape and np.ascontiguousarray(a).tobytes() == np.ascontiguousarray(b).tobytes()
+
+
+def _subsequence(old: list, new: list):
+    """Positions in ``old`` of the items of ``new`` when ``new`` is ``old`` with some items removed in order, else
+    None."""
+    pos = {k: i for i, k in enumerate(old)}
+    if len(pos) != len(old):
+        return None
+    idx = [pos.get(k, -1) for k in new]
+    if any(i < 0 for i in idx) or any(b <= a for a, b in zip(idx, idx[1:])):
+        return None
+    return np.asarray(idx, dtype=np.int64)
+
+
+def classify_update(old: dict, new: dict):
+    """How the index moved from ``old`` to ``new`` (both ``index_view``s):
+
+    * ``("append", {...})``: old names, edges with their weights, fact keys, passage keys and passage vertices are all
+      prefixes of the new ones -- what ``HippoRAG.index()`` does (the stores append, igraph ``add_vertices`` /
+      ``add_edges``);
+    * ``("delete", {...})``: the new state is the old one with some vertices removed in order, the edge list is the
+      old one filtered and relabelled, fact keys are an ordered subsequence and the passages are those whose vertex
+      stayed -- what ``HippoRAG.delete()`` does (``delete_vertices`` compacts in order, the stores pop in place);
+    * ``("full", None)``: anything else.
+    """
+    n0, n = len(old["names"]), len(new["names"])
+    e0, f0, p0 = old["edge_src"].size, len(old["fact_keys"]), len(old["passage_keys"])
+    if (n >= n0 and new["names"][:n0] == old["names"] and new["edge_src"].size >= e0
+            and _same_bits(new["edge_src"][:e0], old["edge_src"]) and _same_bits(new["edge_dst"][:e0], old["edge_dst"])
+            and _same_bits(new["edge_w"][:e0], old["edge_w"]) and new["fact_keys"][:f0] == old["fact_keys"]
+            and new["passage_keys"][:p0] == old["passage_keys"]
+            and _same_bits(new["passage_vid"][:p0], old["passage_vid"])):
+        return "append", {"n_new_nodes": n - n0, "edges_from": e0, "facts_from": f0, "passages_from": p0}
+    kept = _subsequence(old["names"], new["names"])
+    kept_facts = _subsequence(old["fact_keys"], new["fact_keys"])
+    if kept is None or kept_facts is None or n == 0:
+        return "full", None
+    keep = np.zeros(n0, bool)
+    keep[kept] = True
+    vmap = np.where(keep, np.cumsum(keep) - 1, -1).astype(np.int32)
+    ke = keep[old["edge_src"]] & keep[old["edge_dst"]]
+    kp = keep[old["passage_vid"]]
+    if not (_same_bits(vmap[old["edge_src"][ke]], new["edge_src"]) and _same_bits(vmap[old["edge_dst"][ke]],
+                                                                                   new["edge_dst"])
+            and _same_bits(old["edge_w"][ke], new["edge_w"])
+            and [k for k, s in zip(old["passage_keys"], kp) if s] == new["passage_keys"]
+            and _same_bits(vmap[old["passage_vid"][kp]], new["passage_vid"])):
+        return "full", None
+    kf = np.zeros(f0, bool)
+    kf[kept_facts] = True
+    return "delete", {"nodes": np.flatnonzero(~keep).astype(np.int32), "facts": np.flatnonzero(~kf).astype(np.int32),
+                      "kept_facts": kept_facts}
+
+
+def _fact_ends(facts, name_to_vid):
+    """Subject / object vertex of each fact triple, -1 when absent (``HippoRAG.py:1584``, ``:1591-1595``)."""
+    from hipporag.utils.misc_utils import compute_mdhash_id
+    subj = np.array([name_to_vid.get(compute_mdhash_id(f[0].lower(), prefix="entity-"), -1) for f in facts], np.int32)
+    obj = np.array([name_to_vid.get(compute_mdhash_id(f[2].lower(), prefix="entity-"), -1) for f in facts], np.int32)
+    return subj, obj
+
+
+def _chunk_counts(rag, n, name_to_vid) -> np.ndarray:
+    cnt = np.zeros(n, dtype=np.int32)
+    for key, chunks in (rag.ent_node_to_chunk_ids or {}).items():                   # :1598-1601
+        vid = name_to_vid.get(key)
+        if vid is not None:
+            cnt[vid] = len(chunks)
+    return cnt
+
+
 def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_workers: int = 1,
                filter_chunk: int = 256, ppr_tol: float = 0.0, cache: bool = True, run_ppr_fp64: bool = False,
-               **engine_opts):
+               incremental: bool = False, **engine_opts):
     """Rebinds the hot-path methods of ``rag`` (a reference ``HippoRAG`` instance) in place.
 
     ``filter_workers > 1`` (SURVEY.md 8(f)-1) runs the per-query recognition-memory filter calls (LLM HTTP
@@ -91,6 +177,14 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     ``retrieve_ircot``, which call it -- runs stage B the same way (``Engine.stage_b_f64``): the reset vector built
     in the reference's dtypes, float64 PPR to ``ppr_tol``, float64 ``doc_scores`` as the reference returns them.
     ``retrieve_dpr`` has no PPR and is the same in both modes.
+    ``incremental=True`` follows ``index()`` / ``delete()`` in place instead of reloading: the graph is loaded from
+    the igraph edge list on a mutable handle (``Engine(mutable=True)``; the tables still come from the cache or
+    ``extract_tables``), and after the reference's own ``prepare_retrieval_objects`` has run, the change is
+    classified (``classify_update``): an append goes through ``Engine.append`` and an ordered delete through
+    ``Engine.delete``, with only the new facts ``eval``-ed; anything else is the full reload.
+    ``rag._b200_state["last_update"]`` records which ran ("append", "delete" or "full").  Incremental updates do not
+    write the binary cache: the next cold start rebuilds it, as after any change today.  The default
+    (``incremental=False``) loads the host-built CSR and reloads everything after ``index()`` / ``delete()``.
     ``engine_opts`` go to ``Engine.set_options``.
     """
     from hipporag.utils.misc_utils import QuerySolution
@@ -107,11 +201,86 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
 
     def _engine() -> Engine:
         if state["engine"] is None:
-            state["engine"] = Engine(device)
+            state["engine"] = Engine(device, mutable=incremental)
+        elif incremental and not state.get("mutable_set"):
+            state["engine"].set_mutable()
+        state["mutable_set"] = incremental
         return state["engine"]
+
+    def _embeddings(self):
+        fe = np.asarray(self.fact_embeddings, dtype=np.float32)
+        pe = np.asarray(self.passage_embeddings, dtype=np.float32)
+        return (fe.reshape(len(self.fact_node_keys), -1) if fe.size else np.zeros((0, pe.shape[1]), np.float32)), pe
+
+    def _try_update(self, eng: Engine, view: dict) -> str:
+        """Applies the change since the last load in place; returns what ran ("append" / "delete") or "full" when
+        it has to be reloaded."""
+        old = state.get("view")
+        if old is None:
+            return "full"
+        kind, info = classify_update(old, view)
+        name_to_vid = self.node_name_to_vertex_idx
+        n = len(view["names"])
+        if kind == "append":
+            f0, p0, e0 = info["facts_from"], info["passages_from"], info["edges_from"]
+            old_subj, old_obj = state["fact_ends"]
+            absent = np.flatnonzero((old_subj < 0) | (old_obj < 0))
+            if absent.size:   # an old fact's entity that has a vertex now would change its row: not an append
+                s, o = _fact_ends([state["facts"][i] for i in absent], name_to_vid)
+                if np.any(s != old_subj[absent]) or np.any(o != old_obj[absent]):
+                    return "full"
+            new_keys = view["fact_keys"][f0:]
+            rows = self.fact_embedding_store.get_rows(new_keys) if new_keys else {}
+            new_facts = [eval(rows[k]["content"]) for k in new_keys]                           # :1693
+            subj, obj = _fact_ends(new_facts, name_to_vid)
+            fe, pe = _embeddings(self)
+            eng.append(info["n_new_nodes"], view["edge_src"][e0:], view["edge_dst"][e0:], view["edge_w"][e0:],
+                       view["passage_vid"][p0:], subj, obj, _chunk_counts(self, n, name_to_vid), fe[f0:], pe[p0:])
+            state["facts"] = list(state["facts"]) + new_facts
+            state["fact_ends"] = (np.r_[old_subj, subj].astype(np.int32), np.r_[old_obj, obj].astype(np.int32))
+            return "append"
+        if kind == "delete":
+            eng.delete(info["nodes"], info["facts"], _chunk_counts(self, n, name_to_vid))
+            kept = info["kept_facts"]
+            state["facts"] = [state["facts"][i] for i in kept]
+            keep = np.ones(len(old["names"]), bool)
+            keep[info["nodes"]] = False
+            vmap = np.where(keep, np.cumsum(keep) - 1, -1).astype(np.int32)
+            state["fact_ends"] = tuple(np.where(a[kept] >= 0, vmap[np.maximum(a[kept], 0)], -1).astype(np.int32)
+                                       for a in state["fact_ends"])
+            return "delete"
+        return "full"
+
+    def prepare_incremental(self):
+        eng = _engine()
+        view = index_view(self)
+        try:
+            kind = _try_update(self, eng, view)
+        except HragError as e:                # rejected, or the index was dropped: reload it whole
+            logger.warning(f"b200 in-place index update failed, reloading: {e}")
+            kind = "full"
+        if kind == "full":
+            from . import cache as _cache
+            wd = getattr(self, "working_dir", None) if cache else None
+            tb = _cache.load(wd, _cache.fingerprint(self)) if wd else None
+            state["cache_hit"] = tb is not None
+            if tb is None:
+                tb = extract_tables(self)
+            eng.load_graph(len(view["names"]), view["edge_src"], view["edge_dst"], view["edge_w"])
+            eng.load_tables(tb["passage_vid"], tb["fact_subj_vid"], tb["fact_obj_vid"], tb["ent_chunk_count"])
+            eng.load_embeddings(*_embeddings(self))
+            state["facts"] = tb["facts"]
+            state["fact_ends"] = (np.asarray(tb["fact_subj_vid"], np.int32), np.asarray(tb["fact_obj_vid"], np.int32))
+        if engine_opts:
+            eng.set_options(**engine_opts)
+        state["view"] = view
+        state["last_update"] = kind
+        state["uploaded"] = True
 
     def prepare_retrieval_objects(self):
         orig_prepare()
+        if incremental:
+            return prepare_incremental(self)
         eng = _engine()
         from . import cache as _cache
         from .engine import build_transition_csr

@@ -5,6 +5,7 @@
 // HBM layout per handle (N nodes, P passages, F facts, d dims; DESIGN.md section 3):
 //   graph     row_ptr int32[n_rows+1], cv int2[nnz] {col, fp32 bits of P[i,j]}, row_order int32[n_rows]   (resident)
 //             + val_lo fp32[nnz] = fp32(P64 - hi) when loaded from float64 values (the fp64 solver's operator)
+//             + edges src/dst int32[E], w fp64[E]: the COO list as given, mutable handles only (index_update.cu)
 //   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N], slot_map[2][N] (node -> rhs slot)       (resident)
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
 //   state     mixed solver: H0..H3, H0b [N, 32] fp16 in one IPC-exportable slab; fp32 solver: V, XA, XC [N, B] fp32
@@ -90,8 +91,11 @@ struct Buf {
 enum Stage { ST_SIM_FACT = 0, ST_SEL_FACT, ST_SIM_PASS, ST_SEED, ST_PPR, ST_TOPK, ST_COMM, ST_COUNT };
 struct Span { int stage; cudaEvent_t a, b; };
 
+// The igraph edge list as the caller gave it (hrag_set_mutable handles loaded from a COO list only): int32 src, int32
+// dst, fp64 w, 16 bytes per edge, n edges in use; capacity grows geometrically under hrag_index_append.
+struct EdgeList { Buf src, dst, w; int64_t n = 0; };
 // Storage behind the views the kernel launchers take (PprGraph g, SeedTables t), filled in by ingest.cu
-struct GraphMem { Buf row_ptr, cv, row_order, long_rows, long_seg_ptr, segs, seg_partial, val_lo; };
+struct GraphMem { Buf row_ptr, cv, row_order, long_rows, long_seg_ptr, segs, seg_partial, val_lo; EdgeList edges; };
 struct TableMem { Buf passage_vid, fact_subj_vid, fact_obj_vid, ent_chunk_count; };
 struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passages)
     const float* f32 = nullptr;   // fp32 rows: borrowed from the caller (device upload, caller keeps it alive) or own
@@ -110,6 +114,7 @@ struct hrag_handle {
 
     hrag::PprGraph g;                  // view of `graph`
     hrag::GraphMem graph;
+    bool mutable_index = false;        // hrag_set_mutable: the next COO load keeps its edge list (graph.edges)
     int64_t chunk_rows = 0;      // rows per rank (sharded) = ceil(N / world)
     std::vector<int64_t> row_bounds;   // optional [world + 1]: rank r owns rows [row_bounds[r], row_bounds[r + 1]) -- a
                                        // work-balanced partition (non-zeros + 4 per row) instead of equal row counts
@@ -272,6 +277,9 @@ int coo_to_csr(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32_t* src, 
 int install_graph(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, int64_t nnz, const int64_t* row_ptr,
                   int64_t base, const int32_t* col, const float* val, const double* val64,
                   const std::vector<int64_t>& bounds);
+
+// index_update.cu: *out = a copy of a device edge list of n edges (what a mutable handle keeps).
+int copy_edge_list(hrag_t* h, int64_t n, const int32_t* src, const int32_t* dst, const double* w, EdgeList* out);
 
 int exchange_rows(hrag_t* h, float* y, int B);
 int p2p_wait(hrag_t* h);

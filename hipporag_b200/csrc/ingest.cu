@@ -87,9 +87,13 @@ int load_graph_coo_impl(hrag_t* h, const std::string& who, int64_t n_nodes, int6
         a = row_ptr[(size_t)lo], b = row_ptr[(size_t)hi];
     }
     HRAG_CHECK(b - a < ((int64_t)1 << 31) - 8, who + ": nnz must fit int32");
+    EdgeList kept;   // a mutable handle keeps the list itself for hrag_index_append / hrag_index_delete
+    if (h->mutable_index && h->world == 1) HRAG_TRY(copy_edge_list(h, n_edges, src, dst, w, &kept));
     // fp64 values: the same fp32 plane as the fp64 CSR entry, plus the lo plane hrag_ppr_f64 needs
-    return install_graph(h, n_nodes, lo, hi, b - a, csr.row_ptr.as<int64_t>() + lo, a, csr.col.as<int32_t>() + a,
-                         nullptr, csr.val.as<double>() + a, bounds);
+    HRAG_TRY(install_graph(h, n_nodes, lo, hi, b - a, csr.row_ptr.as<int64_t>() + lo, a, csr.col.as<int32_t>() + a,
+                           nullptr, csr.val.as<double>() + a, bounds));
+    if (kept.src.p) h->graph.edges = std::move(kept);
+    return 0;
 }
 
 // Drops embedding matrix `which`, sets dim and the rows of a `rows`-row matrix that this handle keeps (node-range

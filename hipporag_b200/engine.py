@@ -123,11 +123,13 @@ def _stage_b_inputs(q_pass, kept_idx, kept_score, dpr_only):
 class Engine:
     """One handle = one H100.  Not thread-safe (like the reference's ``HippoRAG`` object)."""
 
-    def __init__(self, device: int = 0, shard_mode: int = 0):
+    def __init__(self, device: int = 0, shard_mode: int = 0, mutable: bool = False):
         self._lib = _lib.load()
         self._h = C.c_void_p()
         dev = (C.c_int * 1)(device)
         _lib.check(self._lib.hrag_create(dev, 1, shard_mode, C.byref(self._h)))
+        if mutable:
+            self.set_mutable()
         self.device = device
         self.rank, self.world = 0, 1
         self.n_nodes = 0
@@ -172,23 +174,33 @@ class Engine:
         _lib.check(self._lib.hrag_p2p_import(self._h, blob, len(handles)))
 
     # ---------------------------------------------------------------- uploads
+    def set_mutable(self, on: bool = True):
+        """Before ``load_graph``: keep the edge list on the device (16 bytes per edge), which ``append`` and
+        ``delete`` need (``hrag_set_mutable``)."""
+        _lib.check(self._lib.hrag_set_mutable(self._h, 1 if on else 0))
+
+    def _check_device_edges(self, edge_src, edge_dst, edge_w) -> bool:
+        """True for three CUDA tensors (checked, and ready to read on the library's stream), False for host arrays."""
+        if not any(hasattr(a, "is_cuda") for a in (edge_src, edge_dst, edge_w)):
+            return False
+        import torch
+        want = (torch.int32, torch.int32, torch.float64)
+        for a, dt in zip((edge_src, edge_dst, edge_w), want):
+            if not (hasattr(a, "is_cuda") and a.is_cuda and a.device.index == self.device and a.dtype == dt
+                    and a.dim() == 1 and a.is_contiguous()):
+                raise ValueError("a device edge list is three contiguous 1-D CUDA tensors on the handle's device: "
+                                 "int32 edge_src, int32 edge_dst, float64 edge_w")
+        if not edge_src.shape == edge_dst.shape == edge_w.shape:
+            raise ValueError("edge_src, edge_dst, edge_w must have the same length")
+        torch.cuda.current_stream(self.device).synchronize()     # the library reads them on its own stream
+        return True
+
     def load_graph(self, n_nodes: int, edge_src, edge_dst, edge_w):
         """igraph-style edge list -> device CSR of P (built by the library on the GPU: hrag_load_graph_coo).
 
         The edge list may also be three contiguous 1-D CUDA torch tensors on this handle's device -- int32, int32 and
         float64 -- which are read in place (hrag_load_graph_coo_device) and not kept after the call."""
-        tensors = [a for a in (edge_src, edge_dst, edge_w) if hasattr(a, "is_cuda")]
-        if tensors:
-            import torch
-            want = (torch.int32, torch.int32, torch.float64)
-            for a, dt in zip((edge_src, edge_dst, edge_w), want):
-                if not (hasattr(a, "is_cuda") and a.is_cuda and a.device.index == self.device and a.dtype == dt
-                        and a.dim() == 1 and a.is_contiguous()):
-                    raise ValueError("a device edge list is three contiguous 1-D CUDA tensors on the handle's device: "
-                                     "int32 edge_src, int32 edge_dst, float64 edge_w")
-            if not edge_src.shape == edge_dst.shape == edge_w.shape:
-                raise ValueError("edge_src, edge_dst, edge_w must have the same length")
-            torch.cuda.current_stream(self.device).synchronize()     # the library reads them on its own stream
+        if self._check_device_edges(edge_src, edge_dst, edge_w):
             _lib.check(self._lib.hrag_load_graph_coo_device(
                 self._h, n_nodes, int(edge_src.shape[0]), C.c_void_p(edge_src.data_ptr()),
                 C.c_void_p(edge_dst.data_ptr()), C.c_void_p(edge_w.data_ptr())))
@@ -269,6 +281,89 @@ class Engine:
         self.dim = dim
         if which == 0:
             self.n_facts = int(rows)
+
+    # ---------------------------------------------------------------- incremental updates (mutable handles)
+    def reserve(self, nodes: int = 0, edges: int = 0, facts: int = 0, passages: int = 0):
+        """Size the capacity of the edge list, tables and embedding planes up front (``hrag_index_reserve``), so no
+        later ``append`` copies a plane into a larger allocation."""
+        _lib.check(self._lib.hrag_index_reserve(self._h, int(nodes), int(edges), int(facts), int(passages)))
+
+    def _emb_rows(self, emb, name):
+        """(pointer, rows, on_device, keep-alive, dim) of new embedding rows: a 2-D numpy array or contiguous fp32
+        CUDA tensor on the handle's device."""
+        if emb is None:
+            return None, 0, False, None, None
+        if hasattr(emb, "is_cuda"):
+            if not (emb.is_cuda and emb.device.index == self.device and emb.is_contiguous()
+                    and str(emb.dtype) == "torch.float32" and emb.dim() == 2):
+                raise ValueError(f"device {name} rows must be a contiguous 2-D fp32 CUDA tensor on the handle's device")
+            return C.c_void_p(emb.data_ptr()), int(emb.shape[0]), True, emb, int(emb.shape[1])
+        a = _f32(emb)
+        if a.size == 0:
+            return None, 0, False, None, None
+        if a.ndim != 2:
+            raise ValueError(f"{name} rows must be a 2-D array")
+        return _ptr(a), int(a.shape[0]), False, a, int(a.shape[1])
+
+    def _update(self, rc: int):
+        """Status of an update entry.  A rejected call leaves the index as it was; one that failed after its inputs
+        were checked (out of memory) leaves no index at all, and then the sizes here go to 0 as well."""
+        if rc != 0:
+            if self.debug_index("ent_chunk_count", size_only=True) == 0:
+                self.n_nodes = self.n_passages = self.n_facts = self.dim = 0
+            _lib.check(rc)
+
+    def append(self, n_new_nodes: int, edge_src=(), edge_dst=(), edge_w=(), passage_vid=(), fact_subj_vid=(),
+               fact_obj_vid=(), ent_chunk_count=None, fact_emb=None, passage_emb=None):
+        """``HippoRAG.index()`` on the device (``hrag_index_append``): append ``n_new_nodes`` vertices, the edges (ids
+        in the grown range; host arrays or three CUDA tensors as ``load_graph`` takes them), the passage and fact
+        rows of the tables with their embedding rows (numpy or CUDA tensors, copied), and replace
+        ``ent_chunk_count`` by the whole new table.  The handle then equals a fresh load of the grown arrays."""
+        n_new = int(n_new_nodes)
+        if self._check_device_edges(edge_src, edge_dst, edge_w):
+            ne, es, ed, ew, on_dev = int(edge_src.shape[0]), edge_src, edge_dst, edge_w, _lib.DEVICE_EDGES
+            ps, pd, pw = (C.c_void_p(t.data_ptr()) for t in (edge_src, edge_dst, edge_w))
+        else:
+            es, ed, ew = _i32(edge_src), _i32(edge_dst), np.ascontiguousarray(edge_w, dtype=np.float64)
+            if es.shape != ed.shape or es.shape != ew.shape:
+                raise ValueError("edge_src, edge_dst, edge_w must have the same length")
+            ne, on_dev = int(es.shape[0]), 0
+            ps, pd, pw = _ptr(es), _ptr(ed), _ptr(ew)
+        pv, fs, fo = _i32(passage_vid), _i32(fact_subj_vid), _i32(fact_obj_vid)
+        if fs.shape != fo.shape:
+            raise ValueError("fact_subj_vid / fact_obj_vid length mismatch")
+        cc = _i32(ent_chunk_count)
+        if cc.shape != (self.n_nodes + n_new,):
+            raise ValueError("ent_chunk_count must have one entry per vertex of the grown graph")
+        fp, f_rows, f_dev, f_keep, f_dim = self._emb_rows(fact_emb, "fact embedding")
+        pp, p_rows, p_dev, p_keep, p_dim = self._emb_rows(passage_emb, "passage embedding")
+        if f_rows != fs.shape[0] or p_rows != pv.shape[0]:
+            raise ValueError("one new embedding row per new fact / passage")
+        if f_dim is not None and p_dim is not None and f_dim != p_dim:
+            raise ValueError("the new fact and passage rows must share dim")
+        dim = f_dim or p_dim or self.dim                    # the library checks it against the index's
+        if f_dev or p_dev:
+            import torch
+            torch.cuda.current_stream(self.device).synchronize()
+        on_dev |= (_lib.DEVICE_FACT_EMB if f_dev else 0) | (_lib.DEVICE_PASSAGE_EMB if p_dev else 0)
+        self._update(self._lib.hrag_index_append(self._h, n_new, ne, ps, pd, pw, pv.shape[0], _ptr(pv), fs.shape[0],
+                                                 _ptr(fs), _ptr(fo), _ptr(cc), dim, fp, pp, on_dev))
+        del es, ed, ew, f_keep, p_keep                      # alive until the call has returned
+        self.n_nodes += n_new
+        self.n_passages += int(pv.shape[0])
+        self.n_facts += int(fs.shape[0])
+
+    def delete(self, nodes=(), facts=(), ent_chunk_count=None):
+        """``HippoRAG.delete()`` on the device (``hrag_index_delete``): remove the vertices ``nodes`` and the fact rows
+        ``facts`` (sorted, unique), renumbering what stays in order; passages whose vertex went are dropped with
+        their embedding rows; ``ent_chunk_count`` is the whole new table."""
+        nd, fd, cc = _i32(nodes), _i32(facts), _i32(ent_chunk_count)
+        if cc.shape != (self.n_nodes - nd.shape[0],):
+            raise ValueError("ent_chunk_count must have one entry per remaining vertex")
+        self._update(self._lib.hrag_index_delete(self._h, nd.shape[0], _ptr(nd), fd.shape[0], _ptr(fd), _ptr(cc)))
+        self.n_nodes -= int(nd.shape[0])
+        self.n_facts -= int(fd.shape[0])
+        self.n_passages = self.debug_index("passage_vid", size_only=True) // 4
 
     def set_options(self, ppr_method: Optional[int] = None, ppr_iters: Optional[int] = None,
                     ppr_batch: Optional[int] = None, sim_mode: Optional[int] = None,
@@ -428,6 +523,24 @@ class Engine:
         buf = np.empty(n.value // np.dtype(dtype).itemsize, dtype=dtype)
         _lib.check(self._lib.hrag_debug_graph(self._h, which, _ptr(buf), n.value, C.byref(n)))
         return buf.reshape(-1, width) if width > 1 else buf
+
+    INDEX_PLANES = {"passage_vid": (0, np.int32), "fact_subj_vid": (1, np.int32), "fact_obj_vid": (2, np.int32),
+                    "ent_chunk_count": (3, np.int32), "fact_hi": (4, np.uint16), "fact_lo": (5, np.uint16),
+                    "passage_hi": (6, np.uint16), "passage_lo": (7, np.uint16), "fact_f32": (8, np.float32),
+                    "passage_f32": (9, np.float32), "edge_src": (10, np.int32), "edge_dst": (11, np.int32),
+                    "edge_w": (12, np.float64)}
+
+    def debug_index(self, plane: str, size_only: bool = False):
+        """A copy of one plane of the tables, embeddings or resident edge list (``hrag_debug_index``): the embedding
+        planes as [rows, dim] (bf16 bits as uint16), every other plane 1-D; ``size_only`` returns its size in bytes."""
+        which, dtype = self.INDEX_PLANES[plane]
+        n = C.c_int64()
+        _lib.check(self._lib.hrag_debug_index(self._h, which, None, 0, C.byref(n)))
+        if size_only:
+            return n.value
+        buf = np.empty(n.value // np.dtype(dtype).itemsize, dtype=dtype)
+        _lib.check(self._lib.hrag_debug_index(self._h, which, _ptr(buf), n.value, C.byref(n)))
+        return buf.reshape(-1, self.dim) if 4 <= which <= 9 and self.dim else buf
 
 
 FactFilter = Callable[[int, Sequence[int], Sequence[float]], Sequence[int]]

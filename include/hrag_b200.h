@@ -145,6 +145,49 @@ int hrag_load_embeddings_begin(hrag_t* h, int which, int64_t rows, int32_t dim);
 int hrag_load_embeddings_chunk(hrag_t* h, int which, int64_t row0, int64_t n_rows, const float* emb,
                                int on_device);
 
+/* Incremental updates of a loaded index: what HippoRAG.index() (HippoRAG.py:262-335: the stores append, igraph
+ * add_vertices / add_edges, :1187, :1220) and HippoRAG.delete() (:337-411: the stores pop in place, igraph
+ * delete_vertices compacts in order, :408) do to the arrays this handle mirrors, applied on the device without a
+ * reload.  After any sequence of updates the handle holds, byte for byte, what a fresh load (hrag_load_graph_coo,
+ * hrag_load_tables, hrag_load_embeddings) of the resulting arrays gives: the graph planes are rebuilt from the
+ * resident edge list by the loaders' own builder, tables and embedding planes are appended to or compacted in order.
+ * Every input is checked before the handle is touched (a rejected call leaves it as it was); a call that fails after
+ * that (out of memory) leaves no graph, tables or embeddings rather than a half-updated index.
+ *
+ * on != 0 before a COO graph load: the handle keeps the edge list as given (int32 src, int32 dst, fp64 w: 16 bytes
+ * of HBM per edge, edges with w <= 0 or NaN included), which the update entries need.  The update entries reject
+ * handles without it (not mutable, graph loaded from a CSR), node-range-sharded handles (world > 1) and embedding
+ * matrices whose fp32 rows are borrowed from the caller (hrag_load_embeddings with on_device != 0). */
+int hrag_set_mutable(hrag_t* h, int on);
+
+/* Optional: sizes the capacity of the edge list (edges), ent_chunk_count (nodes), the fact tables and fact embedding
+ * planes (facts) and the passage table and planes (passages) up front, so that no later append copies a plane into
+ * a larger allocation (which holds both copies for a moment).  Without it capacity grows by half at a time. */
+int hrag_index_reserve(hrag_t* h, int64_t nodes, int64_t edges, int64_t facts, int64_t passages);
+
+/* HippoRAG.index(): appends n_new_nodes vertices (ids N .. N + n_new_nodes - 1), n_new_edges edges (endpoints in
+ * the grown range), n_new_passages rows of passage_vid, n_new_facts rows of fact_subj_vid / fact_obj_vid (-1 =
+ * absent) -- as hrag_load_tables takes them -- with their embedding rows fact_emb [n_new_facts, dim] and
+ * passage_emb [n_new_passages, dim]; ent_chunk_count is the whole new table [N + n_new_nodes].  dim must be the
+ * index's.  Only the new rows are uploaded and split into the bf16 planes.  Host arrays, except where on_device sets
+ * HRAG_DEVICE_EDGES (src / dst / w are device pointers, checked on the device), HRAG_DEVICE_FACT_EMB or
+ * HRAG_DEVICE_PASSAGE_EMB (the embedding rows are device pointers; they are copied, not borrowed). */
+#define HRAG_DEVICE_EDGES        1
+#define HRAG_DEVICE_FACT_EMB     2
+#define HRAG_DEVICE_PASSAGE_EMB  4
+int hrag_index_append(hrag_t* h, int64_t n_new_nodes, int64_t n_new_edges, const int32_t* src, const int32_t* dst,
+                      const double* w, int64_t n_new_passages, const int32_t* passage_vid, int64_t n_new_facts,
+                      const int32_t* fact_subj_vid, const int32_t* fact_obj_vid, const int32_t* ent_chunk_count,
+                      int32_t dim, const float* fact_emb, const float* passage_emb, int on_device);
+
+/* HippoRAG.delete(): removes the vertices del_nodes (sorted, unique) and the fact rows del_facts (sorted, unique),
+ * host arrays.  The remaining vertices are renumbered in order, edges with a deleted endpoint go and the others keep
+ * their order (parallel edges are summed in input order), passage rows whose vertex went are dropped and the others
+ * relabelled, fact subjects / objects are relabelled (a deleted vertex becomes -1), and the embedding rows follow
+ * their passages and facts, compacted in place.  ent_chunk_count is the whole new table [N - n_del_nodes]. */
+int hrag_index_delete(hrag_t* h, int64_t n_del_nodes, const int32_t* del_nodes, int64_t n_del_facts,
+                      const int32_t* del_facts, const int32_t* ent_chunk_count);
+
 /* Engine knobs that are not BaseConfig fields (SURVEY.md 5).  ppr_iters > 0 pins the sweep count of the
  * fp32 solver; by default it is derived from the damping factor (see hrag_stage_b). */
 int hrag_set_options(hrag_t* h, int ppr_method, int ppr_iters, int ppr_batch, int sim_mode);
@@ -268,6 +311,13 @@ int hrag_debug_copy(hrag_t* h, int which, float* host_out, int64_t max_elems, in
  * int32[n_long], 5 long_seg_ptr int32[n_long + 1] (empty when n_long = 0), 6 segs int4[n_seg].  *n_written = the
  * plane's size in bytes; host_out = NULL only reports it. */
 int hrag_debug_graph(hrag_t* h, int plane, void* host_out, int64_t max_bytes, int64_t* n_written);
+/* One plane of the loaded tables, embeddings or edge list, byte for byte (tests compare updated and fresh handles):
+ * plane = 0 passage_vid int32[P], 1 fact_subj_vid int32[F], 2 fact_obj_vid int32[F], 3 ent_chunk_count int32[N],
+ * 4 / 5 the bf16 hi / lo planes of the fact embeddings [F, dim], 6 / 7 those of the passage embeddings [P, dim],
+ * 8 / 9 the fp32 fact / passage rows [rows, dim] (empty when not held), 10 edge src int32[E], 11 edge dst int32[E],
+ * 12 edge weight fp64[E] (the list a mutable handle keeps).  *n_written = the plane's size in bytes; host_out =
+ * NULL only reports it. */
+int hrag_debug_index(hrag_t* h, int plane, void* host_out, int64_t max_bytes, int64_t* n_written);
 /* keep != 0: stage A materialises the fact score matrix even in the tensor-core modes (whose
  * default epilogue selects min/max/top-k in registers and never writes scores). */
 int hrag_debug_keep_scores(hrag_t* h, int keep);

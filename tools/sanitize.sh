@@ -30,6 +30,17 @@ r.engine.similarity(1, qp[:3])
 idx, score, nv = r.engine.stage_a(qf, 10)
 r.engine.stage_b(qp, idx, score, link_top_k=10, topk=50)
 r.engine.knn_threshold(0, fe[:200], 0.3, 64)
+# in-place index updates (index_update.cu): an append and a delete on a mutable handle, then one mixed stage B
+m = hb.B200Retriever(kg.n_nodes, src, dst, w, kg.passage_vid, kg.fact_subj_vid, kg.fact_obj_vid, kg.ent_chunk_count,
+                     fe, pe, engine=hb.Engine(0, mutable=True)).engine
+N = kg.n_nodes
+m.append(3, np.array([N, N + 1, 5], np.int32), np.array([7, 9, N + 2], np.int32), np.array([1.0, 0.5, 2.0]),
+         np.array([N + 2], np.int32), np.array([N, 3], np.int32), np.array([N + 1, -1], np.int32),
+         np.r_[kg.ent_chunk_count, [1, 2, 0]].astype(np.int32), fe[:2], pe[:1])
+m.delete(np.array([0, 11, N + 1], np.int32), np.array([1, 4], np.int32),
+         np.delete(np.r_[kg.ent_chunk_count, [1, 2, 0]], [0, 11, N + 1]).astype(np.int32))
+idx, score, nv = m.stage_a(qf, 5)
+m.stage_b(qp, idx, score, topk=50)
 print("driver ok", ids.shape)
 PY
 compute-sanitizer --tool $TOOL --error-exitcode 7 python /tmp/hrag_sanitize_driver.py 2>&1 | tail -15
