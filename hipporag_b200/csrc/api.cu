@@ -156,8 +156,16 @@ int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d
     const SweepPlan plan = plan_sweeps(h, damping, iters_arg, tol_arg, h->ppr_precision == HRAG_PPR_MIXED && Bq > 16);
     const bool mixed = plan.mixed;
     const int Bp = mixed ? 32 : round_batch(std::min(h->ppr_batch, Bq));
-    if (mixed) { HRAG_TRY(ensure_state_mixed(h)); HRAG_TRY(ensure_compact_rhs(h)); }
-    else HRAG_TRY(ensure_state(h, Bp));
+    // single GPU: consecutive sub-batches are solved in pairs, one walk of the CSR per sweep for both (an odd last one
+    // alone); node-range sharding solves them one by one (its exchange is fused into the single-state sweep)
+    const bool pairs = mixed && k_facts > 0 && h->world == 1 && Bq > 32;
+    if (mixed) {
+        HRAG_TRY(ensure_state_mixed(h));
+        if (pairs) HRAG_TRY(ensure_state_pair(h));
+        HRAG_TRY(ensure_compact_rhs(h, pairs ? 4 : 2));
+    } else {
+        HRAG_TRY(ensure_state(h, Bp));
+    }
     HRAG_TRY(h->seed_vid.ensure((size_t)Bq * kSeedSlots * sizeof(int)));     // [Bq, kSeedSlots] seed slots
     HRAG_TRY(h->seed_w.ensure((size_t)Bq * kSeedSlots * sizeof(double)));
     {
@@ -170,39 +178,55 @@ int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d
         HRAG_TRY(minmax_apply(S, Bq, P, ld, mm_pass, h->stream));
     }
     if (mixed && k_facts > 0) {
-        // Two streams: stream2 builds sub-batch i+1's compact right-hand side (passage weights + phrase seeds on
-        // P + 2048 slots, its column scales, the fp16 copy and the dense first iterate) while `stream` runs the
-        // sweeps of sub-batch i.
+        // Two streams: stream2 builds solve i+1's compact right-hand sides (passage weights + phrase seeds on
+        // P + 2048 slots, column scales, the fp16 copy and the dense first iterate) while `stream` runs the sweeps of
+        // solve i.  Solve i (one sub-batch, or a pair) uses the sets of parity i & 1: set p, and p + 2 for the second
+        // sub-batch of a pair.
         if (plan.check) h->check_tol = std::max(h->check_tol, plan.tol), h->check_kappa = plan.kappa;
         HRAG_CUDA(cudaEventRecord(h->ev_inputs, h->stream));            // S, min/max, seed lists are ready
         HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_inputs, 0));
         int it = 0;
-        for (int q0 = 0; q0 < Bq; q0 += 32, ++it) {
-            const int nb = std::min(32, Bq - q0);
-            const int set = it & 1;
-            void* x0 = set ? h->H0b : h->H[0];
-            float* scale = set ? h->mixed_aux1.as<float>() : h->mixed_aux.as<float>();
-            double* vsum = h->sums.as<double>() + kSumV + 32 * set;
-            int* slot_map = h->slot_map[set].as<int>();
-            if (it >= 2) HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_released[set], 0));   // set is free again
-            HRAG_TRY(compact_prepare_rhs(h->t, nb, q0, S, ld, mm_pass, pnw, kSeedSlots,
-                                         h->seed_vid.as<int>(), h->seed_w.as<double>(), damping, slot_map,
-                                         h->slot_vid[set].as<int>(), h->Vc[set].as<float>(), h->R16[set].p, x0,
-                                         (int64_t)h->g.n_global, h->prep_scratch.as<float>(), vsum, scale, h->stream2));
-            HRAG_CUDA(cudaEventRecord(h->ev_ready[set], h->stream2));
-            HRAG_CUDA(cudaStreamWaitEvent(h->stream, h->ev_ready[set], 0));
-            void *X0 = nullptr, *D = nullptr;
-            HRAG_TRY(dev_ppr_mixed(h, plan, damping, slot_map, h->Vc[set].as<float>(), h->R16[set].p, x0, scale, vsum,
-                                   &X0, &D));
+        for (int q0 = 0; q0 < Bq; ++it) {
+            const int n = pairs && Bq - q0 > 32 ? 2 : 1;
+            const int par = it & 1;
+            if (it >= 2) HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_released[par], 0));   // sets are free again
+            MixedRhs in[2];
+            int nb[2] = {0, 0};
+            for (int k = 0; k < n; ++k) {
+                const int set = par + 2 * k, qk = q0 + 32 * k;
+                nb[k] = std::min(32, Bq - qk);
+                void* pair_x0 = par ? h->HP0b : h->HP[0];
+                in[k].x0_dense = n == 2 ? pair_x0 : (par ? h->H0b : h->H[0]);
+                in[k].slot_map = h->slot_map[set].as<int>();
+                in[k].Vexact = h->Vc[set].as<float>();
+                in[k].rhs16 = h->R16[set].p;
+                in[k].scale = set_scale(h, set);
+                in[k].vsum = h->sums.as<double>() + kSumV + 32 * set;
+                HRAG_TRY(compact_prepare_rhs(h->t, nb[k], qk, S, ld, mm_pass, pnw, kSeedSlots, h->seed_vid.as<int>(),
+                                             h->seed_w.as<double>(), damping, h->slot_map[set].as<int>(),
+                                             h->slot_vid[set].as<int>(), h->Vc[set].as<float>(), h->R16[set].p,
+                                             static_cast<char*>(in[k].x0_dense) + 64 * k, 32 * n,
+                                             (int64_t)h->g.n_global, h->prep_scratch.as<float>(),
+                                             h->sums.as<double>() + kSumV + 32 * set, set_scale(h, set), h->stream2));
+            }
+            HRAG_CUDA(cudaEventRecord(h->ev_ready[par], h->stream2));
+            HRAG_CUDA(cudaStreamWaitEvent(h->stream, h->ev_ready[par], 0));
+            void *X0[2] = {nullptr, nullptr}, *D[2] = {nullptr, nullptr};
+            HRAG_TRY(dev_ppr_mixed(h, plan, damping, n, in, X0, D));
             {
                 StageTimer tm(h, ST_TOPK);
-                HRAG_TRY(gather_passage_scores_mixed(h->t, nb, q0, X0, D, 1.f / kMixedT, h->sums.as<double>(),
-                                                     h->sums.as<double>() + 32, h->mode.as<int>(),
-                                                     mm_pass, S, ld, h->stream));
-                HRAG_TRY(compact_release_slots(P, nb, q0, kSeedSlots, h->seed_vid.as<int>(), slot_map, h->stream));
+                for (int k = 0; k < n; ++k) {
+                    const double* sums = h->sums.as<double>() + (k ? kSumPair : 0);
+                    HRAG_TRY(gather_passage_scores_mixed(h->t, nb[k], q0 + 32 * k, X0[k], D[k], 32 * n, 1.f / kMixedT,
+                                                         sums + kSumX0, sums + kSumD, h->mode.as<int>(), mm_pass, S, ld,
+                                                         h->stream));
+                    HRAG_TRY(compact_release_slots(P, nb[k], q0 + 32 * k, kSeedSlots, h->seed_vid.as<int>(),
+                                                   h->slot_map[par + 2 * k].as<int>(), h->stream));
+                }
             }
             HRAG_TRY(p2p_signal(h));   // peers may overwrite this rank's state buffers from here on
-            HRAG_CUDA(cudaEventRecord(h->ev_released[set], h->stream));
+            HRAG_CUDA(cudaEventRecord(h->ev_released[par], h->stream));
+            q0 += 32 * n;
         }
         // (every prepare was consumed by a solve on `stream`, so stream2 is drained in stream order)
     }
@@ -282,7 +306,8 @@ int dev_stage_b_solve_f64(hrag_t* h, int Bq, const float* S, const float2* mm_pa
 // sub-batches).  Rates measured at C3 on an H100 SXM (132 SMs, 700 W): K1m alone 34.4 G non-zeros/s (14.5 M in
 // 0.422 ms per sweep); K2 next to the sweeps 1.56 TFLOP/s per SM -- half its rate alone (3.0), as its TMA operand
 // loads queue behind the sweeps' gathers.  At C3 the rule gives 54; 48 and 56 measured the same step time, 40 and
-// 66 slower.
+// 66 slower.  (Stage B's paired sweeps run at 46.0 G non-zeros/s per 32 columns; the scan has not been repeated
+// with them, so the rule keeps the rate it was tuned with.)
 int overlap_ctas(const hrag_t* h, int Bq, const SweepPlan& plan) {
     constexpr double kGemmFlopPerSmMs = 1.56e9, kSweepNnzPerMs = 3.44e7;
     const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
@@ -684,7 +709,11 @@ int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float
     HRAG_CHECK(B == 4 || B == 8 || B == 16 || B == 32 || B == 64, "hrag_bench_sweep: B in {4,8,16,32,64}");
     HRAG_CHECK(h->g.n_global > 0, "hrag_bench_sweep: graph not loaded");
     HRAG_CUDA(cudaSetDevice(h->device));
-    const bool mixed = method == 2 || method == 3;   // fp16-state sweep (Chebyshev form), B = 32; 2 = dense rhs, 3 = compact rhs
+    // fp16-state sweep (Chebyshev form), B = 32: 2 = dense rhs, 3 = compact rhs, 4 = the paired sweep of two
+    // compact-rhs sub-batches ([N, 2, 32] state), timed per paired sweep (64 columns)
+    const bool paired = method == 4;
+    const bool mixed = method == 2 || method == 3 || paired;
+    HRAG_CHECK(!paired || h->world == 1, "hrag_bench_sweep: the paired sweep runs on a single-GPU handle");
     const bool cheb = method == HRAG_PPR_CHEBYSHEV;
     const int* slot_map = nullptr;
     const void* rhs = nullptr;
@@ -693,16 +722,21 @@ int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float
         HRAG_CHECK(B == 32, "hrag_bench_sweep: the mixed solver runs at B = 32");
         HRAG_TRY(ensure_state_mixed(h));
         rhs = h->H[0];
-        if (method == 3) {
+        if (method >= 3) {
             HRAG_CHECK(h->t.passage_vid != nullptr, "hrag_bench_sweep: the compact-rhs sweep needs hrag_load_tables");
-            HRAG_TRY(ensure_compact_rhs(h));
+            HRAG_TRY(ensure_compact_rhs(h, 2));
             slot_map = h->slot_map[0].as<int>();
             rhs = h->R16[0].p;
-            HRAG_CUDA(cudaMemsetAsync(h->R16[0].p, 0x2c, h->R16[0].cap, h->stream));
+            for (int s = 0; s < 2; ++s) HRAG_CUDA(cudaMemsetAsync(h->R16[s].p, 0x2c, h->R16[s].cap, h->stream));
         }
         const size_t hb = (size_t)h->g.n_global * 32 * 2;
         for (int i = 0; i < 3; ++i) HRAG_CUDA(cudaMemsetAsync(h->H[i], 0x2c, hb, h->stream));   // 0x2c2c = 0.065
         A = h->H[1], C = h->H[2];
+        if (paired) {
+            HRAG_TRY(ensure_state_pair(h));
+            for (int i = 1; i < 3; ++i) HRAG_CUDA(cudaMemsetAsync(h->HP[i], 0x2c, 2 * hb, h->stream));
+            A = h->HP[1], C = h->HP[2];
+        }
     } else {
         HRAG_TRY(ensure_state(h, B));
         const size_t bytes = (size_t)h->g.n_global * B * sizeof(float);
@@ -721,7 +755,18 @@ int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float
             void* x = (i & 1) ? C : A;
             void* y = (i & 1) ? A : C;
             float* yf = static_cast<float*>(y);
-            if (mixed) HRAG_TRY(mixed_sweep_x(h, 0, x, slot_map, rhs, nullptr, nullptr, y, y, 0.5f, 1.07f, 1.f, nullptr, nullptr));
+            if (paired) {
+                MixedSweepIO io[2];
+                for (int k = 0; k < 2; ++k) {
+                    io[k].xh = static_cast<char*>(x) + 64 * k;
+                    io[k].slot_map = h->slot_map[k].as<int>();
+                    io[k].rhs_h = h->R16[k].p;
+                    io[k].prevh = io[k].yh = static_cast<char*>(y) + 64 * k;
+                }
+                HRAG_TRY(mixed_sweep2(h->g, 0, io, 0.5f, 1.07f, 1.f, nullptr, nullptr, h->stream));
+            } else if (mixed) {
+                HRAG_TRY(mixed_sweep_x(h, 0, x, slot_map, rhs, nullptr, nullptr, y, y, 0.5f, 1.07f, 1.f, nullptr, nullptr));
+            }
             else HRAG_TRY(ppr_sweep(h->g, B, static_cast<float*>(x), h->V.as<float>(), cheb ? yf : nullptr, yf, 0.5f,
                                     cheb ? 1.07f : 1.f, nullptr, nullptr, h->stream));
             if (!mixed) HRAG_TRY(exchange_rows(h, yf, B));

@@ -6,10 +6,12 @@
 //   graph     row_ptr int32[n_rows+1], cv int2[nnz] {col, fp32 bits of P[i,j]}, row_order int32[n_rows]   (resident)
 //             + val_lo fp32[nnz] = fp32(P64 - hi) when loaded from float64 values (the fp64 solver's operator)
 //             + edges src/dst int32[E], w fp64[E]: the COO list as given, mutable handles only (index_update.cu)
-//   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N], slot_map[2][N] (node -> rhs slot)       (resident)
+//   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N], slot_map[2 or 4][N] (node -> rhs slot) (resident)
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
-//   state     mixed solver: H0..H3, H0b [N, 32] fp16 in one IPC-exportable slab; fp32 solver: V, XA, XC [N, B] fp32
-//   rhs       compact: Vc [P + 2048, 32] fp32 (exact v) + R16 [P + 2048, 32] fp16 (scaled), two sets (double-buffered)
+//   state     mixed solver: H0..H3, H0b [N, 32] fp16 in one IPC-exportable slab, and for paired solves HP0..HP3, HP0b
+//             [N, 2, 32] fp16 (two sub-batches interleaved row by row); fp32 solver: V, XA, XC [N, B] fp32
+//   rhs       compact: Vc [P + 2048, 32] fp32 (exact v) + R16 [P + 2048, 32] fp16 (scaled), two sets (double-buffered),
+//             four when sub-batches are solved in pairs
 //   scores    S_pass [chunk, P] fp32; fact scores are never materialised in the fused modes (72 B per query x tile)
 // Streams: `stream` runs the similarity, the solves and the selection; `stream2` builds the compact right-hand side of
 // sub-batch i + 1 while sub-batch i is being solved.  On one GPU a sub-batch's solve is replayed as a CUDA graph.
@@ -105,6 +107,23 @@ struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passag
 
 }  // namespace hrag
 
+namespace hrag {
+// The inputs of one sub-batch's mixed solve: its right-hand side (compact through slot_map, or dense), exact v, the
+// dense first iterate, column scales and sums of v.  In a pair, x0_dense is the [N, 2, 32] buffer of both.
+struct MixedRhs {
+    const int* slot_map = nullptr;
+    const float* Vexact = nullptr;
+    const void* rhs16 = nullptr;
+    void* x0_dense = nullptr;
+    const float* scale = nullptr;
+    const double* vsum = nullptr;
+    bool operator==(const MixedRhs& o) const {
+        return slot_map == o.slot_map && Vexact == o.Vexact && rhs16 == o.rhs16 && x0_dense == o.x0_dense &&
+               scale == o.scale && vsum == o.vsum;
+    }
+};
+}  // namespace hrag
+
 struct hrag_handle {
     int device = 0;
     int shard_mode = 0;
@@ -152,11 +171,19 @@ struct hrag_handle {
     void* H[4] = {nullptr, nullptr, nullptr, nullptr};
     void* H0b = nullptr;
     hrag::Buf mixed_aux, rho, p2p_err, done_ctr;
+    // paired solves (single GPU, stage B): HP[i] / HP0b are H[i] / H0b for two sub-batches at once, [N, 2, 32]; the
+    // second sub-batch's column-sum partials go to partials_b
+    hrag::Buf slab_pair, partials_b;
+    void* HP[4] = {nullptr, nullptr, nullptr, nullptr};
+    void* HP0b = nullptr;
     // double-buffered per-sub-batch inputs (set s: x0 = H[0] / H0b, scales mixed_aux / mixed_aux1, compact rhs
-    // Vc[s] / R16[s] addressed through slot_map[s]): stream2 prepares sub-batch i+1 while `stream` sweeps sub-batch i
+    // Vc[s] / R16[s] addressed through slot_map[s]): stream2 prepares sub-batch i+1 while `stream` sweeps sub-batch i.
+    // A pair of sub-batches uses sets s and s + 2 (x0 = HP[0] / HP0b, the second one 64 B in); mixed_aux1 holds the
+    // scales of sets 1..3.
     hrag::Buf mixed_aux1, prep_scratch;
-    hrag::Buf slot_map[2], slot_vid[2], Vc[2], R16[2];
+    hrag::Buf slot_map[4], slot_vid[4], Vc[4], R16[4];
     bool slot_maps_valid = false;
+    int slot_maps_built = 0;                  // sets 0 .. slot_maps_built - 1 hold valid slot maps
     // scratch and I/O staging
     hrag::Buf S_fact, S_pass, mm_fact, mm_pass, mode, seed_vid, seed_w, q_hi, q_lo, part_mm, part_keys;
     hrag::Buf xr_mm, xr_keys;             // fact-sharded stage A: [world, Bq] min/max and [world, Bq, 8] best keys
@@ -165,14 +192,15 @@ struct hrag_handle {
     // second slot of what stream_sim hands to `stream` in hrag_retrieve_resident (slot 0: d_top_*, d_nvalid,
     // S_pass, mm_pass); allocated by the first call with two or more chunks
     struct { hrag::Buf top_idx, top_score, nvalid, S_pass, mm_pass; } pipe;
-    // CUDA graphs of the mixed solve, one per (buffer set, sweep plan, g_buf_generation)
+    // CUDA graphs of the mixed solve, one per (buffer sets, sweep plan, g_buf_generation)
     struct SolveGraph {
-        const void *x0 = nullptr, *slot_map = nullptr, *rhs16 = nullptr, *vexact = nullptr;
+        int n = 0;                        // sub-batches solved together (1, or 2 = a pair)
+        hrag::MixedRhs in[2];
         int m1 = 0, m2 = 0;
         float alpha = 0.f;
         int64_t generation = 0;
         cudaGraphExec_t exec = nullptr;
-        void *X0 = nullptr, *D = nullptr;
+        void *X0[2] = {nullptr, nullptr}, *D[2] = {nullptr, nullptr};
         int64_t sweeps = 0, columns = 0, launches = 0;
     };
     std::vector<SolveGraph> solve_graphs;
@@ -226,8 +254,9 @@ inline int d2h(hrag_t* h, void* dst, const void* src, size_t bytes) {
 
 constexpr int kSeedSlots = kSeedSlotsPerQuery;   // 2 phrases per kept fact, <= 32 kept facts
 constexpr float kMixedT = 64.f;    // residual scale: r ~ 5e-4 x, keeps it in fp16's normal range
-// sums layout (doubles): [0, 32) column sums of x0, [32, 64) of d, [64, 96) of |r|, [96, 160) of v (two buffer sets)
-constexpr int kSumX0 = 0, kSumD = 32, kSumR = 64, kSumV = 96;
+// sums layout (doubles): [0, 32) column sums of x0, [32, 64) of d, [64, 96) of |r|, [96, 224) of v (buffer sets 0..3),
+// [224, 320) the x0 / d / |r| sums of the second sub-batch of a pair
+constexpr int kSumX0 = 0, kSumD = 32, kSumR = 64, kSumV = 96, kSumPair = 224;
 constexpr double kDefaultTol = 1e-6;     // relative L1 accuracy of the PPR vector when the caller passes tol <= 0
 struct SweepPlan {
     bool mixed = false;
@@ -241,10 +270,14 @@ SweepPlan plan_sweeps(const hrag_t* h, float alpha, int iters_arg, float tol_arg
 int round_batch(int b);
 int ensure_state(hrag_t* h, int B);
 int ensure_state_mixed(hrag_t* h);
-int ensure_compact_rhs(hrag_t* h);
+int ensure_state_pair(hrag_t* h);        // HP / HP0b, partials_b (single GPU)
+int ensure_compact_rhs(hrag_t* h, int n_sets);
+float* set_scale(hrag_t* h, int set);    // column scales of compact-rhs set 0..3
 int resolve_spans(hrag_t* h);   // end of a call: checks the mixed solves, accumulates the stage times
-int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot_map, const float* Vexact,
-                  const void* rhs16, void* x0_dense, const float* scale, const double* vsum, void** X0, void** D);
+// The mixed solve of n = 1 sub-batch, or of n = 2 in one paired walk per sweep (single GPU; in[0].x0_dense is then the
+// pair's [N, 2, 32] buffer).  X0[k] / D[k] = sub-batch k's iterate and correction (rows 32 halves apart, 64 in a pair),
+// their column sums at h->sums + kSumX0 / kSumD (+ kSumPair for k = 1).
+int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, int n, const MixedRhs* in, void** X0, void** D);
 int dev_ppr(hrag_t* h, int B, int iters, float alpha, float** result);
 
 // Float64 PPR by iterative refinement (solve.cu), shared by hrag_ppr_f64 and hrag_stage_b_f64.

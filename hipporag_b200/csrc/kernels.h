@@ -74,6 +74,22 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
                 float t, float* partials, int* n_partials, int* overflow, const PeerOut& peers, const SweepSync& sync,
                 cudaStream_t stream);
 int mixed_partial_rows(const PprGraph& g);
+// The same sweep on two states at once (single GPU): one walk of each row's non-zeros feeds both, and each state gets
+// exactly the bytes, column sums and partials mixed_sweep would give it.  The two states are interleaved row by row in
+// [N, 2, 32] buffers: io[1]'s xh / prevh / yh (and a dense rhs_h) point 64 B after io[0]'s; a compact rhs_h, v32,
+// col_scale, slot_map and partials are each state's own.
+struct MixedSweepIO {
+    const void* xh = nullptr;
+    const int* slot_map = nullptr;
+    const void* rhs_h = nullptr;
+    const float* v32 = nullptr;
+    const float* col_scale = nullptr;
+    const void* prevh = nullptr;
+    void* yh = nullptr;
+    float* partials = nullptr;
+};
+int mixed_sweep2(const PprGraph& g, int mode, const MixedSweepIO (&io)[2], float alpha, float w, float t,
+                 int* n_partials, int* overflow, cudaStream_t stream);
 // vsum[32] <- column sums of V32 [n_rows, 32] (>= 0; `partials` = scratch of >= 1024*32 floats);
 // scale[b] = 2^floor(log2(32768 (1 - alpha) / vsum[b])) -- overflow-proof, see ppr_mixed.cu;
 // V16 = fp16(scale * V32).
@@ -85,10 +101,11 @@ int slot_map_build(int N, int P, const int* passage_vid, int* slot_map, cudaStre
 int compact_rhs_partial_rows(int P);
 // Builds, for the nb queries [q0, q0 + nb) of a chunk: Vc [P + 32*slots_per_query, 32] fp32 (passage weights
 // pnw * minmax(S) on the passage slots, phrase weights on freshly assigned seed slots), its column sums / fp16
-// scales, rhs16 = fp16(scale * Vc), and the dense first iterate x0_dense [n_nodes, 32] fp16.
+// scales, rhs16 = fp16(scale * Vc), and the dense first iterate x0_dense [n_nodes, 32] fp16, rows x0_ld halves apart
+// (32, or 64 for one state of an interleaved pair).
 int compact_prepare_rhs(const SeedTables& t, int nb, int q0, const float* S, int64_t ldS, const float2* minmax,
                         float pnw, int slots_per_query, const int* seed_vid, const double* seed_w, float alpha,
-                        int* slot_map, int* slot_vid, float* Vc, void* rhs16, void* x0_dense, int64_t n_nodes,
+                        int* slot_map, int* slot_vid, float* Vc, void* rhs16, void* x0_dense, int x0_ld, int64_t n_nodes,
                         float* partials, double* vsum, float* scale, cudaStream_t stream);
 int compact_release_slots(int P, int nb, int q0, int slots_per_query, const int* seed_vid, int* slot_map,
                           cudaStream_t stream);
@@ -97,9 +114,10 @@ int residual_check(const double* rsum, const double* vsum, const float* scale, f
                    cudaStream_t stream);
 int epoch_wait(const SweepSync& sync, cudaStream_t stream);
 int epoch_signal(const SweepSync& sync, cudaStream_t stream);
-int gather_passage_scores_mixed(const SeedTables& t, int nb, int q0, const void* X0, const void* D, float inv_t,
-                                const double* sum0, const double* sum1, const int* mode, const float2* minmax,
-                                float* S, int64_t ldS, cudaStream_t stream);
+// X0 / D rows are ldx halves apart (32, or 64 for one state of an interleaved pair)
+int gather_passage_scores_mixed(const SeedTables& t, int nb, int q0, const void* X0, const void* D, int ldx,
+                                float inv_t, const double* sum0, const double* sum1, const int* mode,
+                                const float2* minmax, float* S, int64_t ldS, cudaStream_t stream);
 int state_to_scores_mixed(const void* X0, const void* D, float inv_t, int nb, int N, const double* sum0,
                           const double* sum1, float* out, cudaStream_t stream);
 

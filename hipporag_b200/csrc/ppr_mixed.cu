@@ -127,19 +127,21 @@ __device__ __forceinline__ void sync_signal(const SweepSync& sy) {
 // MODE 0: y = w * (alpha * acc + rhs) + (1 - w) * prev        (all fp16 in memory)
 // MODE 1: y = t * (scale * v32 - x0 + alpha * acc)            (the refinement residual)
 // rhs / v32 are addressed through slot_map (null = dense).  Returns (in out[]) the value as
-// STORED (after fp16 rounding) so column sums match memory; MODE 1 + FINAL returns |value|.
-template <bool CHEB, int MODE>
+// STORED (after fp16 rounding) so column sums match memory; MODE 1 + FINAL returns |value|.  RS: row stride in uint4 of
+// x0h / prevh / yh and of a dense rhs_h (kLPR; 2 kLPR when two states are interleaved row by row); compact rhs_h and v32
+// are per state.
+template <bool CHEB, int MODE, int RS = kLPR>
 __device__ __forceinline__ void row_epilogue_h(float (&acc)[8], int row, int lane, const int* __restrict__ slot_map,
                                                const uint4* __restrict__ rhs_h, const float4* __restrict__ v32,
                                                const float* __restrict__ col_scale, const uint4* x0h,
                                                const uint4* prevh, uint4* yh, float alpha, float w, float t,
                                                const PeerOut& peers, int* overflow, float (&out)[8], uint4& packed_out) {
-    const size_t o = (size_t)row * kLPR + lane;
+    const size_t o = (size_t)row * RS + lane;
     const int slot = slot_map ? __ldg(slot_map + row) : row;
     if (MODE == 0) {
         if (slot >= 0) {
             float r[8];
-            h8_to_f(ld_stream16(rhs_h + (size_t)slot * kLPR + lane), r);
+            h8_to_f(ld_stream16(rhs_h + (size_t)slot * (slot_map ? kLPR : RS) + lane), r);
 #pragma unroll
             for (int j = 0; j < 8; ++j) out[j] = fmaf(alpha, acc[j], r[j]);
         } else {
@@ -256,6 +258,64 @@ k_sweep_h(const SweepArgs a) {
     if (FINAL) block_colsum_h(out, a.partials + (size_t)blockIdx.x * kB);
 }
 
+// Paired sweep: one walk of a row's non-zeros serves two states A and B (two sub-batches of 32 columns) stored
+// interleaved, [N, 2, 32]: each cv entry is loaded once and its two 16-byte gathers per lane fall in one 128-byte line,
+// and the column-independent bytes (cv, row_ptr, row_order) are paid once per 64 columns.  Each state's sums keep
+// k_sweep_h's order: the same fma sequence per lane, the same epilogue and the same column-sum partials.
+constexpr int kRS2 = 2 * kLPR;          // row stride of the interleaved pair in uint4
+__device__ __forceinline__ void group_row_dot_h2(const int2* __restrict__ cv, int s, int e,
+                                                 const uint4* __restrict__ xa, const uint4* __restrict__ xb,
+                                                 float (&acc_a)[8], float (&acc_b)[8]) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc_a[j] = acc_b[j] = 0.f;
+    for (int i = s; i < e; i += kU) {
+        int2 c[kU];
+        uint4 a[kU], b[kU];
+#pragma unroll
+        for (int j = 0; j < kU; ++j) c[j] = ld_cv(cv + i + j, i + j < e);
+#pragma unroll
+        for (int j = 0; j < kU; ++j) {
+            a[j] = ld_gather(xa + (size_t)c[j].x * kRS2, i + j < e);
+            b[j] = ld_gather(xb + (size_t)c[j].x * kRS2, i + j < e);
+        }
+#pragma unroll
+        for (int j = 0; j < kU; ++j) {
+            fma8(acc_a, __int_as_float(c[j].y), a[j]);
+            fma8(acc_b, __int_as_float(c[j].y), b[j]);
+        }
+    }
+}
+
+// 64 registers (4 CTAs per SM: 8 gathers in flight per lane, 8 K per SM against k_sweep_h's 6 K); FINAL keeps both
+// states' stored values for the column sums and takes 72 registers (3 CTAs per SM) rather than spill.
+template <bool CHEB, int MODE, bool FINAL>
+__global__ void __launch_bounds__(kThreads, FINAL ? 3 : 4)
+k_sweep_h2(const SweepArgs a, const SweepArgs b) {
+    const int g = threadIdx.x / kLPR, l = threadIdx.x % kLPR;
+    const int slot_r = blockIdx.x * kGPB + g;
+    float out_a[8], out_b[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) out_a[j] = out_b[j] = 0.f;
+    if (slot_r < a.n_rows) {
+        const int r = a.row_order ? __ldg(a.row_order + slot_r) : slot_r;
+        const int s = __ldg(a.row_ptr + r), e = __ldg(a.row_ptr + r + 1);
+        if (e - s <= a.long_thresh) {
+            float acc_a[8], acc_b[8];
+            uint4 packed;
+            group_row_dot_h2(a.cv, s, e, a.xh + l, b.xh + l, acc_a, acc_b);
+            row_epilogue_h<CHEB, MODE, kRS2>(acc_a, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh,
+                                             a.prevh, a.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out_a, packed);
+            row_epilogue_h<CHEB, MODE, kRS2>(acc_b, a.row_base + r, l, b.slot_map, b.rhs_h, b.v32, b.col_scale, b.xh,
+                                             b.prevh, b.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out_b, packed);
+        }
+    }
+    if (FINAL) {
+        block_colsum_h(out_a, a.partials + (size_t)blockIdx.x * kB);
+        __syncthreads();                             // block_colsum_h's shared scratch is reused
+        block_colsum_h(out_b, b.partials + (size_t)blockIdx.x * kB);
+    }
+}
+
 // K5, the sharded sweep: the same row computation with the exchange fused in.
 template <bool CHEB, int MODE, bool FINAL>
 __global__ void __launch_bounds__(kThreads, 6)
@@ -333,14 +393,15 @@ k_sweep_h_push(const SweepArgs a, const PeerOut peers, const SweepSync sy) {
     sync_signal(sy);
 }
 
+template <int RS = kLPR>
 __global__ void __launch_bounds__(kThreads)
 k_sweep_long_segments_h(int n_seg, const int4* __restrict__ segs, const int2* __restrict__ cv,
                         const uint4* __restrict__ xh, F8* __restrict__ seg_partial, const SweepSync sy) {
     sync_wait(sy);
-    segment_partial<LaneF16, kLPR>(n_seg, segs, cv, nullptr, xh, seg_partial);
+    segment_partial<LaneF16, kLPR, RS>(n_seg, segs, cv, nullptr, xh, seg_partial);
 }
 
-template <bool CHEB, int MODE, bool FINAL>
+template <bool CHEB, int MODE, bool FINAL, int RS = kLPR>
 __global__ void __launch_bounds__(kThreads)
 k_sweep_long_finalize_h(int n_long, const int* __restrict__ long_rows, const int* __restrict__ long_seg_ptr,
                         const F8* __restrict__ seg_partial, const SweepArgs a, const PeerOut peers,
@@ -354,8 +415,8 @@ k_sweep_long_finalize_h(int n_long, const int* __restrict__ long_rows, const int
         const int r = __ldg(long_rows + k);
         F8 acc = segment_sum<LaneF16, kLPR>(long_seg_ptr, k, seg_partial + l);
         uint4 packed;
-        row_epilogue_h<CHEB, MODE>(acc.v, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh, a.prevh,
-                                   a.yh, a.alpha, a.w, a.t, peers, a.overflow, out, packed);
+        row_epilogue_h<CHEB, MODE, RS>(acc.v, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh,
+                                       a.prevh, a.yh, a.alpha, a.w, a.t, peers, a.overflow, out, packed);
     }
     if (FINAL) block_colsum_h(out, a.partials + (size_t)blockIdx.x * kB);
     sync_signal(sy);
@@ -491,11 +552,11 @@ k_rhs_seeds(int P, int nb, int q0, int slots_per_query, const int* __restrict__ 
 }
 
 // rhs16[slot, :] = fp16(scale * Vc[slot, :]) for every slot, and the same row scattered into the dense
-// first iterate x0 (zeroed by the caller): x0[vertex(slot), :]
+// first iterate x0 (zeroed by the caller): x0[vertex(slot), :], rows x0_stride uint4 apart
 __global__ void __launch_bounds__(256)
 k_rhs_convert(int P, int n_slots, const int* __restrict__ passage_vid, const int* __restrict__ slot_vid,
               const float4* __restrict__ Vc, const float* __restrict__ scale, uint4* __restrict__ rhs16,
-              uint4* __restrict__ x0) {
+              uint4* __restrict__ x0, int x0_stride) {
     const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;       // one 8-column group
     const int slot = (int)(i >> 2), l = (int)(i & 3);
     if (slot >= n_slots) return;
@@ -506,7 +567,7 @@ k_rhs_convert(int P, int n_slots, const int* __restrict__ passage_vid, const int
     for (int j = 0; j < 8; ++j) f[j] *= __ldg(scale + l * 8 + j);
     const uint4 h = f_to_h8(f);
     rhs16[i] = h;
-    if (vid >= 0) x0[(size_t)vid * kLPR + l] = h;
+    if (vid >= 0) x0[(size_t)vid * x0_stride + l] = h;
 }
 
 // undo k_rhs_seeds: seed vertices that were given a slot of their own go back to "no rhs"
@@ -548,13 +609,14 @@ __global__ void __launch_bounds__(256)
 k_gather_passage_scores_mixed(int P, int nb, int q0, const int* __restrict__ passage_vid,
                               const __half* __restrict__ X0, const __half* __restrict__ D, float inv_t,
                               const double* __restrict__ sum0, const double* __restrict__ sum1,
-                              const int* __restrict__ mode, const float2* __restrict__ minmax, float* S, int64_t ldS) {
+                              const int* __restrict__ mode, const float2* __restrict__ minmax, float* S, int64_t ldS,
+                              int ldx) {
     const int64_t tI = (int64_t)blockIdx.x * 256 + threadIdx.x;
     const int p = (int)(tI / nb), b = (int)(tI % nb);
     if (p >= P) return;
     float* dst = S + (size_t)(q0 + b) * ldS + p;
     if (mode[q0 + b]) {
-        const size_t o = (size_t)__ldg(passage_vid + p) * kB + b;
+        const size_t o = (size_t)__ldg(passage_vid + p) * ldx + b;
         const float z = __half2float(X0[o]) + inv_t * __half2float(D[o]);        // x = x0 + d
         const float tot = (float)(sum0[b] + (double)inv_t * sum1[b]);
         *dst = __fdiv_rn(z, tot);
@@ -626,7 +688,7 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
     sy.total_ctas = (unsigned)(grid_rows + grid.nb_long);
     F8* segp = reinterpret_cast<F8*>(g.seg_partial);
     if (g.n_long) {     // only waits: the segment kernel writes no exchanged rows
-        k_sweep_long_segments_h<<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, a.xh, segp, sy);
+        k_sweep_long_segments_h<><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, a.xh, segp, sy);
         count_launch();
     }
     SweepArgs al = a;
@@ -647,6 +709,55 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
         }
     }, mode == 0 && prevh != nullptr, mode == 1, partials != nullptr);
     if (grid.nb_rows + grid.nb_long == 0 && sharded) HRAG_TRY(epoch_signal(sy, st));
+    if (n_partials) *n_partials = grid.nb_rows + grid.nb_long;
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int mixed_sweep2(const PprGraph& g, int mode, const MixedSweepIO (&io)[2], float alpha, float w, float t,
+                 int* n_partials, int* overflow, cudaStream_t st) {
+    HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep2: graph not loaded");
+    HRAG_CHECK(kB <= g.max_batch, "mixed_sweep2: segment partials too small for 32 columns");
+    HRAG_CHECK((io[0].partials == nullptr) == (io[1].partials == nullptr), "mixed_sweep2: partials for both or neither");
+    const SweepGrid grid(g, kGPB);
+    SweepArgs a[2];
+    for (int k = 0; k < 2; ++k) {
+        SweepArgs& x = a[k];
+        x.n_rows = g.n_rows; x.row_base = g.row_lo; x.long_thresh = g.long_thresh;
+        x.row_order = g.row_order;
+        x.row_ptr = g.row_ptr; x.cv = g.cv;
+        x.xh = reinterpret_cast<const uint4*>(io[k].xh);
+        x.slot_map = io[k].slot_map;
+        x.rhs_h = reinterpret_cast<const uint4*>(io[k].rhs_h);
+        x.v32 = reinterpret_cast<const float4*>(io[k].v32);
+        x.col_scale = io[k].col_scale;
+        x.prevh = reinterpret_cast<const uint4*>(io[k].prevh);
+        x.yh = reinterpret_cast<uint4*>(io[k].yh);
+        x.alpha = alpha; x.w = w; x.t = t;
+        x.partials = io[k].partials;
+        x.overflow = overflow;
+    }
+    F8* segp = reinterpret_cast<F8*>(g.seg_partial);
+    with_bools([&](auto cheb, auto resid, auto fin) {
+        if constexpr (!(cheb && resid)) {
+            constexpr int M = resid ? 1 : 0;
+            if (grid.nb_rows) {
+                k_sweep_h2<cheb, M, fin><<<grid.nb_rows, kThreads, 0, st>>>(a[0], a[1]);
+                count_launch();
+            }
+            // long rows: the single-state segment and finalize kernels, once per state (seg_partial is reused in
+            // stream order)
+            for (int k = 0; k < 2 && grid.nb_long; ++k) {
+                SweepArgs al = a[k];
+                al.partials = al.partials ? al.partials + (size_t)grid.nb_rows * kB : nullptr;
+                k_sweep_long_segments_h<kRS2><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, al.xh, segp,
+                                                                               SweepSync());
+                k_sweep_long_finalize_h<cheb, M, fin, kRS2><<<grid.nb_long, kThreads, 0, st>>>(
+                    g.n_long, g.long_rows, g.long_seg_ptr, segp, al, PeerOut(), SweepSync());
+                count_launch(2);
+            }
+        }
+    }, mode == 0 && io[0].prevh != nullptr, mode == 1, io[0].partials != nullptr);
     if (n_partials) *n_partials = grid.nb_rows + grid.nb_long;
     HRAG_CUDA(cudaGetLastError());
     return 0;
@@ -679,13 +790,15 @@ int compact_rhs_partial_rows(int P) { return (int)ceil_div(std::max(P, 1), 32); 
 
 int compact_prepare_rhs(const SeedTables& t, int nb, int q0, const float* S, int64_t ldS, const float2* minmax,
                         float pnw, int slots_per_query, const int* seed_vid, const double* seed_w, float alpha,
-                        int* slot_map, int* slot_vid, float* Vc, void* rhs16, void* x0_dense, int64_t n_nodes,
+                        int* slot_map, int* slot_vid, float* Vc, void* rhs16, void* x0_dense, int x0_ld, int64_t n_nodes,
                         float* partials, double* vsum, float* scale, cudaStream_t st) {
     const int P = t.n_passages;
     const int n_seed_slots = kB * slots_per_query;
     HRAG_CHECK(slots_per_query > 0, "compact_prepare_rhs: slots_per_query must be positive");
     const int nblk = compact_rhs_partial_rows(P);
-    HRAG_CUDA(cudaMemsetAsync(x0_dense, 0, (size_t)n_nodes * kB * 2, st));
+    HRAG_CHECK(x0_ld == kB || x0_ld == 2 * kB, "compact_prepare_rhs: x0 rows are 32 or 64 halves apart");
+    if (x0_ld == kB) HRAG_CUDA(cudaMemsetAsync(x0_dense, 0, (size_t)n_nodes * kB * 2, st));
+    else HRAG_CUDA(cudaMemset2DAsync(x0_dense, (size_t)x0_ld * 2, 0, kB * 2, (size_t)n_nodes, st));
     HRAG_CUDA(cudaMemsetAsync(Vc + (size_t)P * kB, 0, (size_t)n_seed_slots * kB * sizeof(float), st));
     k_rhs_passages<<<nblk, 256, 0, st>>>(P, nb, S, ldS, q0, minmax, pnw, Vc, partials);
     k_rhs_seeds<<<1, 1024, 0, st>>>(P, nb, q0, slots_per_query, seed_vid, seed_w, slot_map, slot_vid, Vc,
@@ -693,7 +806,7 @@ int compact_prepare_rhs(const SeedTables& t, int nb, int q0, const float* S, int
     const int n_slots = P + n_seed_slots;
     k_rhs_convert<<<(unsigned)ceil_div((int64_t)n_slots * kLPR, 256), 256, 0, st>>>(
         P, n_slots, t.passage_vid, slot_vid, reinterpret_cast<const float4*>(Vc), scale,
-        reinterpret_cast<uint4*>(rhs16), reinterpret_cast<uint4*>(x0_dense));
+        reinterpret_cast<uint4*>(rhs16), reinterpret_cast<uint4*>(x0_dense), x0_ld / 8);
     count_launch(3);
     HRAG_CUDA(cudaGetLastError());
     return 0;
@@ -715,14 +828,14 @@ int residual_check(const double* rsum, const double* vsum, const float* scale, f
     return 0;
 }
 
-int gather_passage_scores_mixed(const SeedTables& t, int nb, int q0, const void* X0, const void* D, float inv_t,
-                                const double* sum0, const double* sum1, const int* mode, const float2* minmax,
-                                float* S, int64_t ldS, cudaStream_t st) {
+int gather_passage_scores_mixed(const SeedTables& t, int nb, int q0, const void* X0, const void* D, int ldx,
+                                float inv_t, const double* sum0, const double* sum1, const int* mode,
+                                const float2* minmax, float* S, int64_t ldS, cudaStream_t st) {
     if (t.n_passages == 0 || nb == 0) return 0;
     const int64_t total = (int64_t)t.n_passages * nb;
     k_gather_passage_scores_mixed<<<(unsigned)ceil_div(total, 256), 256, 0, st>>>(
         t.n_passages, nb, q0, t.passage_vid, reinterpret_cast<const __half*>(X0), reinterpret_cast<const __half*>(D),
-        inv_t, sum0, sum1, mode, minmax, S, ldS);
+        inv_t, sum0, sum1, mode, minmax, S, ldS, ldx);
     count_launch();
     HRAG_CUDA(cudaGetLastError());
     return 0;

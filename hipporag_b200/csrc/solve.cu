@@ -45,30 +45,47 @@ int ensure_state_mixed(hrag_t* h) {
         if (!h->done_ctr.p) HRAG_TRY(h->done_ctr.zeros(sizeof(unsigned int)));
     }
     HRAG_TRY(h->partials.ensure((size_t)std::max(mixed_partial_rows(h->g), 1024) * 32 * sizeof(float)));
-    HRAG_TRY(h->sums.ensure(192 * sizeof(double)));      // sums of x0, of d, of |r|, and of v (two sets)
+    HRAG_TRY(h->sums.ensure(320 * sizeof(double)));      // sums of x0, of d, of |r| (x2), and of v (four sets)
     HRAG_TRY(h->mixed_aux.ensure(32 * sizeof(float)));   // column scales, set 0
     // [0] running max of the measured residual (float), [1] fp16 overflow flag (int)
     if (h->rho.p == nullptr) HRAG_TRY(h->rho.zeros(2 * sizeof(float)));
     return 0;
 }
 
-// Compact right-hand-side buffers of stage B (two sets, see the handle) + the node -> slot tables.
-int ensure_compact_rhs(hrag_t* h) {
+int ensure_state_pair(hrag_t* h) {
+    HRAG_CHECK(h->world == 1, "internal: paired solves run on a single GPU");
+    const size_t hb2 = (size_t)h->g.n_global * 64 * 2;
+    HRAG_TRY(h->slab_pair.ensure(5 * hb2));
+    for (int i = 0; i < 4; ++i) h->HP[i] = static_cast<char*>(h->slab_pair.p) + (size_t)i * hb2;
+    h->HP0b = static_cast<char*>(h->slab_pair.p) + 4 * hb2;
+    HRAG_TRY(h->partials_b.ensure(h->partials.cap));
+    return 0;
+}
+
+// Compact right-hand-side buffers of stage B (two sets, four for paired solves; see the handle) + the node -> slot
+// tables.
+int ensure_compact_rhs(hrag_t* h, int n_sets) {
     const size_t n_slots = (size_t)h->t.n_passages + 32 * kSeedSlots;
-    for (int s = 0; s < 2; ++s) {
+    for (int s = 0; s < n_sets; ++s) {
         HRAG_TRY(h->slot_map[s].ensure((size_t)h->g.n_global * sizeof(int)));
         HRAG_TRY(h->slot_vid[s].ensure(n_slots * sizeof(int)));
         HRAG_TRY(h->Vc[s].ensure(n_slots * 32 * sizeof(float)));
         HRAG_TRY(h->R16[s].ensure(n_slots * 32 * 2));
     }
-    HRAG_TRY(h->mixed_aux1.ensure(32 * sizeof(float)));
+    HRAG_TRY(h->mixed_aux1.ensure(3 * 32 * sizeof(float)));
     HRAG_TRY(h->prep_scratch.ensure((size_t)std::max(compact_rhs_partial_rows(h->t.n_passages), 1024) * 32 * sizeof(float)));
-    if (!h->slot_maps_valid) {
-        for (int s = 0; s < 2; ++s)
-            HRAG_TRY(slot_map_build(h->g.n_global, h->t.n_passages, h->t.passage_vid, h->slot_map[s].as<int>(), h->stream));
+    if (!h->slot_maps_valid) {                       // a graph or table load invalidated every set
+        h->slot_maps_built = 0;
         h->slot_maps_valid = true;
     }
+    for (; h->slot_maps_built < n_sets; ++h->slot_maps_built)
+        HRAG_TRY(slot_map_build(h->g.n_global, h->t.n_passages, h->t.passage_vid,
+                                h->slot_map[h->slot_maps_built].as<int>(), h->stream));
     return 0;
+}
+
+float* set_scale(hrag_t* h, int set) {
+    return set == 0 ? h->mixed_aux.as<float>() : h->mixed_aux1.as<float>() + 32 * (set - 1);
 }
 
 int resolve_spans(hrag_t* h) {
@@ -135,25 +152,62 @@ static float cheb_step(int it, float alpha, double* w, T* a, T* c, T* prev, T** 
     return (float)*w;
 }
 
-// m Chebyshev sweeps of the fp16 solver on (I - aP) x = rhs, first iterate x_first (= rhs as a dense [N, 32]
-// array); rhs itself is addressed through slot_map (null = dense).  Iterates alternate between bufA and bufC;
-// *result = the last one, its column sums land in sums_out[0..32).
-static int mixed_cheb(hrag_t* h, const int* slot_map, const void* rhs, void* x_first, void* bufA, void* bufC, int m,
-                      float alpha, void** result, double* sums_out) {
+// Sub-batch k's part of a [N, 2, 32] pair buffer (64 B into each row for k = 1); null stays null.
+static void* pair_half(const void* p, int k) {
+    return p ? static_cast<char*>(const_cast<void*>(p)) + 64 * k : nullptr;
+}
+
+// One sweep of the n sub-batches of a solve (n = 2: one paired walk over the interleaved buffers x, prev, y).
+// slot_map / rhs / v32 / scale are per sub-batch; a dense rhs (slot_map null) is a buffer like x.  final: the column-sum
+// partials of sub-batch k go to h->partials (k = 0) / h->partials_b (k = 1).
+static int mixed_sweep_n(hrag_t* h, int n, int mode, const void* x, const int* const* slot_map,
+                         const void* const* rhs, const float* const* v32, const float* const* scale, const void* prev,
+                         void* y, float alpha, float w, float t, bool final, int* n_part) {
+    if (n == 1)
+        return mixed_sweep_x(h, mode, x, slot_map[0], rhs[0], v32[0], scale[0], prev, y, alpha, w, t,
+                             final ? h->partials.as<float>() : nullptr, n_part);
+    MixedSweepIO io[2];
+    for (int k = 0; k < 2; ++k) {
+        io[k].xh = pair_half(x, k);
+        io[k].slot_map = slot_map[k];
+        io[k].rhs_h = slot_map[k] ? rhs[k] : pair_half(rhs[k], k);
+        io[k].v32 = v32[k];
+        io[k].col_scale = scale[k];
+        io[k].prevh = pair_half(prev, k);
+        io[k].yh = pair_half(y, k);
+        io[k].partials = final ? (k ? h->partials_b : h->partials).as<float>() : nullptr;
+    }
+    int* overflow = h->rho.p ? h->rho.as<int>() + 1 : nullptr;
+    return mixed_sweep2(h->g, mode, io, alpha, w, t, n_part, overflow, h->stream);
+}
+
+// Column sums of sub-batch k of the last final sweep -> h->sums + off (+ kSumPair for k = 1)
+static int mixed_sums(hrag_t* h, int n, int n_part, int off) {
+    for (int k = 0; k < n; ++k)
+        HRAG_TRY(colsum_reduce((k ? h->partials_b : h->partials).as<float>(), n_part, 32,
+                               h->sums.as<double>() + off + (k ? kSumPair : 0), h->stream));
+    return 0;
+}
+
+// m Chebyshev sweeps of the fp16 solver on (I - aP) x = rhs for n sub-batches, first iterate x_first (= rhs as a dense
+// [N, 32] array, [N, 2, 32] for a pair); rhs[k] is addressed through slot_map[k] (null = dense).  Iterates alternate
+// between bufA and bufC; *result = the last one, its column sums land in h->sums + sums_off.
+static int mixed_cheb(hrag_t* h, int n, const int* const* slot_map, const void* const* rhs, void* x_first, void* bufA,
+                      void* bufC, int m, float alpha, void** result, int sums_off) {
     HRAG_CHECK(m >= 1, "mixed solver: sweep count must be >= 1");
+    const float* none[2] = {nullptr, nullptr};
     double w = 1.0;
     void *x = x_first, *prev = nullptr, *y = nullptr;
     int n_part = 0;
     for (int it = 1; it <= m; ++it) {
-        float* part = it == m ? h->partials.as<float>() : nullptr;
         const float wf = cheb_step(it, alpha, &w, bufA, bufC, prev, &y);
-        HRAG_TRY(mixed_sweep_x(h, 0, x, slot_map, rhs, nullptr, nullptr, prev, y, alpha, wf, 1.f, part, &n_part));
+        HRAG_TRY(mixed_sweep_n(h, n, 0, x, slot_map, rhs, none, none, prev, y, alpha, wf, 1.f, it == m, &n_part));
         prev = x;
         x = y;
-        h->stats.ppr_sweeps += 1;
-        h->stats.ppr_columns += 32;
+        h->stats.ppr_sweeps += n;
+        h->stats.ppr_columns += 32 * n;
     }
-    HRAG_TRY(colsum_reduce(h->partials.as<float>(), n_part, 32, sums_out, h->stream));   // local rows only: see dev_ppr_mixed_body
+    HRAG_TRY(mixed_sums(h, n, n_part, sums_off));   // local rows only: see dev_ppr_mixed_body
     *result = y;
     return 0;
 }
@@ -201,24 +255,40 @@ SweepPlan plan_sweeps(const hrag_t* h, float alpha, int iters_arg, float tol_arg
     return plan_sweeps_raw(h->ppr_method, h->ppr_iters, h->mixed_m1, h->mixed_m2, alpha, iters_arg, tol_arg, want_mixed);
 }
 
-static int dev_ppr_mixed_body(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot_map, const float* Vexact,
-                              const void* rhs16, void* x0_dense, const float* scale, const double* vsum, void** X0,
+static int dev_ppr_mixed_body(hrag_t* h, const SweepPlan& plan, float alpha, int n, const MixedRhs* in, void** X0,
                               void** D) {
     double* sums = h->sums.as<double>();
-    HRAG_TRY(mixed_cheb(h, slot_map, rhs16, x0_dense, h->H[1], h->H[2], plan.m1, alpha, X0, sums + kSumX0));
-    void* other = (*X0 == h->H[1]) ? h->H[2] : h->H[1];
+    void* const* H = n == 2 ? h->HP : h->H;
+    const int* slot_map[2] = {in[0].slot_map, n == 2 ? in[1].slot_map : nullptr};
+    const void* rhs16[2] = {in[0].rhs16, n == 2 ? in[1].rhs16 : nullptr};
+    const float* vexact[2] = {in[0].Vexact, n == 2 ? in[1].Vexact : nullptr};
+    const float* scale[2] = {in[0].scale, n == 2 ? in[1].scale : nullptr};
+    void* x0_dense = in[0].x0_dense;
+    void* x0 = nullptr;
+    void* d = nullptr;
+    HRAG_TRY(mixed_cheb(h, n, slot_map, rhs16, x0_dense, H[1], H[2], plan.m1, alpha, &x0, kSumX0));
+    void* other = (x0 == H[1]) ? H[2] : H[1];
     int n_part = 0;
-    HRAG_TRY(mixed_sweep_x(h, 1, *X0, slot_map, nullptr, Vexact, scale, nullptr, h->H[3], alpha, 1.f, kMixedT,
-                           h->partials.as<float>(), &n_part));
-    h->stats.ppr_sweeps += 1;
-    h->stats.ppr_columns += 32;
-    HRAG_TRY(colsum_reduce(h->partials.as<float>(), n_part, 32, sums + kSumR, h->stream));
-    HRAG_TRY(mixed_cheb(h, nullptr, h->H[3], h->H[3], x0_dense, other, plan.m2, alpha, D, sums + kSumD));
+    const void* none[2] = {nullptr, nullptr};
+    HRAG_TRY(mixed_sweep_n(h, n, 1, x0, slot_map, none, vexact, scale, nullptr, H[3], alpha, 1.f, kMixedT, true,
+                           &n_part));
+    h->stats.ppr_sweeps += n;
+    h->stats.ppr_columns += 32 * n;
+    HRAG_TRY(mixed_sums(h, n, n_part, kSumR));
+    const int* dense[2] = {nullptr, nullptr};
+    const void* resid[2] = {H[3], H[3]};
+    HRAG_TRY(mixed_cheb(h, n, dense, resid, H[3], x0_dense, other, plan.m2, alpha, &d, kSumD));
     if (h->world > 1) {      // node-range sharding: every rank summed its own rows -- ONE all-reduce for the three sums
         StageTimer tc(h, ST_COMM);
         HRAG_NCCL(g_nccl.AllReduce(sums, sums, 96, ncclDouble, ncclSum, h->comm, h->stream));
     }
-    HRAG_TRY(residual_check(sums + kSumR, vsum, scale, 1.f / kMixedT, h->rho.as<float>(), h->stream));
+    for (int k = 0; k < n; ++k) {
+        const int off = k ? kSumPair : 0;
+        HRAG_TRY(residual_check(sums + off + kSumR, in[k].vsum, in[k].scale, 1.f / kMixedT, h->rho.as<float>(),
+                                h->stream));
+        X0[k] = pair_half(x0, k);
+        D[k] = pair_half(d, k);
+    }
     return 0;
 }
 
@@ -226,18 +296,18 @@ static int dev_ppr_mixed_body(hrag_t* h, const SweepPlan& plan, float alpha, con
 // single GPU it is captured once per (set, plan) into a CUDA graph and replayed (one launch per sub-batch instead of ~20:
 // what bounds small real graphs like MuSiQue-1k, where a sweep is a few microseconds of work).  Multi-GPU runs (epoch
 // values change per sweep) take the plain path.
-int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot_map, const float* Vexact,
-                  const void* rhs16, void* x0_dense, const float* scale, const double* vsum, void** X0, void** D) {
+int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, int n, const MixedRhs* in, void** X0, void** D) {
+    HRAG_CHECK(n == 1 || (n == 2 && h->world == 1), "internal: paired mixed solves run on a single GPU");
     StageTimer tm(h, ST_PPR);
     h->rho_dirty = true;     // set here, not in the body: the body runs on the host only while a graph is captured
     if (h->world > 1) {
-        HRAG_TRY(dev_ppr_mixed_body(h, plan, alpha, slot_map, Vexact, rhs16, x0_dense, scale, vsum, X0, D));
+        HRAG_TRY(dev_ppr_mixed_body(h, plan, alpha, n, in, X0, D));
         return p2p_wait(h);     // the consumers of X0 / D (gather kernels) need every peer's last rows
     }
     hrag_handle::SolveGraph* sg = nullptr;
     for (auto& c : h->solve_graphs)
-        if (c.x0 == x0_dense && c.slot_map == slot_map && c.rhs16 == rhs16 && c.vexact == Vexact && c.m1 == plan.m1 &&
-            c.m2 == plan.m2 && c.alpha == alpha && c.generation == g_buf_generation) sg = &c;
+        if (c.n == n && c.in[0] == in[0] && (n == 1 || c.in[1] == in[1]) && c.m1 == plan.m1 && c.m2 == plan.m2 &&
+            c.alpha == alpha && c.generation == g_buf_generation) sg = &c;
     if (sg == nullptr) {
         if (h->solve_graphs.size() >= 8) {                       // bounded cache: drop everything stale
             HRAG_CUDA(cudaStreamSynchronize(h->stream));         // none of them may still be executing
@@ -245,11 +315,12 @@ int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot
             h->solve_graphs.clear();
         }
         hrag_handle::SolveGraph c;
-        c.x0 = x0_dense; c.slot_map = slot_map; c.rhs16 = rhs16; c.vexact = Vexact; c.m1 = plan.m1; c.m2 = plan.m2;
-        c.alpha = alpha; c.generation = g_buf_generation;
+        c.n = n;
+        for (int k = 0; k < n; ++k) c.in[k] = in[k];
+        c.m1 = plan.m1; c.m2 = plan.m2; c.alpha = alpha; c.generation = g_buf_generation;
         const int64_t sw0 = h->stats.ppr_sweeps, col0 = h->stats.ppr_columns, l0 = launches_since_reset();
         HRAG_CUDA(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
-        const int rc = dev_ppr_mixed_body(h, plan, alpha, slot_map, Vexact, rhs16, x0_dense, scale, vsum, &c.X0, &c.D);
+        const int rc = dev_ppr_mixed_body(h, plan, alpha, n, in, c.X0, c.D);
         cudaGraph_t graph = nullptr;
         const cudaError_t ce = cudaStreamEndCapture(h->stream, &graph);
         HRAG_TRY(rc);
@@ -266,8 +337,10 @@ int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, const int* slot
     h->stats.ppr_sweeps += sg->sweeps;
     h->stats.ppr_columns += sg->columns;
     count_launch((int)sg->launches);
-    *X0 = sg->X0;
-    *D = sg->D;
+    for (int k = 0; k < n; ++k) {
+        X0[k] = sg->X0[k];
+        D[k] = sg->D[k];
+    }
     return 0;
 }
 
@@ -439,8 +512,12 @@ int hrag_ppr(hrag_t* h, int32_t B, const float* reset, float damping, int32_t it
             double* vsum = h->sums.as<double>() + kSumV;
             HRAG_TRY(mixed_prepare_rhs(h->V.as<float>(), (int64_t)N, damping, h->partials.as<float>(), vsum,
                                        h->mixed_aux.as<float>(), h->H[0], h->stream));
-            HRAG_TRY(dev_ppr_mixed(h, plan, damping, nullptr, h->V.as<float>(), h->H[0], h->H[0],
-                                   h->mixed_aux.as<float>(), vsum, &X0, &D));
+            MixedRhs in;
+            in.Vexact = h->V.as<float>();
+            in.rhs16 = in.x0_dense = h->H[0];
+            in.scale = h->mixed_aux.as<float>();
+            in.vsum = vsum;
+            HRAG_TRY(dev_ppr_mixed(h, plan, damping, 1, &in, &X0, &D));
             HRAG_TRY(state_to_scores_mixed(X0, D, 1.f / kMixedT, nb, N, h->sums.as<double>(),
                                            h->sums.as<double>() + 32, h->d_scores.as<float>(), h->stream));
             HRAG_TRY(p2p_signal(h));
