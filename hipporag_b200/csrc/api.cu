@@ -31,7 +31,7 @@ int sim_dispatch(hrag_t* h, const float* dQ, int Bq, int which, float* S, int64_
     }
     HRAG_TRY(split_queries(h, dQ, Bq, s));
     return sim_tc(h->q_hi.p, h->q_lo.p, Bq, h->emb[which].hi.p, h->emb[which].lo.p, h->emb[which].rows, h->dim,
-                  h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, S, ldS, nullptr, nullptr, n_ctas, s);
+                  h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, S, ldS, nullptr, nullptr, nullptr, n_ctas, s);
 }
 
 constexpr int kFusedTopK = 8;     // candidates the GEMM epilogue / row_minmax_topk keep in registers
@@ -67,12 +67,13 @@ int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, flo
         const int nt = sim_tc_n_tiles(F);
         HRAG_TRY(h->part_mm.ensure((size_t)Bq * nt * sizeof(float2)));
         HRAG_TRY(h->part_keys.ensure((size_t)Bq * nt * 8 * sizeof(uint64_t)));
+        HRAG_TRY(h->part_bound.ensure((size_t)Bq * sizeof(uint64_t)));
         {
             StageTimer tm(h, ST_SIM_FACT, s);
             HRAG_TRY(split_queries(h, d_qf, Bq, s));
             HRAG_TRY(sim_tc(h->q_hi.p, h->q_lo.p, Bq, h->emb[0].hi.p, h->emb[0].lo.p, F, h->dim,
                             h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, nullptr, 0, h->part_mm.as<float2>(),
-                            h->part_keys.as<uint64_t>(), n_ctas, s));
+                            h->part_keys.as<uint64_t>(), h->part_bound.as<uint64_t>(), n_ctas, s));
         }
         if (h->world > 1) {
             // facts are sharded by row range (SURVEY.md 8(e)): local GEMM + local top-8 -> all-gather of 8 candidates
@@ -301,15 +302,13 @@ int dev_stage_b_solve_f64(hrag_t* h, int Bq, const float* S, const float2* mm_pa
 
 // Persistent CTAs of the similarity GEMMs of chunk c + 1 while they share the GPU with chunk c's PPR sweeps in
 // hrag_retrieve_resident: enough SMs that the GEMMs finish within the sweeps, the rest stay with the sweeps (which
-// are bound by DRAM latency, not by SMs: on 132 - 56 SMs a K1m sweep takes 0.488 ms instead of 0.422).
-// Work per chunk of Bq queries: GEMM 2 n_seg Bq (F + P) dim FLOP, sweeps (non-zeros x sweeps per sub-batch x
-// sub-batches).  Rates measured at C3 on an H100 SXM (132 SMs, 700 W): K1m alone 34.4 G non-zeros/s (14.5 M in
-// 0.422 ms per sweep); K2 next to the sweeps 1.56 TFLOP/s per SM -- half its rate alone (3.0), as its TMA operand
-// loads queue behind the sweeps' gathers.  At C3 the rule gives 54; 48 and 56 measured the same step time, 40 and
-// 66 slower.  (Stage B's paired sweeps run at 46.0 G non-zeros/s per 32 columns; the scan has not been repeated
-// with them, so the rule keeps the rate it was tuned with.)
+// are bound by DRAM latency, not by SMs).  Work per chunk of Bq queries: GEMM 2 n_seg Bq (F + P) dim FLOP, sweeps
+// (non-zeros x 32-column sweeps per sub-batch x sub-batches).  Rates measured at C3 inside the overlapped step, with
+// paired sweeps and the bound-gated K2 epilogue, on an H100 SXM (132 SMs, 700 W) at G = 40: a paired sweep 0.381 ms
+// per 32 columns (38.0 G non-zeros/s); K2 2.49 TFLOP/s per SM, 0.73 of its rate alone (3.43), as its TMA operand
+// loads queue behind the sweeps' gathers.  DESIGN.md section 4 K2 has the scan of G.
 int overlap_ctas(const hrag_t* h, int Bq, const SweepPlan& plan) {
-    constexpr double kGemmFlopPerSmMs = 1.56e9, kSweepNnzPerMs = 3.44e7;
+    constexpr double kGemmFlopPerSmMs = 2.49e9, kSweepNnzPerMs = 3.80e7;
     const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
     const double gemm_flop = 2.0 * n_seg * Bq * (double)(h->emb[0].rows + h->emb[1].rows) * h->dim;
     const int64_t sweeps = plan.mixed ? (int64_t)(plan.m1 + 1 + plan.m2) * ceil_div(Bq, 32)
@@ -477,7 +476,8 @@ int hrag_stage_a(hrag_t* h, int32_t B, const float* q_fact, int32_t k, int32_t* 
         const int nb = (int)std::min<int64_t>(chunk, B - q0);
         HRAG_TRY(h2d(h, h->d_q.p, q_fact + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
         HRAG_TRY(dev_stage_a(h, nb, h->d_q.as<float>(), k, h->d_top_idx.as<int>() + q0 * k,
-                             h->d_top_score.as<float>() + q0 * k, h->d_nvalid.as<int>() + q0, h->stream, h->num_sms));
+                             h->d_top_score.as<float>() + q0 * k, h->d_nvalid.as<int>() + q0, h->stream,
+                             h->debug_sim_ctas > 0 ? h->debug_sim_ctas : h->num_sms));
     }
     if (B > 0) {
         HRAG_TRY(d2h(h, top_idx, h->d_top_idx.p, (size_t)B * k * sizeof(int)));
@@ -545,7 +545,7 @@ int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const fl
     const int64_t n_chunks = (B + chunk - 1) / chunk;
     const int k = link_top_k;
     // the per-chunk state the similarity part hands to the solve part: slot 0, and slot 1 when chunks overlap
-    const bool overlap = h->world == 1 && n_chunks >= 2;
+    const bool overlap = h->world == 1 && n_chunks >= 2 && h->debug_sim_ctas >= 0;
     hrag::Buf* top_idx[2] = {&h->d_top_idx, &h->pipe.top_idx};
     hrag::Buf* top_score[2] = {&h->d_top_score, &h->pipe.top_score};
     hrag::Buf* nvalid[2] = {&h->d_nvalid, &h->pipe.nvalid};
@@ -573,7 +573,8 @@ int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const fl
                                  top_score[s]->as<float>(), k, nullptr, damping, passage_node_weight, link_top_k, topk,
                                  iters, tol, d_out_ids + q0 * topk, d_out_scores + q0 * topk);
     };
-    if (!overlap) {   // one chunk, or node-range sharding (its all-gathers and spin-waiting sweeps must not share SMs)
+    // one chunk, node-range sharding (its all-gathers and spin-waiting sweeps must not share SMs), or hrag_debug_sim_ctas
+    if (!overlap) {
         for (int64_t c = 0; c < n_chunks; ++c) {
             HRAG_TRY(similarity(c, h->stream, h->num_sms));
             HRAG_TRY(solve(c));
@@ -583,7 +584,7 @@ int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const fl
     // Two streams: stream_sim runs chunk c + 1's similarity GEMMs on n_ctas SMs while `stream` runs chunk c's sweeps on
     // the others.  Every kernel computes what it computes on one stream, so the results are bit-identical.
     const SweepPlan plan = plan_sweeps(h, damping, iters, tol, h->ppr_precision == HRAG_PPR_MIXED && chunk > 16);
-    const int n_ctas = overlap_ctas(h, (int)chunk, plan);
+    const int n_ctas = h->debug_sim_ctas > 0 ? h->debug_sim_ctas : overlap_ctas(h, (int)chunk, plan);
     HRAG_CUDA(cudaEventRecord(h->ev_sim_start, h->stream));   // the caller's queries, ordered on `stream`
     HRAG_CUDA(cudaStreamWaitEvent(h->stream_sim, h->ev_sim_start, 0));
     HRAG_TRY(similarity(0, h->stream_sim, h->num_sms));        // nothing to overlap with yet: the whole GPU
@@ -805,6 +806,12 @@ int hrag_reset_stats(hrag_t* h) {
 int hrag_debug_keep_scores(hrag_t* h, int keep) {
     HRAG_CHECK(h, "hrag_debug_keep_scores: null handle");
     h->keep_fact_scores = keep != 0;
+    return 0;
+}
+
+int hrag_debug_sim_ctas(hrag_t* h, int n) {
+    HRAG_CHECK(h, "hrag_debug_sim_ctas: null handle");
+    h->debug_sim_ctas = n;
     return 0;
 }
 

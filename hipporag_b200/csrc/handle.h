@@ -150,6 +150,7 @@ struct hrag_handle {
     int ppr_batch = 16;
     int sim_mode = HRAG_SIM_BF16X3;
     bool keep_fact_scores = false;   // debugging: materialise S_fact even in tensor-core modes
+    int debug_sim_ctas = 0;          // hrag_debug_sim_ctas: > 0 GEMM CTAs, < 0 no chunk overlap, 0 defaults
     int ppr_precision = HRAG_PPR_MIXED;   // applies to batches of > 16 queries; smaller ones run fp32
     int mixed_m1 = 0, mixed_m2 = 0;   // 0 = derived from damping (8 / 7 at damping 0.5)
     double check_tol = 0.0, check_kappa = 0.0;   // > 0: this call's mixed solves are verified in resolve_spans
@@ -186,6 +187,7 @@ struct hrag_handle {
     int slot_maps_built = 0;                  // sets 0 .. slot_maps_built - 1 hold valid slot maps
     // scratch and I/O staging
     hrag::Buf S_fact, S_pass, mm_fact, mm_pass, mode, seed_vid, seed_w, q_hi, q_lo, part_mm, part_keys;
+    hrag::Buf part_bound;                 // fused stage A: [Bq] per-query bound on the 8th best key (sim_tc's scratch)
     hrag::Buf xr_mm, xr_keys;             // fact-sharded stage A: [world, Bq] min/max and [world, Bq, 8] best keys
     hrag::Buf d_q, d_q2, d_top_idx, d_top_score, d_nvalid, d_kept_idx, d_kept_score, d_dpr, d_out_ids, d_out_scores;
     hrag::Buf d_reset, d_scores;

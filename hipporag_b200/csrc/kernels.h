@@ -151,10 +151,13 @@ int sim_fp32(const float* Q, int Bq, const float* E, int64_t M, int dim, float* 
 int split_bf16(const float* x, int64_t n, void* hi, void* lo, cudaStream_t stream);
 // With part_mm / part_keys != null the epilogue is FUSED: no score matrix is written; per
 // (query, 256-column tile) it emits min/max (part_mm [Bq, n_tiles]) and the 8 best rank keys
-// (part_keys [Bq, n_tiles, 8]); merge_minmax_topk() finishes the selection.  The grid is persistent: n_ctas CTAs
-// (at most one per SM fits) walk the tiles; the outputs do not depend on n_ctas.
+// (part_keys [Bq, n_tiles, 8]); merge_minmax_topk() finishes the selection.  part_bound [Bq] is the fused epilogue's
+// scratch (zeroed on `stream` by this call): a per-query lower bound on the 8th best key, raised as tiles complete, below
+// which a tile list may drop keys (zero-padded; every tile key >= the bound that is in the tile's 8 best stays).  The
+// grid is persistent:
+// n_ctas CTAs (at most one per SM fits) walk the tiles; the merged outputs do not depend on n_ctas.
 int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const void* e_lo, int64_t M, int dim,
-           int n_seg, float* S, int64_t ldS, float2* part_mm, uint64_t* part_keys, int n_ctas,
+           int n_seg, float* S, int64_t ldS, float2* part_mm, uint64_t* part_keys, uint64_t* part_bound, int n_ctas,
            cudaStream_t stream);
 int sim_tc_n_tiles(int64_t M);
 // Threshold epilogue (index-time synonymy KNN, SURVEY.md 8(f)-2): no score matrix; every score >= thr is appended as

@@ -134,6 +134,7 @@ struct TcParams {
     // fused epilogue (FUSE): per (query, n-tile) min/max and the 8 best rank keys instead of scores
     float2* part_mm;          // [Bq, num_n_tiles]
     uint64_t* part_keys;      // [Bq, num_n_tiles, 8]
+    uint64_t* bound;          // [Bq] zeroed per launch: the largest 8th-best key of any tile list written so far
     // threshold epilogue (FUSE == 2, index-time synonymy KNN): every score >= thr is appended to its query's
     // candidate list as a rank key; cand_count keeps counting past cand_cap so overflow is detectable
     float thr;
@@ -150,6 +151,14 @@ __device__ __forceinline__ void insert_best(uint64_t (&best)[kFuseK], uint64_t k
         for (int k = 0; k < kFuseK; ++k)
             if (key > best[k]) { const uint64_t tmp = best[k]; best[k] = key; key = tmp; }
     }
+}
+// rank_key of an accumulator register read under a branch.  The bits are taken by an opaque move: a plain bitcast there
+// makes the compiler carry the accumulator across the tile loop in integer registers and copy it back before every
+// wgmma, which serialises the MMAs (ptxas C7511).
+__device__ __forceinline__ uint64_t acc_rank_key(float f, uint32_t idx) {
+    uint32_t u;
+    asm("mov.b32 %0, %1;" : "=r"(u) : "f"(f));
+    return rank_key(__uint_as_float(u), idx);
 }
 __device__ __forceinline__ void cmp_swap_desc(uint64_t& a, uint64_t& b) {
     const uint64_t hi = a > b ? a : b, lo = a > b ? b : a;
@@ -317,22 +326,38 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                         }
                 }
             } else if (FUSE == 1) {
+                // The query's bound is the 8th best key of some set of its scores, so it is at most its global 8th
+                // best: a key below it is in no top-k (k <= 8), and the tile's list may drop it.  Only scores that are
+                // not below `cut`, the score of the bound or of this lane's own 8th best key, go through insert_best,
+                // under a warp-uniform branch that is rarely taken once the bound has risen; min / max still see every
+                // valid column.  !(f < cut) keeps every key >= the bound, ties, -0.0 and NaNs included (the empty
+                // bound 0 decodes to a NaN cut, which passes everything).
+                const bool live = q < p.Bq;
+                const uint64_t thr = live ? __ldcg(reinterpret_cast<const unsigned long long*>(p.bound + q)) : 0ull;
+                float cut = key_score(thr);
                 float mn = INFINITY, mx = -INFINITY;
                 uint64_t best[kFuseK];
 #pragma unroll
                 for (int k = 0; k < kFuseK; ++k) best[k] = 0ull;
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j)
+                for (int j = 0; j < BN / 8; ++j) {
+                    bool pass[2];
 #pragma unroll
                     for (int c = 0; c < 2; ++c) {
                         const int col = 8 * j + c0 + c;
-                        if (col < n_valid) {
-                            const float f = d[4 * j + 2 * h + c];
-                            mn = fminf(mn, f);
-                            mx = fmaxf(mx, f);
-                            insert_best(best, rank_key(f, (uint32_t)(n0 + col)));
-                        }
+                        const float f = d[4 * j + 2 * h + c];
+                        const bool valid = col < n_valid;
+                        mn = valid ? fminf(mn, f) : mn;
+                        mx = valid ? fmaxf(mx, f) : mx;
+                        pass[c] = live && valid && !(f < cut);
                     }
+                    if (__any_sync(0xffffffffu, pass[0] || pass[1])) {
+#pragma unroll
+                        for (int c = 0; c < 2; ++c)
+                            if (pass[c]) insert_best(best, acc_rank_key(d[4 * j + 2 * h + c], (uint32_t)(n0 + 8 * j + c0 + c)));
+                        cut = key_score(best[kFuseK - 1] > thr ? best[kFuseK - 1] : thr);
+                    }
+                }
                 // merge the quad's four partial results: after two butterfly rounds every lane holds the row's
                 // min / max and its 8 best keys
 #pragma unroll
@@ -347,6 +372,10 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
 #pragma unroll
                     for (int k = 0; k < kFuseK; k += 2)
                         *reinterpret_cast<ulonglong2*>(p.part_keys + o * kFuseK + k) = make_ulonglong2(best[k], best[k + 1]);
+                    // a full list's 8th key is the 8th best of a subset of the query's scores: a valid bound in any
+                    // order of tiles and CTAs
+                    if (best[kFuseK - 1] > thr)
+                        atomicMax(reinterpret_cast<unsigned long long*>(p.bound + q), (unsigned long long)best[kFuseK - 1]);
                 }
             } else {
                 if (q < p.Bq) {
@@ -451,7 +480,7 @@ int sim_tc_threshold(const void* q_hi, const void* q_lo, int Bq, const void* e_h
     HRAG_TRY(make_map(&mel, e_lo, M, dim, bkc, BN));
     TcParams p;
     p.Bq = Bq; p.M = M; p.dim = dim; p.S = nullptr; p.ldS = 0; p.part_mm = nullptr; p.part_keys = nullptr;
-    p.thr = thr; p.cand_keys = cand_keys; p.cand_count = cand_count; p.cand_cap = cand_cap;
+    p.bound = nullptr; p.thr = thr; p.cand_keys = cand_keys; p.cand_count = cand_count; p.cand_cap = cand_cap;
     p.num_m_tiles = (int)ceil_div(Bq, BM);
     p.num_n_tiles = (int)ceil_div(M, BN);
     const int grid = (int)std::min<int64_t>((int64_t)p.num_m_tiles * p.num_n_tiles, num_sms);
@@ -463,9 +492,11 @@ int sim_tc_threshold(const void* q_hi, const void* q_lo, int Bq, const void* e_h
 }
 
 int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const void* e_lo, int64_t M, int dim,
-           int n_seg, float* S, int64_t ldS, float2* part_mm, uint64_t* part_keys, int n_ctas, cudaStream_t stream) {
+           int n_seg, float* S, int64_t ldS, float2* part_mm, uint64_t* part_keys, uint64_t* part_bound, int n_ctas,
+           cudaStream_t stream) {
     HRAG_CHECK(dim % 8 == 0, "sim_tc: embedding dim must be a multiple of 8 (TMA row pitch)");
     HRAG_CHECK(n_seg == 1 || n_seg == 4, "sim_tc: n_seg must be 1 (bf16) or 4 (split)");
+    HRAG_CHECK(part_mm == nullptr || (part_keys != nullptr && part_bound != nullptr), "sim_tc: fused buffers missing");
     if (Bq == 0 || M == 0) return 0;
     static bool attr_set = false;
     if (!attr_set) {
@@ -483,7 +514,9 @@ int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const v
     HRAG_TRY(make_map(&mel, e_lo, M, dim, bkc, BN));
     TcParams p;
     p.Bq = Bq; p.M = M; p.dim = dim; p.S = S; p.ldS = ldS; p.part_mm = part_mm; p.part_keys = part_keys;
+    p.bound = part_bound;
     const bool fuse = part_mm != nullptr;
+    if (fuse) HRAG_CUDA(cudaMemsetAsync(part_bound, 0, (size_t)Bq * sizeof(uint64_t), stream));
     p.thr = 0.f; p.cand_keys = nullptr; p.cand_count = nullptr; p.cand_cap = 0;
     HRAG_CHECK(fuse || (S != nullptr && ldS % 4 == 0), "sim_tc: score buffer missing");
     p.num_m_tiles = (int)ceil_div(Bq, BM);

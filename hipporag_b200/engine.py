@@ -503,6 +503,11 @@ class Engine:
         """Make stage A write the raw fact score matrix (tests); the default tensor-core epilogue is fused."""
         _lib.check(self._lib.hrag_debug_keep_scores(self._h, 1 if keep else 0))
 
+    def debug_sim_ctas(self, n: int = 0):
+        """Persistent CTAs of the similarity GEMMs (tests, benchmarks): n > 0 for stage_a and the overlapped GEMMs of
+        retrieve_resident, n < 0 runs retrieve_resident's chunks without the overlap, 0 restores the defaults."""
+        _lib.check(self._lib.hrag_debug_sim_ctas(self._h, int(n)))
+
     def debug_scores(self, which: int) -> np.ndarray:
         cols = self.n_facts if which == 0 else self.n_passages
         buf = np.empty(1024 * max(cols, 1), dtype=np.float32)

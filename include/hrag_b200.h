@@ -321,6 +321,11 @@ int hrag_debug_index(hrag_t* h, int plane, void* host_out, int64_t max_bytes, in
 /* keep != 0: stage A materialises the fact score matrix even in the tensor-core modes (whose
  * default epilogue selects min/max/top-k in registers and never writes scores). */
 int hrag_debug_keep_scores(hrag_t* h, int keep);
+/* Persistent CTAs of the similarity GEMMs (tests and benchmarks; the results do not depend on it).  n > 0: hrag_stage_a
+ * runs its GEMMs on n CTAs, and a multi-chunk hrag_retrieve_resident runs the overlapped GEMMs of chunk c + 1 on n
+ * CTAs instead of the count derived from the shapes; n < 0: hrag_retrieve_resident runs its chunks one after the
+ * other without the overlap; n = 0 restores the defaults. */
+int hrag_debug_sim_ctas(hrag_t* h, int n);
 
 #ifdef __cplusplus
 }

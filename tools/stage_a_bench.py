@@ -1,0 +1,123 @@
+#!/usr/bin/env python
+"""Stage A's fact GEMM (K2, k_sim_tc with the fused top-8 epilogue) alone, then the chunk-overlap scan of
+retrieve_resident.
+
+    python tools/stage_a_bench.py [--workload C3] [--reps 5] [--steps 2] [--scan 0,40,48,54,56,66] [--out FILE]
+
+K2 alone: stage_a on the workload's queries (1,024-query chunks) on the whole GPU; `ms_per_chunk` is the library's
+sim_fact span (bf16 split of the queries + the GEMM, CUDA events) divided by the chunks, the median of --reps calls.
+The scan: one retrieve_resident step (the bench.py step) per G, CUDA events around --steps steps after a warm-up step;
+G = 0 is the rule in overlap_ctas, G = -1 runs the chunks one after the other without the overlap.  The G values
+alternate within each of --rounds rounds.  One JSON line per measurement, then a summary with the card's name and
+power limit read in the same run.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import numpy as np  # noqa: E402
+
+import bench  # noqa: E402
+
+
+def card():
+    import torch
+    info = {"gpu": torch.cuda.get_device_name(0)}
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit"], info["max_sm_clock"] = [x.strip() for x in q.split(",")]
+    except (OSError, ValueError, subprocess.TimeoutExpired):
+        info["power_limit"] = "unknown"
+    return info
+
+
+def emit(rec, out):
+    line = json.dumps(rec)
+    print(line, flush=True)
+    if out:
+        with open(out, "a") as f:
+            f.write(line + "\n")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", default="C3")
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--steps", type=int, default=2)
+    ap.add_argument("--rounds", type=int, default=1)
+    ap.add_argument("--scan", default="0,-1,40,48,56,66")
+    ap.add_argument("--out", default="")
+    args = ap.parse_args()
+    import torch
+    from hipporag_b200 import Engine
+    device = torch.device("cuda", 0)
+    info = card()
+    w = bench.WORKLOADS[args.workload]
+    Q = w["queries"]
+    wl = bench.build_workload(args.workload, Q, device, 0)
+    kg = wl.kg
+    e = Engine(0)
+    e.load_graph_csr(kg.n_nodes, *wl.csr)
+    e.load_tables(kg.passage_vid, kg.fact_subj_vid, kg.fact_obj_vid, kg.ent_chunk_count)
+    e.load_embeddings(wl.fe, wl.pe)
+    chunks = -(-Q // 1024)
+    summary = {"workload": args.workload, "queries": Q, "facts": kg.n_facts, "dim": w["dim"], **info}
+
+    # ---- K2 alone
+    qf = wl.qf.cpu().numpy()
+    e.stage_a(qf, bench.LINK_TOP_K)                     # warm-up
+    k2 = []
+    for r in range(args.reps):
+        e.reset_stats()
+        e.stage_a(qf, bench.LINK_TOP_K)
+        ms = e.stats()["ms_sim_fact"] / chunks
+        k2.append(ms)
+        emit({"what": "k2_alone", "rep": r, "ms_per_chunk": round(ms, 3)}, args.out)
+    flop = 2.0 * 4 * 1024 * kg.n_facts * w["dim"]      # four split products per 1,024-query chunk
+    med = float(np.median(k2))
+    summary["k2_alone_ms_per_chunk"] = {"min": round(min(k2), 3), "median": round(med, 3), "max": round(max(k2), 3)}
+    summary["k2_alone_tflops_issued"] = round(flop / (med * 1e-3) / 1e12, 1)
+
+    # ---- G scan of retrieve_resident
+    out_ids = torch.empty((Q, bench.TOPK), dtype=torch.int32, device=device)
+    out_scores = torch.empty((Q, bench.TOPK), dtype=torch.float32, device=device)
+    stream = torch.cuda.ExternalStream(e.stream_ptr, device=device)
+    gs = [int(g) for g in args.scan.split(",") if g.strip()]
+    steps = {g: [] for g in gs}
+    for rnd in range(args.rounds):
+        for g in gs:
+            e.debug_sim_ctas(g)
+
+            def step():
+                e.retrieve_resident(wl.qf, wl.qp, out_ids, out_scores, bench.DAMPING, bench.PNW, bench.LINK_TOP_K,
+                                    bench.TOPK)
+            step()
+            torch.cuda.synchronize()
+            e.reset_stats()
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record(stream)
+            for _ in range(args.steps):
+                step()
+            e1.record(stream)
+            torch.cuda.synchronize()
+            ms = e0.elapsed_time(e1) / args.steps
+            st = e.stats()
+            sweeps = max(st["ppr_sweeps"], 1)
+            rec = {"what": "scan", "round": rnd, "G": g, "ms_per_step": round(ms, 1), "qps": round(Q / ms * 1e3, 1),
+                   "ms_sim_fact": round(st["ms_sim_fact"] / args.steps, 1), "ms_ppr": round(st["ms_ppr"] / args.steps, 1),
+                   "ms_ppr_per_sweep": round(st["ms_ppr"] / sweeps, 4)}
+            steps[g].append(ms)
+            emit(rec, args.out)
+    if gs:
+        e.debug_sim_ctas(0)
+    summary["scan_ms_per_step"] = {str(g): {"min": round(min(v), 1), "max": round(max(v), 1)} for g, v in steps.items()}
+    emit(summary, args.out)
+    e.close()
+
+
+if __name__ == "__main__":
+    main()
