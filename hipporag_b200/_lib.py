@@ -72,7 +72,11 @@ SIGNATURES = {
     "hrag_similarity": (C.c_int, [_p, C.c_int, _i32, _p, _p]),
     "hrag_topk_similarity": (C.c_int, [_p, C.c_int, _i32, _p, _i32, _p, _p]),
     "hrag_knn_threshold": (C.c_int, [_p, C.c_int, _i32, _p, _f32, _i32, _p, _p, _p]),
-    "hrag_bench_sweep": (C.c_int, [_p, _i32, _i32, _i32, C.POINTER(_f32)]),
+    "hrag_knn_index_update": (C.c_int, [_p, _i64, _i32, _p, C.c_int, _i64, _p, _f32, _i32, C.POINTER(_i32)]),
+    "hrag_knn_index_read": (C.c_int, [_p, _i64, _i64, _p, _p, _p]),
+    "hrag_knn_index_info": (C.c_int, [_p, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32)]),
+    "hrag_knn_index_clear": (C.c_int, [_p]),
+    "hrag_bench_sweep":(C.c_int, [_p, _i32, _i32, _i32, C.POINTER(_f32)]),
     "hrag_stream": (_p, [_p]),
     "hrag_get_stats": (C.c_int, [_p, C.POINTER(Stats)]),
     "hrag_reset_stats": (C.c_int, [_p]),

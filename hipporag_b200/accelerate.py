@@ -23,7 +23,8 @@ What is rebound (all paths under the reference's ``src/hipporag/``):
   applies the change to the device in place when it is an append or an ordered delete;
 * ``add_synonymy_edges`` (``:959-1020``) -- runs unchanged, but the ``retrieve_knn`` it calls
   (``utils/embed_utils.py:6-94``, imported into ``HippoRAG.py:35``) is the engine's fused
-  threshold KNN for the duration of the call (``hipporag_b200/knn.py``).
+  threshold KNN for the duration of the call (``hipporag_b200/knn.py``); with ``incremental=True`` the self-KNN stays
+  on the device and each call scores only what changed.
 
 ``linking_top_k`` (``config_utils.py:184``) may be anything in [1, 32] (<= 8 is selected inside the GEMM
 epilogue, larger values by an exact radix select); beyond 32 ``retrieve`` raises instead of clamping.
@@ -158,6 +159,18 @@ def _chunk_counts(rag, n, name_to_vid) -> np.ndarray:
     return cnt
 
 
+def _resident_knn_applies(query_ids, key_ids, query_vecs, key_vecs, thr: float) -> bool:
+    """Whether a ``retrieve_knn`` call is the self-KNN the resident index serves exactly: the same ids and vectors on
+    both sides, a non-empty [rows, dim] matrix with dim % 8 == 0, a threshold float32 does not round down."""
+    from . import knn
+    if list(query_ids) != list(key_ids) or len(key_ids) == 0 or not knn.resident_exact(thr):
+        return False
+    shape = np.shape(key_vecs)
+    if len(shape) != 2 or shape[0] != len(key_ids) or shape[1] % 8:
+        return False
+    return query_vecs is key_vecs or np.array_equal(np.asarray(query_vecs), np.asarray(key_vecs))
+
+
 def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_workers: int = 1,
                filter_chunk: int = 256, ppr_tol: float = 0.0, cache: bool = True, run_ppr_fp64: bool = False,
                incremental: bool = False, **engine_opts):
@@ -182,7 +195,11 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     ``extract_tables``), and after the reference's own ``prepare_retrieval_objects`` has run, the change is
     classified (``classify_update``): an append goes through ``Engine.append`` and an ordered delete through
     ``Engine.delete``, with only the new facts ``eval``-ed; anything else is the full reload.
-    ``rag._b200_state["last_update"]`` records which ran ("append", "delete" or "full").  Incremental updates do not
+    ``rag._b200_state["last_update"]`` records which ran ("append", "delete" or "full").  The synonymy KNN of
+    ``add_synonymy_edges`` is then kept on the engine as well (``knn.retrieve_knn_resident``): each call scores only
+    the entities added since the last one against the others (and lists that lost a neighbour they need), with the
+    same result as the per-call KNN; ``rag._b200_state["last_knn"]`` records what ran ("built", "updated",
+    "unchanged" or "per-call").  Incremental updates do not
     write the binary cache: the next cold start rebuilds it, as after any change today.  The default
     (``incremental=False``) loads the host-built CSR and reloads everything after ``index()`` / ``delete()``.
     ``engine_opts`` go to ``Engine.set_options``.
@@ -543,7 +560,9 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
 
     def add_synonymy_edges(self):
         """``HippoRAG.py:959-1020`` unchanged, with the KNN it calls (``:986-992``) served by the engine: cosine
-        >= synonymy_edge_sim_threshold selected inside the GEMM epilogue, no [chunk, N_ent] score matrix."""
+        >= synonymy_edge_sim_threshold selected inside the GEMM epilogue, no [chunk, N_ent] score matrix.  With
+        ``incremental=True`` the self-KNN is served from the engine's resident index, updated in place; other calls
+        (query ids != key ids, dim % 8 != 0, a threshold float32 rounds down, a rejected call) run per call."""
         import sys
         from . import knn
         mod = sys.modules[type(self).__module__]
@@ -551,6 +570,15 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         thr = float(self.global_config.synonymy_edge_sim_threshold)
 
         def fused_knn(query_ids, key_ids, query_vecs, key_vecs, k=2047, query_batch_size=1000, key_batch_size=10000):
+            if incremental and _resident_knn_applies(query_ids, key_ids, query_vecs, key_vecs, thr):
+                try:
+                    out, ran = knn.retrieve_knn_resident(_engine(), key_ids, key_vecs, k, thr, state.get("knn_keys"))
+                    state["knn_keys"], state["last_knn"] = list(key_ids), ran
+                    return out
+                except HragError as e:           # rejected (or the index was dropped): today's per-call path
+                    logger.warning(f"b200 resident synonymy KNN failed, running it per call: {e}")
+                    state["knn_keys"] = None
+            state["last_knn"] = "per-call"
             return knn.retrieve_knn(query_ids, key_ids, query_vecs, key_vecs, k=k, query_batch_size=query_batch_size,
                                     key_batch_size=key_batch_size, device=device, min_score=thr)
         mod.retrieve_knn = fused_knn

@@ -8,6 +8,8 @@
 //             + edges src/dst int32[E], w fp64[E]: the COO list as given, mutable handles only (index_update.cu)
 //   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N], slot_map[2 or 4][N] (node -> rhs slot) (resident)
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
+//   knn       self-KNN index (knn_index.cu): bf16 hi/lo [entities, d] x 2, ids / scores [entities, pad4(kmax + 1)]
+//             (only after hrag_knn_index_update; independent of the retrieval index)
 //   state     mixed solver: H0..H3, H0b [N, 32] fp16 in one IPC-exportable slab, and for paired solves HP0..HP3, HP0b
 //             [N, 2, 32] fp16 (two sub-batches interleaved row by row); fp32 solver: V, XA, XC [N, B] fp32
 //   rhs       compact: Vc [P + 2048, 32] fp32 (exact v) + R16 [P + 2048, 32] fp16 (scaled), two sets (double-buffered),
@@ -104,6 +106,18 @@ struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passag
     Buf own, hi, lo;              // hi / lo: bf16 split for the tensor-core path (dim % 8 == 0)
     int64_t rows = 0;             // rows held by THIS handle (node-range sharding: the rank's slice of the facts)
 };
+// The resident self-KNN index (knn_index.cu), independent of the retrieval index: the bf16 hi / lo planes of its unit
+// rows, and per row the first kmax keys with score >= thr, best first.  A list row is `width` = pad4(kmax + 1) int32
+// ids (-1 padded) / fp32 scores; ids[row * width + kmax] holds the row's flags (kKnnComplete: the list holds every key
+// >= thr).  held == false: no index (rows == 0 then too).
+struct KnnIndex {
+    Buf hi, lo, ids, scores;
+    int64_t rows = 0;
+    int dim = 0, kmax = 0, width = 0;
+    float thr = 0.f;
+    bool held = false;
+};
+constexpr int kKnnComplete = 1, kKnnRefill = 2;
 
 }  // namespace hrag
 
@@ -140,6 +154,7 @@ struct hrag_handle {
     hrag::SeedTables t;                // view of `tables`
     hrag::TableMem tables;
     hrag::EmbMem emb[2];
+    hrag::KnnIndex knn;                // hrag_knn_index_update: the synonymy KNN of the entities, kept between calls
     int num_sms = 132;
     int64_t fact_row_lo = 0;        // first global fact row of the local slice
     int64_t n_facts_global = 0;
@@ -315,6 +330,14 @@ int install_graph(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, in
 
 // index_update.cu: *out = a copy of a device edge list of n edges (what a mutable handle keeps).
 int copy_edge_list(hrag_t* h, int64_t n, const int32_t* src, const int32_t* dst, const double* w, EdgeList* out);
+// Grows b to `need` bytes (by half its capacity at least), keeping its first `used` bytes.
+int grow_keep(hrag_t* h, Buf& b, size_t used, size_t need);
+// In place: rows [0, n_new) of the plane at `base` become its rows row_src[0 .. n_new) (device, ascending), rows
+// before `first` staying put; row_bytes % 16 == 0; staging is a bounded scratch buffer.
+int compact_rows(hrag_t* h, void* base, size_t row_bytes, int64_t n_new, int64_t first, const int* row_src,
+                 Buf& staging);
+// out row r = base row row_src[r] (device), r < n_rows, on h->stream; row_bytes % 16 == 0.
+int gather_rows(hrag_t* h, const void* base, size_t row_bytes, const int* row_src, int64_t n_rows, void* out);
 
 int exchange_rows(hrag_t* h, float* y, int B);
 int p2p_wait(hrag_t* h);

@@ -116,6 +116,8 @@ __global__ void k_count_bad_edges(int64_t n, int64_t n_nodes, const int32_t* __r
     if (i < n && (src[i] < 0 || src[i] >= n_nodes || dst[i] < 0 || dst[i] >= n_nodes)) atomicAdd(bad, 1ull);
 }
 
+}  // namespace
+
 // Grows b to hold `need` bytes, keeping its first `used` bytes: by half its capacity at least, so a stream of small
 // appends copies a plane O(log) times, not once per append.
 int grow_keep(hrag_t* h, Buf& b, size_t used, size_t need) {
@@ -127,6 +129,8 @@ int grow_keep(hrag_t* h, Buf& b, size_t used, size_t need) {
     b = std::move(nb);
     return 0;
 }
+
+namespace {
 
 // Copies n elements from host (counted in h2d_bytes) or device memory to dst, on h->stream.
 template <class T> int copy_in(hrag_t* h, T* dst, const T* src, int64_t n, bool on_device) {
@@ -160,6 +164,8 @@ int scan_flags(hrag_t* h, int64_t n, const int* flags, int* pos, int64_t* kept, 
     return 0;
 }
 
+}  // namespace
+
 // Rows [0, n_new) of the plane at `base` (rows of row_bytes, a multiple of 16) become its rows row_src[0 .. n_new),
 // in place; rows before `first` (row_src[i] == i there) do not move.  row_src is ascending, so row_src[i] >= i:
 // destinations never lie after their sources.  The rows move chunk by chunk through a bounded staging buffer, each
@@ -182,6 +188,17 @@ int compact_rows(hrag_t* h, void* base, size_t row_bytes, int64_t n_new, int64_t
     }
     return 0;
 }
+
+int gather_rows(hrag_t* h, const void* base, size_t row_bytes, const int* row_src, int64_t n_rows, void* out) {
+    if (n_rows == 0) return 0;
+    const int64_t w16 = (int64_t)(row_bytes / 16);
+    k_gather_rows<<<blocks_for(n_rows * w16), kThreads, 0, h->stream>>>(n_rows, w16, row_src, 0, (const int4*)base,
+                                                                          static_cast<int4*>(out));
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+namespace {
 
 bool borrowed(const EmbMem& e) { return e.f32 != nullptr && e.own.p == nullptr; }
 // the fp32 rows a fresh load of this matrix keeps: an owned matrix, or an empty one (loaded from host memory, it

@@ -480,6 +480,53 @@ class Engine:
                                                 _ptr(scores), _ptr(found)))
         return ids, scores, found
 
+    # ---------------------------------------------------------------- resident self-KNN (synonymy edges)
+    def knn_index_update(self, emb, kept_from=None, min_score: float = 0.8, kmax: int = 128) -> int:
+        """Keep the self-KNN of ``emb`` ([rows, dim] fp32 unit rows, numpy or a contiguous CUDA tensor on the handle's
+        device) on the device (``hrag_knn_index_update``): per row the first ``kmax`` rows with dot product >=
+        ``min_score``, best first.  ``kept_from[i]`` (strictly increasing) is the row held before that is now row i,
+        for the first ``len(kept_from)`` rows; the rest are new.  ``None`` builds from scratch.  Returns 0 built,
+        1 updated, 2 unchanged."""
+        if hasattr(emb, "is_cuda"):
+            if not (emb.is_cuda and emb.device.index == self.device and emb.is_contiguous()
+                    and str(emb.dtype) == "torch.float32" and emb.dim() == 2):
+                raise ValueError("device rows must be a contiguous 2-D fp32 CUDA tensor on the handle's device")
+            import torch
+            torch.cuda.current_stream(self.device).synchronize()
+            ptr, (rows, dim), on_dev, keep = C.c_void_p(emb.data_ptr()), tuple(emb.shape), 1, emb
+        else:
+            keep = _f32(emb)
+            if keep.ndim != 2:
+                raise ValueError("rows must be a 2-D array")
+            ptr, (rows, dim), on_dev = _ptr(keep), keep.shape, 0
+        kf = None if kept_from is None else np.ascontiguousarray(kept_from, dtype=np.int64).reshape(-1)
+        n_kept = 0 if kf is None else int(kf.shape[0])
+        if kf is not None and n_kept == 0:
+            kf = np.zeros(1, np.int64)                      # an empty kept_from is not NULL (NULL = build)
+        mode = C.c_int32()
+        _lib.check(self._lib.hrag_knn_index_update(self._h, int(rows), int(dim), ptr, on_dev, n_kept, _ptr(kf),
+                                                   float(min_score), int(kmax), C.byref(mode)))
+        del keep                                            # alive until the call has returned
+        return int(mode.value)
+
+    def knn_index_info(self) -> Tuple[int, int, int]:
+        """(rows, dim, kmax) of the resident self-KNN index, zeros when none is held."""
+        rows, dim, kmax = C.c_int64(), C.c_int32(), C.c_int32()
+        _lib.check(self._lib.hrag_knn_index_info(self._h, C.byref(rows), C.byref(dim), C.byref(kmax)))
+        return int(rows.value), int(dim.value), int(kmax.value)
+
+    def knn_index_read(self):
+        """The resident self-KNN lists: (ids [rows, kmax] int32, -1 padded; scores [rows, kmax] fp32, 0 padded)."""
+        rows, _, kmax = self.knn_index_info()
+        ids = np.empty((rows, kmax), dtype=np.int32)
+        scores = np.empty((rows, kmax), dtype=np.float32)
+        _lib.check(self._lib.hrag_knn_index_read(self._h, 0, rows, _ptr(ids), _ptr(scores), None))
+        return ids, scores
+
+    def knn_index_clear(self):
+        """Drop the resident self-KNN index and free its memory."""
+        _lib.check(self._lib.hrag_knn_index_clear(self._h))
+
     def bench_sweep(self, batch: int, sweeps: int = 20, method: int = PPR_POWER) -> float:
         ms = C.c_float()
         _lib.check(self._lib.hrag_bench_sweep(self._h, batch, sweeps, method, C.byref(ms)))

@@ -287,6 +287,31 @@ int hrag_topk_similarity(hrag_t* h, int which, int32_t B, const float* q, int32_
 int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float min_score, int32_t kmax,
                        int32_t* out_ids, float* out_scores, int32_t* n_found);
 
+/* The self-KNN of add_synonymy_edges (HippoRAG.py:980-992: every entity against every entity) kept on the device
+ * between calls and updated in place when the entity store changes.  The handle holds one such index, independent of
+ * the retrieval index (no graph or mutable handle needed; hrag_index_append / hrag_index_delete leave it alone): the
+ * bf16 hi / lo planes of its rows and, per row, the first kmax rows with dot product >= min_score, best first (score
+ * desc, row asc) -- after every call exactly what hrag_knn_threshold(rows, rows, min_score, kmax) on a fresh handle,
+ * with the rows whose n_found exceeds 512 redone through hrag_topk_similarity and cut at min_score, gives for the rows
+ * of this call, bit for bit (split bf16 x 4 products whatever hrag_set_options chose).
+ *
+ * emb: [rows, dim] fp32 rows in the NEW order (host, or a device pointer if on_device), dim % 8 == 0.  Row i < n_kept
+ * is the row held at kept_from[i] (strictly increasing), rows >= n_kept are new: only the new keys are scored against
+ * the kept rows, and only new rows and lists that lost a listed key without holding every key >= min_score are scored
+ * against all keys.  Kept rows are verified against the planes held: a changed vector rebuilds.  kept_from == NULL, no
+ * index held, or a changed min_score, kmax (in [1, 512]) or dim builds from scratch.  *mode: 0 built, 1 updated, 2
+ * unchanged (no GEMM ran).  Every argument is checked before the index is touched (a rejected call leaves it as it
+ * was); a failure after that (out of memory) clears it.  Rejected on a node-range-sharded handle (world > 1).  Device
+ * memory: 4 dim + 8 pad4(kmax + 1) bytes per row, capacity grown by half at a time. */
+int hrag_knn_index_update(hrag_t* h, int64_t rows, int32_t dim, const float* emb, int on_device, int64_t n_kept,
+                          const int64_t* kept_from, float min_score, int32_t kmax, int32_t* mode);
+/* Rows [row0, row0 + n) of the index: ids / scores [n, kmax] (host, -1 / 0 padded), n_valid[n] (may be NULL). */
+int hrag_knn_index_read(hrag_t* h, int64_t row0, int64_t n, int32_t* ids, float* scores, int32_t* n_valid);
+/* What the index holds: *rows, *dim and *kmax (all 0 when no index is held). */
+int hrag_knn_index_info(hrag_t* h, int64_t* rows, int32_t* dim, int32_t* kmax);
+/* Drops the index and frees its memory. */
+int hrag_knn_index_clear(hrag_t* h);
+
 /* K1 micro-benchmark: runs `sweeps` SpMM sweeps at batch width B on resident synthetic
  * state and returns the average milliseconds per sweep (CUDA events on the launch stream).
  * method: 0 power / 1 Chebyshev (fp32 state), 2 fp16 state with a dense rhs, 3 fp16 state with the

@@ -41,6 +41,14 @@ m.delete(np.array([0, 11, N + 1], np.int32), np.array([1, 4], np.int32),
          np.delete(np.r_[kg.ent_chunk_count, [1, 2, 0]], [0, 11, N + 1]).astype(np.int32))
 idx, score, nv = m.stage_a(qf, 5)
 m.stage_b(qp, idx, score, topk=50)
+# the resident synonymy KNN (knn_index.cu): a build with overflowing rows, then an append + delete update
+rng = np.random.default_rng(4)
+ent = rng.choice([-1.0, 1.0], size=(1500, 64)).astype(np.float32)
+ent[:600, :48] = ent[0, :48]
+ent /= 8
+m.knn_index_update(ent, None, 0.375, 128)
+m.knn_index_update(np.concatenate([ent[3:], ent[:40]]), np.arange(3, 1500), 0.375, 128)
+m.knn_index_read()
 print("driver ok", ids.shape)
 PY
 compute-sanitizer --tool $TOOL --error-exitcode 7 python /tmp/hrag_sanitize_driver.py 2>&1 | tail -15
