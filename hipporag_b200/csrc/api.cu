@@ -157,16 +157,8 @@ int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d
     const SweepPlan plan = plan_sweeps(h, damping, iters_arg, tol_arg, h->ppr_precision == HRAG_PPR_MIXED && Bq > 16);
     const bool mixed = plan.mixed;
     const int Bp = mixed ? 32 : round_batch(std::min(h->ppr_batch, Bq));
-    // single GPU: consecutive sub-batches are solved in pairs, one walk of the CSR per sweep for both (an odd last one
-    // alone); node-range sharding solves them one by one (its exchange is fused into the single-state sweep)
-    const bool pairs = mixed && k_facts > 0 && h->world == 1 && Bq > 32;
-    if (mixed) {
-        HRAG_TRY(ensure_state_mixed(h));
-        if (pairs) HRAG_TRY(ensure_state_pair(h));
-        HRAG_TRY(ensure_compact_rhs(h, pairs ? 4 : 2));
-    } else {
-        HRAG_TRY(ensure_state(h, Bp));
-    }
+    if (mixed) HRAG_TRY(ensure_stage_b_mixed(h, Bq, k_facts));
+    else HRAG_TRY(ensure_state(h, Bp));
     HRAG_TRY(h->seed_vid.ensure((size_t)Bq * kSeedSlots * sizeof(int)));     // [Bq, kSeedSlots] seed slots
     HRAG_TRY(h->seed_w.ensure((size_t)Bq * kSeedSlots * sizeof(double)));
     {
@@ -178,59 +170,7 @@ int dev_stage_b_solve(hrag_t* h, int Bq, float* S, float2* mm_pass, const int* d
         StageTimer tm(h, ST_TOPK);
         HRAG_TRY(minmax_apply(S, Bq, P, ld, mm_pass, h->stream));
     }
-    if (mixed && k_facts > 0) {
-        // Two streams: stream2 builds solve i+1's compact right-hand sides (passage weights + phrase seeds on
-        // P + 2048 slots, column scales, the fp16 copy and the dense first iterate) while `stream` runs the sweeps of
-        // solve i.  Solve i (one sub-batch, or a pair) uses the sets of parity i & 1: set p, and p + 2 for the second
-        // sub-batch of a pair.
-        if (plan.check) h->check_tol = std::max(h->check_tol, plan.tol), h->check_kappa = plan.kappa;
-        HRAG_CUDA(cudaEventRecord(h->ev_inputs, h->stream));            // S, min/max, seed lists are ready
-        HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_inputs, 0));
-        int it = 0;
-        for (int q0 = 0; q0 < Bq; ++it) {
-            const int n = pairs && Bq - q0 > 32 ? 2 : 1;
-            const int par = it & 1;
-            if (it >= 2) HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_released[par], 0));   // sets are free again
-            MixedRhs in[2];
-            int nb[2] = {0, 0};
-            for (int k = 0; k < n; ++k) {
-                const int set = par + 2 * k, qk = q0 + 32 * k;
-                nb[k] = std::min(32, Bq - qk);
-                void* pair_x0 = par ? h->HP0b : h->HP[0];
-                in[k].x0_dense = n == 2 ? pair_x0 : (par ? h->H0b : h->H[0]);
-                in[k].slot_map = h->slot_map[set].as<int>();
-                in[k].Vexact = h->Vc[set].as<float>();
-                in[k].rhs16 = h->R16[set].p;
-                in[k].scale = set_scale(h, set);
-                in[k].vsum = h->sums.as<double>() + kSumV + 32 * set;
-                HRAG_TRY(compact_prepare_rhs(h->t, nb[k], qk, S, ld, mm_pass, pnw, kSeedSlots, h->seed_vid.as<int>(),
-                                             h->seed_w.as<double>(), damping, h->slot_map[set].as<int>(),
-                                             h->slot_vid[set].as<int>(), h->Vc[set].as<float>(), h->R16[set].p,
-                                             static_cast<char*>(in[k].x0_dense) + 64 * k, 32 * n,
-                                             (int64_t)h->g.n_global, h->prep_scratch.as<float>(),
-                                             h->sums.as<double>() + kSumV + 32 * set, set_scale(h, set), h->stream2));
-            }
-            HRAG_CUDA(cudaEventRecord(h->ev_ready[par], h->stream2));
-            HRAG_CUDA(cudaStreamWaitEvent(h->stream, h->ev_ready[par], 0));
-            void *X0[2] = {nullptr, nullptr}, *D[2] = {nullptr, nullptr};
-            HRAG_TRY(dev_ppr_mixed(h, plan, damping, n, in, X0, D));
-            {
-                StageTimer tm(h, ST_TOPK);
-                for (int k = 0; k < n; ++k) {
-                    const double* sums = h->sums.as<double>() + (k ? kSumPair : 0);
-                    HRAG_TRY(gather_passage_scores_mixed(h->t, nb[k], q0 + 32 * k, X0[k], D[k], 32 * n, 1.f / kMixedT,
-                                                         sums + kSumX0, sums + kSumD, h->mode.as<int>(), mm_pass, S, ld,
-                                                         h->stream));
-                    HRAG_TRY(compact_release_slots(P, nb[k], q0 + 32 * k, kSeedSlots, h->seed_vid.as<int>(),
-                                                   h->slot_map[par + 2 * k].as<int>(), h->stream));
-                }
-            }
-            HRAG_TRY(p2p_signal(h));   // peers may overwrite this rank's state buffers from here on
-            HRAG_CUDA(cudaEventRecord(h->ev_released[par], h->stream));
-            q0 += 32 * n;
-        }
-        // (every prepare was consumed by a solve on `stream`, so stream2 is drained in stream order)
-    }
+    if (mixed && k_facts > 0) HRAG_TRY(stage_b_mixed(h, plan, Bq, S, ld, mm_pass, pnw, damping));
     for (int q0 = 0; q0 < Bq && k_facts > 0 && !mixed; q0 += Bp) {
         const int nb = std::min(Bp, Bq - q0);
         {
@@ -420,7 +360,7 @@ void hrag_destroy(hrag_t* h) {
     cudaStreamSynchronize(h->stream);
     if (h->stream_sim) cudaStreamSynchronize(h->stream_sim);
     if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
-    for (auto& c : h->solve_graphs) cudaGraphExecDestroy(c.exec);
+    drop_captured_solves(h);
     for (auto e : h->pool) cudaEventDestroy(e);
     for (void* p : h->peer_slab) if (p) cudaIpcCloseMemHandle(p);
     for (cudaEvent_t e : {h->ev_ready[0], h->ev_ready[1], h->ev_released[0], h->ev_released[1], h->ev_inputs,
@@ -703,86 +643,6 @@ int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float mi
         HRAG_CUDA(cudaStreamSynchronize(h->stream));
     }
     return resolve_spans(h);
-}
-
-int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float* ms_per_sweep) {
-    HRAG_CHECK(h && ms_per_sweep && sweeps >= 1, "hrag_bench_sweep: bad arguments");
-    HRAG_CHECK(B == 4 || B == 8 || B == 16 || B == 32 || B == 64, "hrag_bench_sweep: B in {4,8,16,32,64}");
-    HRAG_CHECK(h->g.n_global > 0, "hrag_bench_sweep: graph not loaded");
-    HRAG_CUDA(cudaSetDevice(h->device));
-    // fp16-state sweep (Chebyshev form), B = 32: 2 = dense rhs, 3 = compact rhs, 4 = the paired sweep of two
-    // compact-rhs sub-batches ([N, 2, 32] state), timed per paired sweep (64 columns)
-    const bool paired = method == 4;
-    const bool mixed = method == 2 || method == 3 || paired;
-    HRAG_CHECK(!paired || h->world == 1, "hrag_bench_sweep: the paired sweep runs on a single-GPU handle");
-    const bool cheb = method == HRAG_PPR_CHEBYSHEV;
-    const int* slot_map = nullptr;
-    const void* rhs = nullptr;
-    void *A = nullptr, *C = nullptr;
-    if (mixed) {
-        HRAG_CHECK(B == 32, "hrag_bench_sweep: the mixed solver runs at B = 32");
-        HRAG_TRY(ensure_state_mixed(h));
-        rhs = h->H[0];
-        if (method >= 3) {
-            HRAG_CHECK(h->t.passage_vid != nullptr, "hrag_bench_sweep: the compact-rhs sweep needs hrag_load_tables");
-            HRAG_TRY(ensure_compact_rhs(h, 2));
-            slot_map = h->slot_map[0].as<int>();
-            rhs = h->R16[0].p;
-            for (int s = 0; s < 2; ++s) HRAG_CUDA(cudaMemsetAsync(h->R16[s].p, 0x2c, h->R16[s].cap, h->stream));
-        }
-        const size_t hb = (size_t)h->g.n_global * 32 * 2;
-        for (int i = 0; i < 3; ++i) HRAG_CUDA(cudaMemsetAsync(h->H[i], 0x2c, hb, h->stream));   // 0x2c2c = 0.065
-        A = h->H[1], C = h->H[2];
-        if (paired) {
-            HRAG_TRY(ensure_state_pair(h));
-            for (int i = 1; i < 3; ++i) HRAG_CUDA(cudaMemsetAsync(h->HP[i], 0x2c, 2 * hb, h->stream));
-            A = h->HP[1], C = h->HP[2];
-        }
-    } else {
-        HRAG_TRY(ensure_state(h, B));
-        const size_t bytes = (size_t)h->g.n_global * B * sizeof(float);
-        HRAG_CUDA(cudaMemsetAsync(h->V.p, 0x3c, bytes, h->stream));     // 0x3c3c3c3c = 0.0115f
-        HRAG_CUDA(cudaMemsetAsync(h->XA.p, 0x3c, bytes, h->stream));
-        HRAG_CUDA(cudaMemsetAsync(h->XC.p, 0x3c, bytes, h->stream));
-        A = h->XA.p, C = h->XC.p;
-    }
-    cudaEvent_t e0, e1;
-    HRAG_CUDA(cudaEventCreate(&e0));
-    HRAG_CUDA(cudaEventCreate(&e1));
-    for (int pass = 0; pass < 2; ++pass) {   // pass 0 = warm-up (3 sweeps), pass 1 = timed
-        const int n = pass == 0 ? 3 : sweeps;
-        if (pass == 1) HRAG_CUDA(cudaEventRecord(e0, h->stream));
-        for (int i = 0; i < n; ++i) {
-            void* x = (i & 1) ? C : A;
-            void* y = (i & 1) ? A : C;
-            float* yf = static_cast<float*>(y);
-            if (paired) {
-                MixedSweepIO io[2];
-                for (int k = 0; k < 2; ++k) {
-                    io[k].xh = static_cast<char*>(x) + 64 * k;
-                    io[k].slot_map = h->slot_map[k].as<int>();
-                    io[k].rhs_h = h->R16[k].p;
-                    io[k].prevh = io[k].yh = static_cast<char*>(y) + 64 * k;
-                }
-                HRAG_TRY(mixed_sweep2(h->g, 0, io, 0.5f, 1.07f, 1.f, nullptr, nullptr, h->stream));
-            } else if (mixed) {
-                HRAG_TRY(mixed_sweep_x(h, 0, x, slot_map, rhs, nullptr, nullptr, y, y, 0.5f, 1.07f, 1.f, nullptr, nullptr));
-            }
-            else HRAG_TRY(ppr_sweep(h->g, B, static_cast<float*>(x), h->V.as<float>(), cheb ? yf : nullptr, yf, 0.5f,
-                                    cheb ? 1.07f : 1.f, nullptr, nullptr, h->stream));
-            if (!mixed) HRAG_TRY(exchange_rows(h, yf, B));
-        }
-        if (pass == 1) HRAG_CUDA(cudaEventRecord(e1, h->stream));
-    }
-    HRAG_CUDA(cudaStreamSynchronize(h->stream));
-    float ms = 0.f;
-    HRAG_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0);
-    cudaEventDestroy(e1);
-    *ms_per_sweep = ms / sweeps;
-    for (auto& s : h->spans) { h->pool.push_back(s.a); h->pool.push_back(s.b); }
-    h->spans.clear();
-    return 0;
 }
 
 void* hrag_stream(hrag_t* h) { return h ? (void*)h->stream : nullptr; }

@@ -55,9 +55,6 @@ int exchange_rows_bytes(hrag_t* h, void* y, size_t row_bytes) {
 }
 int exchange_rows(hrag_t* h, float* y, int B) { return exchange_rows_bytes(h, y, (size_t)B * sizeof(float)); }
 
-static unsigned long long* local_flags(hrag_t* h) {
-    return reinterpret_cast<unsigned long long*>(static_cast<char*>(h->slab.p) + 5 * h->slab_hb);
-}
 PeerOut peers_for(hrag_t* h, void* y) {
     PeerOut po;
     if (!h->p2p) return po;
@@ -73,16 +70,14 @@ PeerOut peers_for(hrag_t* h, void* y) {
 SweepSync sync_for_sweep(hrag_t* h) {
     SweepSync sy;
     if (!h->p2p) return sy;
-    sy.flags = local_flags(h);
+    sy.flags = epoch_flags(h, h->slab.p);
     sy.need = h->epoch;
     sy.world = h->world;
     sy.rank = h->rank;
     sy.error_flag = h->p2p_err.as<int>();
     sy.done_ctr = h->done_ctr.as<unsigned int>();
     for (int r = 0; r < h->world; ++r)
-        if (r != h->rank)
-            sy.remote[sy.n_remote++] = reinterpret_cast<unsigned long long*>(static_cast<char*>(h->peer_slab[r]) +
-                                                                              5 * h->slab_hb) + h->rank;
+        if (r != h->rank) sy.remote[sy.n_remote++] = epoch_flags(h, h->peer_slab[r]) + h->rank;
     h->epoch += 1;
     sy.epoch = h->epoch;
     return sy;
@@ -102,13 +97,11 @@ int p2p_signal(hrag_t* h) {
     return epoch_signal(sy, h->stream);
 }
 // one fp16 sweep + its exchange: fused peer stores (K5) when the peers are mapped, NCCL all-gather otherwise
-int mixed_sweep_x(hrag_t* h, int mode, const void* x, const int* slot_map, const void* rhs, const float* v32,
-                  const float* scale, const void* prev, void* y, float alpha, float w, float t, float* part,
-                  int* n_part) {
-    int* overflow = h->rho.p ? h->rho.as<int>() + 1 : nullptr;
-    HRAG_TRY(mixed_sweep(h->g, mode, x, slot_map, rhs, v32, scale, prev, y, alpha, w, t, part, n_part, overflow,
-                         peers_for(h, y), sync_for_sweep(h), h->stream));
-    if (!h->p2p) HRAG_TRY(exchange_rows_bytes(h, y, 32 * 2));
+int mixed_sweep_x(hrag_t* h, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_part,
+                  int* overflow) {
+    HRAG_TRY(mixed_sweep(h->g, mode, io, alpha, w, t, n_part, overflow, peers_for(h, io.yh), sync_for_sweep(h),
+                         h->stream));
+    if (!h->p2p) HRAG_TRY(exchange_rows_bytes(h, io.yh, 32 * 2));
     return 0;
 }
 

@@ -245,13 +245,13 @@ int install_graph(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t row_hi, in
     g.max_batch = 64;
     const int n_rows = g.n_rows;
 
-    // every input is valid: the old graph and the fp32 state sized for it go first (a reload never holds two graphs;
-    // the frees bump g_buf_generation, which invalidates every captured solve); the new graph becomes the handle's
+    // every input is valid: the old graph, the fp32 state sized for it, the slot maps and the captured solves go first
+    // (a reload never holds two graphs); the new graph becomes the handle's
     // only once all of it is built (a failure leaves no graph; the next load frees what was allocated)
+    HRAG_TRY(invalidate_solves(h));
     h->graph = GraphMem{};
     h->g = PprGraph();
     h->V.reset(); h->XA.reset(); h->XC.reset(); h->partials.reset();
-    h->slot_maps_valid = false;
     h->row_bounds = bounds;
     h->chunk_rows = h->world > 1 ? ceil_div(n_nodes, h->world) : n_nodes;
     GraphMem& m = h->graph;

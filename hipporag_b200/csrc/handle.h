@@ -6,14 +6,14 @@
 //   graph     row_ptr int32[n_rows+1], cv int2[nnz] {col, fp32 bits of P[i,j]}, row_order int32[n_rows]   (resident)
 //             + val_lo fp32[nnz] = fp32(P64 - hi) when loaded from float64 values (the fp64 solver's operator)
 //             + edges src/dst int32[E], w fp64[E]: the COO list as given, mutable handles only (index_update.cu)
-//   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N], slot_map[2 or 4][N] (node -> rhs slot) (resident)
+//   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N]                                         (resident)
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
 //   knn       self-KNN index (knn_index.cu): bf16 hi/lo [entities, d] x 2, ids / scores [entities, pad4(kmax + 1)]
 //             (only after hrag_knn_index_update; independent of the retrieval index)
-//   state     mixed solver: H0..H3, H0b [N, 32] fp16 in one IPC-exportable slab, and for paired solves HP0..HP3, HP0b
+//   state     mixed solver: x0[2], A, C, R [N, 32] fp16 in one IPC-exportable slab, and for paired solves the same
 //             [N, 2, 32] fp16 (two sub-batches interleaved row by row); fp32 solver: V, XA, XC [N, B] fp32
-//   rhs       compact: Vc [P + 2048, 32] fp32 (exact v) + R16 [P + 2048, 32] fp16 (scaled), two sets (double-buffered),
-//             four when sub-batches are solved in pairs
+//   rhs       compact: slot_map [N] (node -> rhs slot), Vc [P + 2048, 32] fp32 (exact v) + R16 [P + 2048, 32] fp16
+//             (scaled), two sets (double-buffered), four when sub-batches are solved in pairs
 //   scores    S_pass [chunk, P] fp32; fact scores are never materialised in the fused modes (72 B per query x tile)
 // Streams: `stream` runs the similarity, the solves and the selection; `stream2` builds the compact right-hand side of
 // sub-batch i + 1 while sub-batch i is being solved.  On one GPU a sub-batch's solve is replayed as a CUDA graph.
@@ -122,6 +122,29 @@ constexpr int kKnnComplete = 1, kKnnRefill = 2;
 }  // namespace hrag
 
 namespace hrag {
+// One fp16 state layout of the mixed solver (solve.cu): the first iterates x0[p] of the solves of parity p (a solve's
+// dense first iterate, written while the solve before it runs), and the work buffers A, C (Chebyshev iterates) and R
+// (residual).  Rows are ld halves apart: 32 for one sub-batch, 64 for two sub-batches interleaved row by row.
+struct StateLayout {
+    void* x0[2] = {nullptr, nullptr};
+    void *A = nullptr, *C = nullptr, *R = nullptr;
+    int ld = 32;
+    size_t bytes = 0;    // of one buffer
+    // sub-batch k's part of one of these buffers (k = 1: the second 32 halves of every row of a pair); null stays null
+    void* part(const void* buf, int k) const {
+        return buf ? static_cast<char*>(const_cast<void*>(buf)) + 64 * k : nullptr;
+    }
+};
+// One compact right-hand-side set of stage B's mixed solves: slot_map [N] (node -> slot, -1 = none), slot_vid [slots]
+// (slot -> node), exact v Vc [slots, 32] fp32 and R16 = fp16(scale * Vc), with slots = P + 2048; its 32 column scales
+// (float) and column sums of v (double).  hrag_ppr's dense solves use set 0's scale and vsum only.
+struct RhsSet { Buf slot_map, slot_vid, Vc, R16, scale, vsum; };
+// Column sums of one sub-batch's mixed solve: of the first solve's iterate, of the correction and of |residual|.
+// Contiguous, so the sharded solve all-reduces the three at once.
+struct MixedSums { double x0[32], d[32], r[32]; };
+// What the mixed solves of a call report, read and cleared by resolve_spans: the running maximum of the measured
+// relative L1 residual of their fp16 first solves, and whether an fp16 iterate left fp16's range.
+struct MixedRho { float rho_max; int overflow; };
 // The inputs of one sub-batch's mixed solve: its right-hand side (compact through slot_map, or dense), exact v, the
 // dense first iterate, column scales and sums of v.  In a pair, x0_dense is the [N, 2, 32] buffer of both.
 struct MixedRhs {
@@ -174,31 +197,22 @@ struct hrag_handle {
     bool rho_dirty = false;           // a mixed solve ran in this call: rho must be read / cleared in resolve_spans
     double last_bound = 0.0;          // a-posteriori bound on the relative L1 error of the last mixed / fp64 call
 
-    // fp32 solver state [N, B]; column-sum partials and sums, shared with the mixed solver
+    // fp32 solver state [N, B], its column-sum partials and sums (V also holds hrag_ppr's exact v for the mixed solver)
     hrag::Buf V, XA, XC, partials, sums;
     // fp64 solver (hrag_ppr_f64, hrag_stage_b_f64): iterate X64 and reset V64 [N, B] fp64, host-layout staging io64
     // [B, max(N, pad4(P))] fp64 (reset in; probabilities, or stage B's passage scores, out), column-sum partials
     // part64, sums64 = [vsum | rsum | xsum] x 16
     hrag::Buf X64, V64, io64, part64, sums64;
-    // mixed solver: one allocation [H0 | H1 | H2 | H3 | H0b | flags] so a single IPC handle exposes every buffer a
-    // peer sweep may have to write into (K5, fused exchange for node-range sharding); H / H0b point into it
-    hrag::Buf slab;
-    size_t slab_hb = 0;                       // bytes of one fp16 state buffer inside the slab
-    void* H[4] = {nullptr, nullptr, nullptr, nullptr};
-    void* H0b = nullptr;
-    hrag::Buf mixed_aux, rho, p2p_err, done_ctr;
-    // paired solves (single GPU, stage B): HP[i] / HP0b are H[i] / H0b for two sub-batches at once, [N, 2, 32]; the
-    // second sub-batch's column-sum partials go to partials_b
-    hrag::Buf slab_pair, partials_b;
-    void* HP[4] = {nullptr, nullptr, nullptr, nullptr};
-    void* HP0b = nullptr;
-    // double-buffered per-sub-batch inputs (set s: x0 = H[0] / H0b, scales mixed_aux / mixed_aux1, compact rhs
-    // Vc[s] / R16[s] addressed through slot_map[s]): stream2 prepares sub-batch i+1 while `stream` sweeps sub-batch i.
-    // A pair of sub-batches uses sets s and s + 2 (x0 = HP[0] / HP0b, the second one 64 B in); mixed_aux1 holds the
-    // scales of sets 1..3.
-    hrag::Buf mixed_aux1, prep_scratch;
-    hrag::Buf slot_map[4], slot_vid[4], Vc[4], R16[4];
-    bool slot_maps_valid = false;
+    // mixed solver, laid out by solve.cu: the single state layout lives in `slab` ([x0[0] | A | C | R | x0[1] | epoch
+    // flags], so a single IPC handle exposes every buffer a peer sweep may have to write into: K5, fused exchange for
+    // node-range sharding), the pair layout of paired solves (single GPU, stage B) in slab_pair
+    hrag::Buf slab, slab_pair;
+    hrag::StateLayout single, pair;
+    hrag::Buf mixed_part[2], mixed_sums;      // sub-batch k's column-sum partials; MixedSums [2]
+    hrag::Buf rho, p2p_err, done_ctr;         // rho: MixedRho
+    // stage B's compact right-hand sides: stream2 prepares solve i + 1's while `stream` sweeps solve i's
+    hrag::RhsSet rhs[4];
+    hrag::Buf prep_scratch;
     int slot_maps_built = 0;                  // sets 0 .. slot_maps_built - 1 hold valid slot maps
     // scratch and I/O staging
     hrag::Buf S_fact, S_pass, mm_fact, mm_pass, mode, seed_vid, seed_w, q_hi, q_lo, part_mm, part_keys;
@@ -271,9 +285,6 @@ inline int d2h(hrag_t* h, void* dst, const void* src, size_t bytes) {
 
 constexpr int kSeedSlots = kSeedSlotsPerQuery;   // 2 phrases per kept fact, <= 32 kept facts
 constexpr float kMixedT = 64.f;    // residual scale: r ~ 5e-4 x, keeps it in fp16's normal range
-// sums layout (doubles): [0, 32) column sums of x0, [32, 64) of d, [64, 96) of |r|, [96, 224) of v (buffer sets 0..3),
-// [224, 320) the x0 / d / |r| sums of the second sub-batch of a pair
-constexpr int kSumX0 = 0, kSumD = 32, kSumR = 64, kSumV = 96, kSumPair = 224;
 constexpr double kDefaultTol = 1e-6;     // relative L1 accuracy of the PPR vector when the caller passes tol <= 0
 struct SweepPlan {
     bool mixed = false;
@@ -287,14 +298,18 @@ SweepPlan plan_sweeps(const hrag_t* h, float alpha, int iters_arg, float tol_arg
 int round_batch(int b);
 int ensure_state(hrag_t* h, int B);
 int ensure_state_mixed(hrag_t* h);
-int ensure_state_pair(hrag_t* h);        // HP / HP0b, partials_b (single GPU)
-int ensure_compact_rhs(hrag_t* h, int n_sets);
-float* set_scale(hrag_t* h, int set);    // column scales of compact-rhs set 0..3
+// The epoch flag words of the fused exchange inside a state slab (this rank's or a peer's), one per rank
+unsigned long long* epoch_flags(const hrag_t* h, void* slab);
+// Stage B's mixed solves of Bq queries (kept facts k_facts): ensure_stage_b_mixed allocates their state before the
+// seeds; stage_b_mixed (k_facts > 0) runs them after the seeds and gathers the PPR scores into S in place.
+int ensure_stage_b_mixed(hrag_t* h, int Bq, int k_facts);
+int stage_b_mixed(hrag_t* h, const SweepPlan& plan, int Bq, float* S, int64_t ldS, const float2* mm_pass, float pnw,
+                  float damping);
+// A new graph, new tables or an index update: the slot maps and the captured solves are stale.  drop_captured_solves
+// synchronises `stream` and destroys the captured solves only.
+int invalidate_solves(hrag_t* h);
+int drop_captured_solves(hrag_t* h);
 int resolve_spans(hrag_t* h);   // end of a call: checks the mixed solves, accumulates the stage times
-// The mixed solve of n = 1 sub-batch, or of n = 2 in one paired walk per sweep (single GPU; in[0].x0_dense is then the
-// pair's [N, 2, 32] buffer).  X0[k] / D[k] = sub-batch k's iterate and correction (rows 32 halves apart, 64 in a pair),
-// their column sums at h->sums + kSumX0 / kSumD (+ kSumPair for k = 1).
-int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, int n, const MixedRhs* in, void** X0, void** D);
 int dev_ppr(hrag_t* h, int B, int iters, float alpha, float** result);
 
 // Float64 PPR by iterative refinement (solve.cu), shared by hrag_ppr_f64 and hrag_stage_b_f64.
@@ -342,8 +357,7 @@ int gather_rows(hrag_t* h, const void* base, size_t row_bytes, const int* row_sr
 int exchange_rows(hrag_t* h, float* y, int B);
 int p2p_wait(hrag_t* h);
 int p2p_signal(hrag_t* h);
-int mixed_sweep_x(hrag_t* h, int mode, const void* x, const int* slot_map, const void* rhs, const float* v32,
-                  const float* scale, const void* prev, void* y, float alpha, float w, float t, float* part,
-                  int* n_part);
+int mixed_sweep_x(hrag_t* h, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_part,
+                  int* overflow);
 
 }  // namespace hrag

@@ -228,9 +228,7 @@ int check_updatable(hrag_t* h, const std::string& who) {
 
 // After a failure past validation: no graph, no tables, no embeddings rather than a half-updated index.
 void drop_index(hrag_t* h) {
-    cudaStreamSynchronize(h->stream);
-    for (auto& c : h->solve_graphs) cudaGraphExecDestroy(c.exec);
-    h->solve_graphs.clear();
+    invalidate_solves(h);    // synchronises `stream` first: nothing still reads what is freed below
     h->graph = GraphMem{};
     h->g = PprGraph();
     h->tables = TableMem{};
@@ -239,17 +237,13 @@ void drop_index(hrag_t* h) {
     h->emb[1] = EmbMem{};
     h->dim = 0;
     h->n_facts_global = h->fact_row_lo = 0;
-    h->slot_maps_valid = false;
 }
 
 // What every update ends with: the captured mixed solves were captured for the old N and P, so they go, whether or
 // not an allocation they point into was freed; the slot maps are rebuilt from the new passage_vid.
 int finish_update(hrag_t* h) {
-    HRAG_CUDA(cudaStreamSynchronize(h->stream));
-    for (auto& c : h->solve_graphs) cudaGraphExecDestroy(c.exec);
-    h->solve_graphs.clear();
+    HRAG_TRY(invalidate_solves(h));
     g_buf_generation += 1;
-    h->slot_maps_valid = false;
     h->n_facts_global = h->emb[0].rows;
     h->fact_row_lo = 0;
     return 0;

@@ -167,9 +167,9 @@ int hrag_load_tables(hrag_t* h, int64_t n_passages, const int32_t* passage_vid, 
     for (int64_t f = 0; f < n_facts; ++f)
         HRAG_CHECK(fact_subj_vid[f] < N && fact_obj_vid[f] < N, "hrag_load_tables: fact vertex id out of range");
     // every input is valid: the old tables go first; a failed upload leaves none (passage_vid, uploaded last, is null)
+    HRAG_TRY(invalidate_solves(h));
     h->tables = TableMem{};
     h->t = SeedTables();
-    h->slot_maps_valid = false;
     HRAG_TRY(h->tables.fact_subj_vid.upload(fact_subj_vid, (size_t)n_facts, &h->t.fact_subj_vid));
     HRAG_TRY(h->tables.fact_obj_vid.upload(fact_obj_vid, (size_t)n_facts, &h->t.fact_obj_vid));
     HRAG_TRY(h->tables.ent_chunk_count.upload(ent_chunk_count, (size_t)N, &h->t.ent_chunk_count));

@@ -69,15 +69,6 @@ struct SweepSync {
 // rhs_h / v32 are [n_slots, 32] arrays addressed through slot_map[node] (-1 = zero row); slot_map == null
 // means dense [N, 32].  partials as in ppr_sweep ([rows, 32] floats).  *overflow (if not null) is set to 1 when a
 // value to be stored is >= 65520 in magnitude (fp16 would round it to inf; it is clamped to 65504 instead).
-int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map, const void* rhs_h,
-                const float* v32, const float* col_scale, const void* prevh, void* yh, float alpha, float w,
-                float t, float* partials, int* n_partials, int* overflow, const PeerOut& peers, const SweepSync& sync,
-                cudaStream_t stream);
-int mixed_partial_rows(const PprGraph& g);
-// The same sweep on two states at once (single GPU): one walk of each row's non-zeros feeds both, and each state gets
-// exactly the bytes, column sums and partials mixed_sweep would give it.  The two states are interleaved row by row in
-// [N, 2, 32] buffers: io[1]'s xh / prevh / yh (and a dense rhs_h) point 64 B after io[0]'s; a compact rhs_h, v32,
-// col_scale, slot_map and partials are each state's own.
 struct MixedSweepIO {
     const void* xh = nullptr;
     const int* slot_map = nullptr;
@@ -88,6 +79,13 @@ struct MixedSweepIO {
     void* yh = nullptr;
     float* partials = nullptr;
 };
+int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_partials,
+                int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t stream);
+int mixed_partial_rows(const PprGraph& g);
+// The same sweep on two states at once (single GPU): one walk of each row's non-zeros feeds both, and each state gets
+// exactly the bytes, column sums and partials mixed_sweep would give it.  The two states are interleaved row by row in
+// [N, 2, 32] buffers: io[1]'s xh / prevh / yh (and a dense rhs_h) point 64 B after io[0]'s; a compact rhs_h, v32,
+// col_scale, slot_map and partials are each state's own.
 int mixed_sweep2(const PprGraph& g, int mode, const MixedSweepIO (&io)[2], float alpha, float w, float t,
                  int* n_partials, int* overflow, cudaStream_t stream);
 // vsum[32] <- column sums of V32 [n_rows, 32] (>= 0; `partials` = scratch of >= 1024*32 floats);

@@ -657,27 +657,32 @@ int epoch_signal(const SweepSync& sync, cudaStream_t st) {
     return 0;
 }
 
-// One fp16 sweep (mode 0) or the residual sweep (mode 1) over the owned rows.
-int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map, const void* rhs_h, const float* v32,
-                const float* col_scale, const void* prevh, void* yh, float alpha, float w, float t, float* partials,
-                int* n_partials, int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t st) {
-    HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep: graph not loaded");
-    HRAG_CHECK(kB <= g.max_batch, "mixed_sweep: segment partials too small for 32 columns");
-    const SweepGrid grid(g, kGPB);
+// The kernels' arguments for one state's sweep
+static SweepArgs sweep_args(const PprGraph& g, const MixedSweepIO& io, float alpha, float w, float t, int* overflow) {
     SweepArgs a;
     a.n_rows = g.n_rows; a.row_base = g.row_lo; a.long_thresh = g.long_thresh;
     a.row_order = g.row_order;
     a.row_ptr = g.row_ptr; a.cv = g.cv;
-    a.xh = reinterpret_cast<const uint4*>(xh);
-    a.slot_map = slot_map;
-    a.rhs_h = reinterpret_cast<const uint4*>(rhs_h);
-    a.v32 = reinterpret_cast<const float4*>(v32);
-    a.col_scale = col_scale;
-    a.prevh = reinterpret_cast<const uint4*>(prevh);
-    a.yh = reinterpret_cast<uint4*>(yh);
+    a.xh = reinterpret_cast<const uint4*>(io.xh);
+    a.slot_map = io.slot_map;
+    a.rhs_h = reinterpret_cast<const uint4*>(io.rhs_h);
+    a.v32 = reinterpret_cast<const float4*>(io.v32);
+    a.col_scale = io.col_scale;
+    a.prevh = reinterpret_cast<const uint4*>(io.prevh);
+    a.yh = reinterpret_cast<uint4*>(io.yh);
     a.alpha = alpha; a.w = w; a.t = t;
-    a.partials = partials;
+    a.partials = io.partials;
     a.overflow = overflow;
+    return a;
+}
+
+// One fp16 sweep (mode 0) or the residual sweep (mode 1) over the owned rows.
+int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_partials,
+                int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t st) {
+    HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep: graph not loaded");
+    HRAG_CHECK(kB <= g.max_batch, "mixed_sweep: segment partials too small for 32 columns");
+    const SweepGrid grid(g, kGPB);
+    const SweepArgs a = sweep_args(g, io, alpha, w, t, overflow);
     SweepSync sy = sync;
     // sharded (fused exchange): a persistent grid of 6 CTAs per SM, so each CTA pays one system-scope fence per sweep
     // and the epoch is published by the last CTA of the sweep itself, with no extra launch (see k_sweep_h_push).  The
@@ -692,7 +697,7 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
         count_launch();
     }
     SweepArgs al = a;
-    al.partials = partials ? partials + (size_t)grid.nb_rows * kB : nullptr;
+    al.partials = a.partials ? a.partials + (size_t)grid.nb_rows * kB : nullptr;
     with_bools([&](auto cheb, auto resid, auto fin) {
         if constexpr (!(cheb && resid)) {                // the residual (mode 1) has no Chebyshev form
             constexpr int M = resid ? 1 : 0;
@@ -707,7 +712,7 @@ int mixed_sweep(const PprGraph& g, int mode, const void* xh, const int* slot_map
                 count_launch();
             }
         }
-    }, mode == 0 && prevh != nullptr, mode == 1, partials != nullptr);
+    }, mode == 0 && io.prevh != nullptr, mode == 1, io.partials != nullptr);
     if (grid.nb_rows + grid.nb_long == 0 && sharded) HRAG_TRY(epoch_signal(sy, st));
     if (n_partials) *n_partials = grid.nb_rows + grid.nb_long;
     HRAG_CUDA(cudaGetLastError());
@@ -720,23 +725,7 @@ int mixed_sweep2(const PprGraph& g, int mode, const MixedSweepIO (&io)[2], float
     HRAG_CHECK(kB <= g.max_batch, "mixed_sweep2: segment partials too small for 32 columns");
     HRAG_CHECK((io[0].partials == nullptr) == (io[1].partials == nullptr), "mixed_sweep2: partials for both or neither");
     const SweepGrid grid(g, kGPB);
-    SweepArgs a[2];
-    for (int k = 0; k < 2; ++k) {
-        SweepArgs& x = a[k];
-        x.n_rows = g.n_rows; x.row_base = g.row_lo; x.long_thresh = g.long_thresh;
-        x.row_order = g.row_order;
-        x.row_ptr = g.row_ptr; x.cv = g.cv;
-        x.xh = reinterpret_cast<const uint4*>(io[k].xh);
-        x.slot_map = io[k].slot_map;
-        x.rhs_h = reinterpret_cast<const uint4*>(io[k].rhs_h);
-        x.v32 = reinterpret_cast<const float4*>(io[k].v32);
-        x.col_scale = io[k].col_scale;
-        x.prevh = reinterpret_cast<const uint4*>(io[k].prevh);
-        x.yh = reinterpret_cast<uint4*>(io[k].yh);
-        x.alpha = alpha; x.w = w; x.t = t;
-        x.partials = io[k].partials;
-        x.overflow = overflow;
-    }
+    const SweepArgs a[2] = {sweep_args(g, io[0], alpha, w, t, overflow), sweep_args(g, io[1], alpha, w, t, overflow)};
     F8* segp = reinterpret_cast<F8*>(g.seg_partial);
     with_bools([&](auto cheb, auto resid, auto fin) {
         if constexpr (!(cheb && resid)) {

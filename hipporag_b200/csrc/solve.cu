@@ -2,7 +2,6 @@
 // CUDA-graph cache of its solves) and float64 refinement; hrag_ppr, hrag_ppr_f64 and hrag_plan_sweeps.
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 
 #include "handle.h"
 
@@ -30,62 +29,80 @@ int ensure_state(hrag_t* h, int B) {
     return 0;
 }
 
+// [x0[0] | A | C | R | x0[1]] at base, rows `ld` halves apart
+static StateLayout carve_layout(void* base, size_t rows, int ld) {
+    StateLayout L;
+    L.ld = ld;
+    L.bytes = rows * ld * 2;
+    void** bufs[5] = {&L.x0[0], &L.A, &L.C, &L.R, &L.x0[1]};
+    for (int i = 0; i < 5; ++i) *bufs[i] = static_cast<char*>(base) + (size_t)i * L.bytes;
+    return L;
+}
+
+unsigned long long* epoch_flags(const hrag_t* h, void* slab) {
+    return reinterpret_cast<unsigned long long*>(static_cast<char*>(slab) + 5 * h->single.bytes);
+}
+
+static MixedSums* sub_batch_sums(hrag_t* h, int k) { return h->mixed_sums.as<MixedSums>() + k; }
+
 int ensure_state_mixed(hrag_t* h) {
     const size_t rows = state_rows(h);
-    const size_t hb = rows * 32 * 2;
-    if (h->slab.p == nullptr || h->slab_hb != hb) {
+    if (h->slab.p == nullptr || h->single.bytes != rows * 32 * 2) {
         HRAG_CHECK(!h->p2p, "internal: the state slab cannot change after hrag_p2p_import");
         h->slab.reset();
-        HRAG_TRY(h->slab.ensure(5 * hb + 256));
-        HRAG_CUDA(cudaMemset(static_cast<char*>(h->slab.p) + 5 * hb, 0, 256));      // epoch flags
-        h->slab_hb = hb;
-        for (int i = 0; i < 4; ++i) h->H[i] = static_cast<char*>(h->slab.p) + (size_t)i * hb;
-        h->H0b = static_cast<char*>(h->slab.p) + 4 * hb;
+        HRAG_TRY(h->slab.ensure(5 * rows * 32 * 2 + 256));
+        h->single = carve_layout(h->slab.p, rows, 32);
+        HRAG_CUDA(cudaMemset(epoch_flags(h, h->slab.p), 0, 256));
         if (!h->p2p_err.p) HRAG_TRY(h->p2p_err.zeros(sizeof(int)));
         if (!h->done_ctr.p) HRAG_TRY(h->done_ctr.zeros(sizeof(unsigned int)));
     }
-    HRAG_TRY(h->partials.ensure((size_t)std::max(mixed_partial_rows(h->g), 1024) * 32 * sizeof(float)));
-    HRAG_TRY(h->sums.ensure(320 * sizeof(double)));      // sums of x0, of d, of |r| (x2), and of v (four sets)
-    HRAG_TRY(h->mixed_aux.ensure(32 * sizeof(float)));   // column scales, set 0
-    // [0] running max of the measured residual (float), [1] fp16 overflow flag (int)
-    if (h->rho.p == nullptr) HRAG_TRY(h->rho.zeros(2 * sizeof(float)));
+    HRAG_TRY(h->mixed_part[0].ensure((size_t)std::max(mixed_partial_rows(h->g), 1024) * 32 * sizeof(float)));
+    HRAG_TRY(h->mixed_sums.ensure(2 * sizeof(MixedSums)));
+    HRAG_TRY(h->rhs[0].scale.ensure(32 * sizeof(float)));    // hrag_ppr's dense solves use set 0's scale and vsum
+    HRAG_TRY(h->rhs[0].vsum.ensure(32 * sizeof(double)));
+    if (h->rho.p == nullptr) HRAG_TRY(h->rho.zeros(sizeof(MixedRho)));
     return 0;
 }
 
-int ensure_state_pair(hrag_t* h) {
+static int ensure_state_pair(hrag_t* h) {
     HRAG_CHECK(h->world == 1, "internal: paired solves run on a single GPU");
-    const size_t hb2 = (size_t)h->g.n_global * 64 * 2;
-    HRAG_TRY(h->slab_pair.ensure(5 * hb2));
-    for (int i = 0; i < 4; ++i) h->HP[i] = static_cast<char*>(h->slab_pair.p) + (size_t)i * hb2;
-    h->HP0b = static_cast<char*>(h->slab_pair.p) + 4 * hb2;
-    HRAG_TRY(h->partials_b.ensure(h->partials.cap));
+    const size_t rows = (size_t)h->g.n_global;
+    HRAG_TRY(h->slab_pair.ensure(5 * rows * 64 * 2));
+    h->pair = carve_layout(h->slab_pair.p, rows, 64);
+    HRAG_TRY(h->mixed_part[1].ensure(h->mixed_part[0].cap));
     return 0;
 }
 
-// Compact right-hand-side buffers of stage B (two sets, four for paired solves; see the handle) + the node -> slot
-// tables.
-int ensure_compact_rhs(hrag_t* h, int n_sets) {
+// Compact right-hand-side sets 0 .. n_sets - 1 of stage B, their slot maps built.
+static int ensure_compact_rhs(hrag_t* h, int n_sets) {
     const size_t n_slots = (size_t)h->t.n_passages + 32 * kSeedSlots;
     for (int s = 0; s < n_sets; ++s) {
-        HRAG_TRY(h->slot_map[s].ensure((size_t)h->g.n_global * sizeof(int)));
-        HRAG_TRY(h->slot_vid[s].ensure(n_slots * sizeof(int)));
-        HRAG_TRY(h->Vc[s].ensure(n_slots * 32 * sizeof(float)));
-        HRAG_TRY(h->R16[s].ensure(n_slots * 32 * 2));
+        RhsSet& r = h->rhs[s];
+        HRAG_TRY(r.slot_map.ensure((size_t)h->g.n_global * sizeof(int)));
+        HRAG_TRY(r.slot_vid.ensure(n_slots * sizeof(int)));
+        HRAG_TRY(r.Vc.ensure(n_slots * 32 * sizeof(float)));
+        HRAG_TRY(r.R16.ensure(n_slots * 32 * 2));
+        HRAG_TRY(r.scale.ensure(32 * sizeof(float)));
+        HRAG_TRY(r.vsum.ensure(32 * sizeof(double)));
     }
-    HRAG_TRY(h->mixed_aux1.ensure(3 * 32 * sizeof(float)));
     HRAG_TRY(h->prep_scratch.ensure((size_t)std::max(compact_rhs_partial_rows(h->t.n_passages), 1024) * 32 * sizeof(float)));
-    if (!h->slot_maps_valid) {                       // a graph or table load invalidated every set
-        h->slot_maps_built = 0;
-        h->slot_maps_valid = true;
-    }
     for (; h->slot_maps_built < n_sets; ++h->slot_maps_built)
         HRAG_TRY(slot_map_build(h->g.n_global, h->t.n_passages, h->t.passage_vid,
-                                h->slot_map[h->slot_maps_built].as<int>(), h->stream));
+                                h->rhs[h->slot_maps_built].slot_map.as<int>(), h->stream));
     return 0;
 }
 
-float* set_scale(hrag_t* h, int set) {
-    return set == 0 ? h->mixed_aux.as<float>() : h->mixed_aux1.as<float>() + 32 * (set - 1);
+int drop_captured_solves(hrag_t* h) {
+    const cudaError_t e = cudaStreamSynchronize(h->stream);   // none of them may still be executing
+    for (auto& c : h->solve_graphs) cudaGraphExecDestroy(c.exec);
+    h->solve_graphs.clear();
+    HRAG_CUDA(e);
+    return 0;
+}
+
+int invalidate_solves(hrag_t* h) {
+    h->slot_maps_built = 0;
+    return drop_captured_solves(h);
 }
 
 int resolve_spans(hrag_t* h) {
@@ -98,28 +115,26 @@ int resolve_spans(hrag_t* h) {
                              "the results of this call are invalid");
     }
     if ((h->rho_dirty || h->check_tol > 0.0) && h->rho.p) {
-        // every mixed solve of this call (a fresh capture or a replayed graph) raised rho[0] = the running maximum of
-        // the measured relative L1 residual of its fp16 first solve, and rho[1] if an fp16 iterate left fp16's range.
-        // Both are cleared here, checked call or not, so the next call is judged by its own solves only.
-        float rho[2] = {0.f, 0.f};
-        HRAG_CUDA(cudaMemcpy(rho, h->rho.p, sizeof(rho), cudaMemcpyDeviceToHost));
+        // every mixed solve of this call (a fresh capture or a replayed graph) raised rho_max, and overflow if an fp16
+        // iterate left fp16's range.  Both are cleared here, checked call or not, so the next call is judged by its own
+        // solves only.
+        MixedRho rho;
+        HRAG_CUDA(cudaMemcpy(&rho, h->rho.p, sizeof(rho), cudaMemcpyDeviceToHost));
         HRAG_CUDA(cudaMemset(h->rho.p, 0, sizeof(rho)));
-        int overflow = 0;
-        memcpy(&overflow, &rho[1], sizeof(int));
         const double tol = h->check_tol, kappa = h->check_kappa;
         h->check_tol = h->check_kappa = 0.0;
         h->rho_dirty = false;
-        if (overflow) {
+        if (rho.overflow) {
             set_error("PPR (mixed solver): an fp16 iterate reached 65520 in magnitude and would have been clamped, so "
                       "the result is invalid -- pass more sweeps (iters) or use HRAG_PPR_FP32");
             return 5;
         }
         if (tol > 0.0) {
             // a-posteriori check of the mixed solver: the refinement round contracts rho by kappa (plan_sweeps)
-            h->last_rho = rho[0];
-            h->last_bound = (float)(rho[0] * kappa);
-            if (!(rho[0] * kappa <= 10.0 * tol)) {
-                set_error("PPR (mixed solver): measured relative residual " + std::to_string(rho[0]) +
+            h->last_rho = rho.rho_max;
+            h->last_bound = (float)(rho.rho_max * kappa);
+            if (!(rho.rho_max * kappa <= 10.0 * tol)) {
+                set_error("PPR (mixed solver): measured relative residual " + std::to_string(rho.rho_max) +
                           " x predicted contraction " + std::to_string(kappa) + " misses tol " + std::to_string(tol) +
                           " -- pass more sweeps (iters) or use HRAG_PPR_FP32");
                 return 4;
@@ -152,62 +167,50 @@ static float cheb_step(int it, float alpha, double* w, T* a, T* c, T* prev, T** 
     return (float)*w;
 }
 
-// Sub-batch k's part of a [N, 2, 32] pair buffer (64 B into each row for k = 1); null stays null.
-static void* pair_half(const void* p, int k) {
-    return p ? static_cast<char*>(const_cast<void*>(p)) + 64 * k : nullptr;
-}
-
-// One sweep of the n sub-batches of a solve (n = 2: one paired walk over the interleaved buffers x, prev, y).
-// slot_map / rhs / v32 / scale are per sub-batch; a dense rhs (slot_map null) is a buffer like x.  final: the column-sum
-// partials of sub-batch k go to h->partials (k = 0) / h->partials_b (k = 1).
-static int mixed_sweep_n(hrag_t* h, int n, int mode, const void* x, const int* const* slot_map,
-                         const void* const* rhs, const float* const* v32, const float* const* scale, const void* prev,
-                         void* y, float alpha, float w, float t, bool final, int* n_part) {
-    if (n == 1)
-        return mixed_sweep_x(h, mode, x, slot_map[0], rhs[0], v32[0], scale[0], prev, y, alpha, w, t,
-                             final ? h->partials.as<float>() : nullptr, n_part);
+// One sweep of the n sub-batches of a solve in layout L (n = 2: one paired walk over the interleaved buffers x, prev,
+// y).  in[k] holds sub-batch k's slot_map, rhs_h, v32 and col_scale; a dense rhs_h (slot_map null) is a buffer of L
+// like x.  final: the column-sum partials of sub-batch k go to h->mixed_part[k].
+static int mixed_sweep_n(hrag_t* h, const StateLayout& L, int n, int mode, const MixedSweepIO* in, const void* x,
+                         const void* prev, void* y, float alpha, float w, float t, bool final, int* n_part) {
     MixedSweepIO io[2];
-    for (int k = 0; k < 2; ++k) {
-        io[k].xh = pair_half(x, k);
-        io[k].slot_map = slot_map[k];
-        io[k].rhs_h = slot_map[k] ? rhs[k] : pair_half(rhs[k], k);
-        io[k].v32 = v32[k];
-        io[k].col_scale = scale[k];
-        io[k].prevh = pair_half(prev, k);
-        io[k].yh = pair_half(y, k);
-        io[k].partials = final ? (k ? h->partials_b : h->partials).as<float>() : nullptr;
+    for (int k = 0; k < n; ++k) {
+        io[k] = in[k];
+        if (!io[k].slot_map) io[k].rhs_h = L.part(io[k].rhs_h, k);
+        io[k].xh = L.part(x, k);
+        io[k].prevh = L.part(prev, k);
+        io[k].yh = L.part(y, k);
+        io[k].partials = final ? h->mixed_part[k].as<float>() : nullptr;
     }
-    int* overflow = h->rho.p ? h->rho.as<int>() + 1 : nullptr;
+    int* overflow = h->rho.p ? &h->rho.as<MixedRho>()->overflow : nullptr;
+    if (n == 1) return mixed_sweep_x(h, mode, io[0], alpha, w, t, n_part, overflow);
     return mixed_sweep2(h->g, mode, io, alpha, w, t, n_part, overflow, h->stream);
 }
 
-// Column sums of sub-batch k of the last final sweep -> h->sums + off (+ kSumPair for k = 1)
-static int mixed_sums(hrag_t* h, int n, int n_part, int off) {
+// Column sums of sub-batch k of the last final sweep -> its MixedSums' `which`
+static int mixed_sums(hrag_t* h, int n, int n_part, double (MixedSums::*which)[32]) {
     for (int k = 0; k < n; ++k)
-        HRAG_TRY(colsum_reduce((k ? h->partials_b : h->partials).as<float>(), n_part, 32,
-                               h->sums.as<double>() + off + (k ? kSumPair : 0), h->stream));
+        HRAG_TRY(colsum_reduce(h->mixed_part[k].as<float>(), n_part, 32, sub_batch_sums(h, k)->*which, h->stream));
     return 0;
 }
 
-// m Chebyshev sweeps of the fp16 solver on (I - aP) x = rhs for n sub-batches, first iterate x_first (= rhs as a dense
-// [N, 32] array, [N, 2, 32] for a pair); rhs[k] is addressed through slot_map[k] (null = dense).  Iterates alternate
-// between bufA and bufC; *result = the last one, its column sums land in h->sums + sums_off.
-static int mixed_cheb(hrag_t* h, int n, const int* const* slot_map, const void* const* rhs, void* x_first, void* bufA,
-                      void* bufC, int m, float alpha, void** result, int sums_off) {
+// m Chebyshev sweeps of the fp16 solver on (I - aP) x = rhs for n sub-batches in layout L, first iterate x_first (= rhs
+// as a dense buffer of L); rhs[k] holds sub-batch k's rhs_h and its slot_map (null = dense).  Iterates alternate
+// between bufA and bufC; *result = the last one, its column sums land in the sub-batches' MixedSums' `which`.
+static int mixed_cheb(hrag_t* h, const StateLayout& L, int n, const MixedSweepIO* rhs, void* x_first, void* bufA,
+                      void* bufC, int m, float alpha, void** result, double (MixedSums::*which)[32]) {
     HRAG_CHECK(m >= 1, "mixed solver: sweep count must be >= 1");
-    const float* none[2] = {nullptr, nullptr};
     double w = 1.0;
     void *x = x_first, *prev = nullptr, *y = nullptr;
     int n_part = 0;
     for (int it = 1; it <= m; ++it) {
         const float wf = cheb_step(it, alpha, &w, bufA, bufC, prev, &y);
-        HRAG_TRY(mixed_sweep_n(h, n, 0, x, slot_map, rhs, none, none, prev, y, alpha, wf, 1.f, it == m, &n_part));
+        HRAG_TRY(mixed_sweep_n(h, L, n, 0, rhs, x, prev, y, alpha, wf, 1.f, it == m, &n_part));
         prev = x;
         x = y;
         h->stats.ppr_sweeps += n;
         h->stats.ppr_columns += 32 * n;
     }
-    HRAG_TRY(mixed_sums(h, n, n_part, sums_off));   // local rows only: see dev_ppr_mixed_body
+    HRAG_TRY(mixed_sums(h, n, n_part, which));   // local rows only: see dev_ppr_mixed_body
     *result = y;
     return 0;
 }
@@ -257,37 +260,38 @@ SweepPlan plan_sweeps(const hrag_t* h, float alpha, int iters_arg, float tol_arg
 
 static int dev_ppr_mixed_body(hrag_t* h, const SweepPlan& plan, float alpha, int n, const MixedRhs* in, void** X0,
                               void** D) {
-    double* sums = h->sums.as<double>();
-    void* const* H = n == 2 ? h->HP : h->H;
-    const int* slot_map[2] = {in[0].slot_map, n == 2 ? in[1].slot_map : nullptr};
-    const void* rhs16[2] = {in[0].rhs16, n == 2 ? in[1].rhs16 : nullptr};
-    const float* vexact[2] = {in[0].Vexact, n == 2 ? in[1].Vexact : nullptr};
-    const float* scale[2] = {in[0].scale, n == 2 ? in[1].scale : nullptr};
+    const StateLayout& L = n == 2 ? h->pair : h->single;
+    // the right-hand sides of the first solve (the compact or dense rhs), the residual (exact v) and the correction (r)
+    MixedSweepIO first[2], resid[2], corr[2];
+    for (int k = 0; k < n; ++k) {
+        first[k].slot_map = resid[k].slot_map = in[k].slot_map;
+        first[k].rhs_h = in[k].rhs16;
+        resid[k].v32 = in[k].Vexact;
+        resid[k].col_scale = in[k].scale;
+        corr[k].rhs_h = L.R;
+    }
     void* x0_dense = in[0].x0_dense;
     void* x0 = nullptr;
     void* d = nullptr;
-    HRAG_TRY(mixed_cheb(h, n, slot_map, rhs16, x0_dense, H[1], H[2], plan.m1, alpha, &x0, kSumX0));
-    void* other = (x0 == H[1]) ? H[2] : H[1];
+    HRAG_TRY(mixed_cheb(h, L, n, first, x0_dense, L.A, L.C, plan.m1, alpha, &x0, &MixedSums::x0));
+    void* other = (x0 == L.A) ? L.C : L.A;
     int n_part = 0;
-    const void* none[2] = {nullptr, nullptr};
-    HRAG_TRY(mixed_sweep_n(h, n, 1, x0, slot_map, none, vexact, scale, nullptr, H[3], alpha, 1.f, kMixedT, true,
-                           &n_part));
+    HRAG_TRY(mixed_sweep_n(h, L, n, 1, resid, x0, nullptr, L.R, alpha, 1.f, kMixedT, true, &n_part));
     h->stats.ppr_sweeps += n;
     h->stats.ppr_columns += 32 * n;
-    HRAG_TRY(mixed_sums(h, n, n_part, kSumR));
-    const int* dense[2] = {nullptr, nullptr};
-    const void* resid[2] = {H[3], H[3]};
-    HRAG_TRY(mixed_cheb(h, n, dense, resid, H[3], x0_dense, other, plan.m2, alpha, &d, kSumD));
+    HRAG_TRY(mixed_sums(h, n, n_part, &MixedSums::r));
+    HRAG_TRY(mixed_cheb(h, L, n, corr, L.R, x0_dense, other, plan.m2, alpha, &d, &MixedSums::d));
     if (h->world > 1) {      // node-range sharding: every rank summed its own rows -- ONE all-reduce for the three sums
+        static_assert(sizeof(MixedSums) == 96 * sizeof(double), "x0, d and r sums are contiguous");
         StageTimer tc(h, ST_COMM);
+        double* sums = sub_batch_sums(h, 0)->x0;
         HRAG_NCCL(g_nccl.AllReduce(sums, sums, 96, ncclDouble, ncclSum, h->comm, h->stream));
     }
     for (int k = 0; k < n; ++k) {
-        const int off = k ? kSumPair : 0;
-        HRAG_TRY(residual_check(sums + off + kSumR, in[k].vsum, in[k].scale, 1.f / kMixedT, h->rho.as<float>(),
-                                h->stream));
-        X0[k] = pair_half(x0, k);
-        D[k] = pair_half(d, k);
+        HRAG_TRY(residual_check(sub_batch_sums(h, k)->r, in[k].vsum, in[k].scale, 1.f / kMixedT,
+                                &h->rho.as<MixedRho>()->rho_max, h->stream));
+        X0[k] = L.part(x0, k);
+        D[k] = L.part(d, k);
     }
     return 0;
 }
@@ -295,8 +299,11 @@ static int dev_ppr_mixed_body(hrag_t* h, const SweepPlan& plan, float alpha, int
 // The solve of one sub-batch is ~20 launches whose arguments depend only on the buffer set and the sweep plan, so on a
 // single GPU it is captured once per (set, plan) into a CUDA graph and replayed (one launch per sub-batch instead of ~20:
 // what bounds small real graphs like MuSiQue-1k, where a sweep is a few microseconds of work).  Multi-GPU runs (epoch
-// values change per sweep) take the plain path.
-int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, int n, const MixedRhs* in, void** X0, void** D) {
+// values change per sweep) take the plain path.  n = 2 solves a pair of sub-batches in one paired walk per sweep
+// (single GPU; in[0].x0_dense is then the pair's [N, 2, 32] buffer).  X0[k] / D[k] = sub-batch k's iterate and
+// correction (rows L.ld halves apart), their column sums in sub_batch_sums(h, k).
+static int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, int n, const MixedRhs* in, void** X0,
+                         void** D) {
     HRAG_CHECK(n == 1 || (n == 2 && h->world == 1), "internal: paired mixed solves run on a single GPU");
     StageTimer tm(h, ST_PPR);
     h->rho_dirty = true;     // set here, not in the body: the body runs on the host only while a graph is captured
@@ -309,11 +316,7 @@ int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, int n, const Mi
         if (c.n == n && c.in[0] == in[0] && (n == 1 || c.in[1] == in[1]) && c.m1 == plan.m1 && c.m2 == plan.m2 &&
             c.alpha == alpha && c.generation == g_buf_generation) sg = &c;
     if (sg == nullptr) {
-        if (h->solve_graphs.size() >= 8) {                       // bounded cache: drop everything stale
-            HRAG_CUDA(cudaStreamSynchronize(h->stream));         // none of them may still be executing
-            for (auto& c : h->solve_graphs) cudaGraphExecDestroy(c.exec);
-            h->solve_graphs.clear();
-        }
+        if (h->solve_graphs.size() >= 8) HRAG_TRY(drop_captured_solves(h));   // bounded cache: drop everything stale
         hrag_handle::SolveGraph c;
         c.n = n;
         for (int k = 0; k < n; ++k) c.in[k] = in[k];
@@ -341,6 +344,74 @@ int dev_ppr_mixed(hrag_t* h, const SweepPlan& plan, float alpha, int n, const Mi
         X0[k] = sg->X0[k];
         D[k] = sg->D[k];
     }
+    return 0;
+}
+
+// single GPU: consecutive sub-batches of stage B are solved in pairs, one walk of the CSR per sweep for both (an odd
+// last one alone); node-range sharding solves them one by one (its exchange is fused into the single-state sweep)
+static bool solve_in_pairs(const hrag_t* h, int Bq) { return h->world == 1 && Bq > 32; }
+
+int ensure_stage_b_mixed(hrag_t* h, int Bq, int k_facts) {
+    const bool pairs = k_facts > 0 && solve_in_pairs(h, Bq);
+    HRAG_TRY(ensure_state_mixed(h));
+    if (pairs) HRAG_TRY(ensure_state_pair(h));
+    return ensure_compact_rhs(h, pairs ? 4 : 2);
+}
+
+// Two streams: stream2 builds solve i+1's compact right-hand sides (passage weights + phrase seeds on P + 2048 slots,
+// column scales, the fp16 copy and the dense first iterate) while `stream` runs the sweeps of solve i.  Solve i (one
+// sub-batch, or a pair) uses the sets of parity i & 1: set p, and p + 2 for the second sub-batch of a pair, and the
+// first iterate x0[p] of its layout.
+int stage_b_mixed(hrag_t* h, const SweepPlan& plan, int Bq, float* S, int64_t ldS, const float2* mm_pass, float pnw,
+                  float damping) {
+    const bool pairs = solve_in_pairs(h, Bq);
+    if (plan.check) h->check_tol = std::max(h->check_tol, plan.tol), h->check_kappa = plan.kappa;
+    HRAG_CUDA(cudaEventRecord(h->ev_inputs, h->stream));            // S, min/max, seed lists are ready
+    HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_inputs, 0));
+    int it = 0;
+    for (int q0 = 0; q0 < Bq; ++it) {
+        const int n = pairs && Bq - q0 > 32 ? 2 : 1;
+        const int par = it & 1;
+        const StateLayout& L = n == 2 ? h->pair : h->single;
+        if (it >= 2) HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_released[par], 0));   // sets are free again
+        MixedRhs in[2];
+        int nb[2] = {0, 0};
+        for (int k = 0; k < n; ++k) {
+            RhsSet& set = h->rhs[par + 2 * k];
+            const int qk = q0 + 32 * k;
+            nb[k] = std::min(32, Bq - qk);
+            in[k].x0_dense = L.x0[par];
+            in[k].slot_map = set.slot_map.as<int>();
+            in[k].Vexact = set.Vc.as<float>();
+            in[k].rhs16 = set.R16.p;
+            in[k].scale = set.scale.as<float>();
+            in[k].vsum = set.vsum.as<double>();
+            HRAG_TRY(compact_prepare_rhs(h->t, nb[k], qk, S, ldS, mm_pass, pnw, kSeedSlots, h->seed_vid.as<int>(),
+                                         h->seed_w.as<double>(), damping, set.slot_map.as<int>(),
+                                         set.slot_vid.as<int>(), set.Vc.as<float>(), set.R16.p, L.part(L.x0[par], k),
+                                         L.ld, (int64_t)h->g.n_global, h->prep_scratch.as<float>(),
+                                         set.vsum.as<double>(), set.scale.as<float>(), h->stream2));
+        }
+        HRAG_CUDA(cudaEventRecord(h->ev_ready[par], h->stream2));
+        HRAG_CUDA(cudaStreamWaitEvent(h->stream, h->ev_ready[par], 0));
+        void *X0[2] = {nullptr, nullptr}, *D[2] = {nullptr, nullptr};
+        HRAG_TRY(dev_ppr_mixed(h, plan, damping, n, in, X0, D));
+        {
+            StageTimer tm(h, ST_TOPK);
+            for (int k = 0; k < n; ++k) {
+                const MixedSums* sums = sub_batch_sums(h, k);
+                HRAG_TRY(gather_passage_scores_mixed(h->t, nb[k], q0 + 32 * k, X0[k], D[k], L.ld, 1.f / kMixedT,
+                                                     sums->x0, sums->d, h->mode.as<int>(), mm_pass, S, ldS,
+                                                     h->stream));
+                HRAG_TRY(compact_release_slots(h->t.n_passages, nb[k], q0 + 32 * k, kSeedSlots, h->seed_vid.as<int>(),
+                                               h->rhs[par + 2 * k].slot_map.as<int>(), h->stream));
+            }
+        }
+        HRAG_TRY(p2p_signal(h));   // peers may overwrite this rank's state buffers from here on
+        HRAG_CUDA(cudaEventRecord(h->ev_released[par], h->stream));
+        q0 += 32 * n;
+    }
+    // (every prepare was consumed by a solve on `stream`, so stream2 is drained in stream order)
     return 0;
 }
 
@@ -509,17 +580,18 @@ int hrag_ppr(hrag_t* h, int32_t B, const float* reset, float damping, int32_t it
         HRAG_TRY(reset_to_state(h->d_reset.as<float>(), nb, N, Bp, h->V.as<float>(), h->stream));
         if (mixed) {
             void *X0 = nullptr, *D = nullptr;
-            double* vsum = h->sums.as<double>() + kSumV;
-            HRAG_TRY(mixed_prepare_rhs(h->V.as<float>(), (int64_t)N, damping, h->partials.as<float>(), vsum,
-                                       h->mixed_aux.as<float>(), h->H[0], h->stream));
             MixedRhs in;
             in.Vexact = h->V.as<float>();
-            in.rhs16 = in.x0_dense = h->H[0];
-            in.scale = h->mixed_aux.as<float>();
-            in.vsum = vsum;
+            in.rhs16 = in.x0_dense = h->single.x0[0];
+            in.scale = h->rhs[0].scale.as<float>();
+            in.vsum = h->rhs[0].vsum.as<double>();
+            HRAG_TRY(mixed_prepare_rhs(in.Vexact, (int64_t)N, damping, h->mixed_part[0].as<float>(),
+                                       h->rhs[0].vsum.as<double>(), h->rhs[0].scale.as<float>(), in.x0_dense,
+                                       h->stream));
             HRAG_TRY(dev_ppr_mixed(h, plan, damping, 1, &in, &X0, &D));
-            HRAG_TRY(state_to_scores_mixed(X0, D, 1.f / kMixedT, nb, N, h->sums.as<double>(),
-                                           h->sums.as<double>() + 32, h->d_scores.as<float>(), h->stream));
+            const MixedSums* sums = sub_batch_sums(h, 0);
+            HRAG_TRY(state_to_scores_mixed(X0, D, 1.f / kMixedT, nb, N, sums->x0, sums->d, h->d_scores.as<float>(),
+                                           h->stream));
             HRAG_TRY(p2p_signal(h));
         } else {
             float* Z = nullptr;
@@ -530,6 +602,81 @@ int hrag_ppr(hrag_t* h, int32_t B, const float* reset, float damping, int32_t it
         HRAG_CUDA(cudaStreamSynchronize(h->stream));
     }
     return resolve_spans(h);
+}
+
+int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float* ms_per_sweep) {
+    HRAG_CHECK(h && ms_per_sweep && sweeps >= 1, "hrag_bench_sweep: bad arguments");
+    HRAG_CHECK(B == 4 || B == 8 || B == 16 || B == 32 || B == 64, "hrag_bench_sweep: B in {4,8,16,32,64}");
+    HRAG_CHECK(h->g.n_global > 0, "hrag_bench_sweep: graph not loaded");
+    HRAG_CUDA(cudaSetDevice(h->device));
+    // fp16-state sweep (Chebyshev form), B = 32: 2 = dense rhs, 3 = compact rhs, 4 = the paired sweep of two
+    // compact-rhs sub-batches ([N, 2, 32] state), timed per paired sweep (64 columns)
+    const bool paired = method == 4;
+    const bool mixed = method == 2 || method == 3 || paired;
+    HRAG_CHECK(!paired || h->world == 1, "hrag_bench_sweep: the paired sweep runs on a single-GPU handle");
+    const bool cheb = method == HRAG_PPR_CHEBYSHEV;
+    MixedSweepIO rhs[2];     // the fp16 sweeps' right-hand sides
+    void *A = nullptr, *C = nullptr;
+    if (mixed) {
+        HRAG_CHECK(B == 32, "hrag_bench_sweep: the mixed solver runs at B = 32");
+        HRAG_TRY(ensure_state_mixed(h));
+        const StateLayout& L = h->single;
+        rhs[0].rhs_h = L.x0[0];
+        if (method >= 3) {
+            HRAG_CHECK(h->t.passage_vid != nullptr, "hrag_bench_sweep: the compact-rhs sweep needs hrag_load_tables");
+            HRAG_TRY(ensure_compact_rhs(h, 2));
+            for (int s = 0; s < 2; ++s) {
+                rhs[s].slot_map = h->rhs[s].slot_map.as<int>();
+                rhs[s].rhs_h = h->rhs[s].R16.p;
+                HRAG_CUDA(cudaMemsetAsync(h->rhs[s].R16.p, 0x2c, h->rhs[s].R16.cap, h->stream));
+            }
+        }
+        const size_t hb = (size_t)h->g.n_global * 32 * 2;
+        for (void* p : {L.x0[0], L.A, L.C}) HRAG_CUDA(cudaMemsetAsync(p, 0x2c, hb, h->stream));   // 0x2c2c = 0.065
+        A = L.A, C = L.C;
+        if (paired) {
+            HRAG_TRY(ensure_state_pair(h));
+            for (void* p : {h->pair.A, h->pair.C}) HRAG_CUDA(cudaMemsetAsync(p, 0x2c, 2 * hb, h->stream));
+            A = h->pair.A, C = h->pair.C;
+        }
+    } else {
+        HRAG_TRY(ensure_state(h, B));
+        const size_t bytes = (size_t)h->g.n_global * B * sizeof(float);
+        HRAG_CUDA(cudaMemsetAsync(h->V.p, 0x3c, bytes, h->stream));     // 0x3c3c3c3c = 0.0115f
+        HRAG_CUDA(cudaMemsetAsync(h->XA.p, 0x3c, bytes, h->stream));
+        HRAG_CUDA(cudaMemsetAsync(h->XC.p, 0x3c, bytes, h->stream));
+        A = h->XA.p, C = h->XC.p;
+    }
+    cudaEvent_t e0, e1;
+    HRAG_CUDA(cudaEventCreate(&e0));
+    HRAG_CUDA(cudaEventCreate(&e1));
+    for (int pass = 0; pass < 2; ++pass) {   // pass 0 = warm-up (3 sweeps), pass 1 = timed
+        const int n = pass == 0 ? 3 : sweeps;
+        if (pass == 1) HRAG_CUDA(cudaEventRecord(e0, h->stream));
+        for (int i = 0; i < n; ++i) {
+            void* x = (i & 1) ? C : A;
+            void* y = (i & 1) ? A : C;
+            float* yf = static_cast<float*>(y);
+            if (mixed) {
+                HRAG_TRY(mixed_sweep_n(h, paired ? h->pair : h->single, paired ? 2 : 1, 0, rhs, x, y, y, 0.5f, 1.07f,
+                                       1.f, false, nullptr));
+            } else {
+                HRAG_TRY(ppr_sweep(h->g, B, static_cast<float*>(x), h->V.as<float>(), cheb ? yf : nullptr, yf, 0.5f,
+                                   cheb ? 1.07f : 1.f, nullptr, nullptr, h->stream));
+                HRAG_TRY(exchange_rows(h, yf, B));
+            }
+        }
+        if (pass == 1) HRAG_CUDA(cudaEventRecord(e1, h->stream));
+    }
+    HRAG_CUDA(cudaStreamSynchronize(h->stream));
+    float ms = 0.f;
+    HRAG_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+    *ms_per_sweep = ms / sweeps;
+    for (auto& s : h->spans) { h->pool.push_back(s.a); h->pool.push_back(s.b); }
+    h->spans.clear();
+    return 0;
 }
 
 int hrag_ppr_f64(hrag_t* h, int32_t B, const double* reset, double damping, double tol, double* out) {
