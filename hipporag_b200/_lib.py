@@ -82,6 +82,7 @@ SIGNATURES = {
     "hrag_reset_stats": (C.c_int, [_p]),
     "hrag_debug_keep_scores": (C.c_int, [_p, C.c_int]),
     "hrag_debug_sim_ctas": (C.c_int, [_p, C.c_int]),
+    "hrag_debug_dense_first_sweep": (C.c_int, [_p, C.c_int]),
     "hrag_debug_copy": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
     "hrag_debug_graph": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
     "hrag_debug_index": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),

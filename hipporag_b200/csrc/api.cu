@@ -675,6 +675,12 @@ int hrag_debug_sim_ctas(hrag_t* h, int n) {
     return 0;
 }
 
+int hrag_debug_dense_first_sweep(hrag_t* h, int on) {
+    HRAG_CHECK(h, "hrag_debug_dense_first_sweep: null handle");
+    h->debug_dense_first_sweep = on != 0;
+    return 0;
+}
+
 int hrag_debug_copy(hrag_t* h, int which, float* host_out, int64_t max_elems, int64_t* n_written) {
     HRAG_CHECK(h && host_out && n_written, "hrag_debug_copy: null argument");
     HRAG_CUDA(cudaSetDevice(h->device));

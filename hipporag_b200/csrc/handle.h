@@ -123,7 +123,8 @@ constexpr int kKnnComplete = 1, kKnnRefill = 2;
 
 namespace hrag {
 // One fp16 state layout of the mixed solver (solve.cu): the first iterates x0[p] of the solves of parity p (a solve's
-// dense first iterate, written while the solve before it runs), and the work buffers A, C (Chebyshev iterates) and R
+// dense first iterate, written while the solve before it runs, when it is built; either way the correction's first
+// work buffer), and the work buffers A, C (Chebyshev iterates) and R
 // (residual).  Rows are ld halves apart: 32 for one sub-batch, 64 for two sub-batches interleaved row by row.
 struct StateLayout {
     void* x0[2] = {nullptr, nullptr};
@@ -147,6 +148,7 @@ struct MixedSums { double x0[32], d[32], r[32]; };
 struct MixedRho { float rho_max; int overflow; };
 // The inputs of one sub-batch's mixed solve: its right-hand side (compact through slot_map, or dense), exact v, the
 // dense first iterate, column scales and sums of v.  In a pair, x0_dense is the [N, 2, 32] buffer of both.
+// x0_compact: the first iterate is not built in x0_dense; the first solve reads it through slot_map (solve.cu).
 struct MixedRhs {
     const int* slot_map = nullptr;
     const float* Vexact = nullptr;
@@ -154,9 +156,10 @@ struct MixedRhs {
     void* x0_dense = nullptr;
     const float* scale = nullptr;
     const double* vsum = nullptr;
+    bool x0_compact = false;
     bool operator==(const MixedRhs& o) const {
         return slot_map == o.slot_map && Vexact == o.Vexact && rhs16 == o.rhs16 && x0_dense == o.x0_dense &&
-               scale == o.scale && vsum == o.vsum;
+               scale == o.scale && vsum == o.vsum && x0_compact == o.x0_compact;
     }
 };
 }  // namespace hrag
@@ -189,6 +192,7 @@ struct hrag_handle {
     int sim_mode = HRAG_SIM_BF16X3;
     bool keep_fact_scores = false;   // debugging: materialise S_fact even in tensor-core modes
     int debug_sim_ctas = 0;          // hrag_debug_sim_ctas: > 0 GEMM CTAs, < 0 no chunk overlap, 0 defaults
+    bool debug_dense_first_sweep = false;   // hrag_debug_dense_first_sweep: stage B builds the dense first iterate
     int ppr_precision = HRAG_PPR_MIXED;   // applies to batches of > 16 queries; smaller ones run fp32
     int mixed_m1 = 0, mixed_m2 = 0;   // 0 = derived from damping (8 / 7 at damping 0.5)
     double check_tol = 0.0, check_kappa = 0.0;   // > 0: this call's mixed solves are verified in resolve_spans

@@ -69,6 +69,8 @@ struct SweepSync {
 // rhs_h / v32 are [n_slots, 32] arrays addressed through slot_map[node] (-1 = zero row); slot_map == null
 // means dense [N, 32].  partials as in ppr_sweep ([rows, 32] floats).  *overflow (if not null) is set to 1 when a
 // value to be stored is >= 65520 in magnitude (fp16 would round it to inf; it is clamped to 65504 instead).
+// x0c (single GPU, compact rhs, mode 0): the solve's first iterate is the rhs itself, read through slot_map instead of
+// a dense copy -- 1: as xh (sweep 1, xh unused), 2: as prevh (sweep 2, a Chebyshev sweep; prevh unused).
 struct MixedSweepIO {
     const void* xh = nullptr;
     const int* slot_map = nullptr;
@@ -78,6 +80,7 @@ struct MixedSweepIO {
     const void* prevh = nullptr;
     void* yh = nullptr;
     float* partials = nullptr;
+    int x0c = 0;
 };
 int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_partials,
                 int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t stream);
@@ -99,8 +102,8 @@ int slot_map_build(int N, int P, const int* passage_vid, int* slot_map, cudaStre
 int compact_rhs_partial_rows(int P);
 // Builds, for the nb queries [q0, q0 + nb) of a chunk: Vc [P + 32*slots_per_query, 32] fp32 (passage weights
 // pnw * minmax(S) on the passage slots, phrase weights on freshly assigned seed slots), its column sums / fp16
-// scales, rhs16 = fp16(scale * Vc), and the dense first iterate x0_dense [n_nodes, 32] fp16, rows x0_ld halves apart
-// (32, or 64 for one state of an interleaved pair).
+// scales, rhs16 = fp16(scale * Vc), and (x0_dense not null) the dense first iterate x0_dense [n_nodes, 32] fp16, rows
+// x0_ld halves apart (32, or 64 for one state of an interleaved pair).
 int compact_prepare_rhs(const SeedTables& t, int nb, int q0, const float* S, int64_t ldS, const float2* minmax,
                         float pnw, int slots_per_query, const int* seed_vid, const double* seed_w, float alpha,
                         int* slot_map, int* slot_vid, float* Vc, void* rhs16, void* x0_dense, int x0_ld, int64_t n_nodes,

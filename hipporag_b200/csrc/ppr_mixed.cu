@@ -26,6 +26,12 @@
 // of three passes over [N, 32] fp32.  slot_map == nullptr means "dense": slot = row (hrag_ppr's
 // arbitrary reset vectors, and the residual rhs of the correction solve).
 //
+// First iterate.  The first solve starts from x = rhs, so on a single GPU its first two sweeps read that iterate where
+// it already is, compactly (template argument X0C): sweep 1 gathers row c as rhs[slot_map[c]] and skips the load of a
+// row without a slot (about 3 in 4 of the gathers of a sweep over the whole graph, and those would miss L2), sweep 2's
+// Chebyshev epilogue takes prev = its rhs row.  No dense [N, 32] copy of the rhs is built.  Every skipped gather is a
+// zero operand of the same fma sequence, so the sums are bit for bit those of the dense first iterate.
+//
 // Row walk: 4 gathers in flight per lane, the ragged end of a row is one PREDICATED batch (not a
 // serial tail), and the 64 rows of a CTA are handed to the groups by length (row_order) so the 8
 // rows that share a warp finish together.
@@ -69,8 +75,35 @@ __device__ __forceinline__ void st_y(uint4* p, const uint4& v) { *p = v; }
 
 constexpr int kU = 4;                   // independent gathers in flight per lane
 
-__device__ __forceinline__ void group_row_dot_h(const int2* __restrict__ cv, int s, int e,
-                                                const uint4* __restrict__ xh /* + lane */, float (&acc)[8]) {
+// Where the first iterate x0 = rhs of a solve is read from (template argument X0C of the sweep kernels): kX0Dense, a
+// dense state like every other iterate; kX0AsX, sweep 1 gathers it through the slot map (RhsRows); kX0AsPrev, sweep
+// 2's Chebyshev epilogue takes prev = the rhs row it already reads.
+constexpr int kX0Dense = 0, kX0AsX = 1, kX0AsPrev = 2;
+
+// The compact first iterate as a gathered operand: row c = rhs[slot_map[c]] (rows kLPR uint4 apart, rhs already
+// + lane), zeros when c has no slot -- without a load.
+struct RhsRows {
+    const int* slot_map;
+    const uint4* rhs;
+    __device__ __forceinline__ RhsRows operator+(int lane) const { return {slot_map, rhs + lane}; }
+};
+template <int RS>
+__device__ __forceinline__ uint4 gather_row(const RhsRows& x, int col) {
+    const int slot = __ldg(x.slot_map + col);
+    return slot >= 0 ? __ldg(x.rhs + (size_t)slot * kLPR) : make_uint4(0u, 0u, 0u, 0u);
+}
+// predicated gather of row c of the state (rows RS uint4 apart) or of the compact first iterate
+__device__ __forceinline__ uint4 ld_gather_row(const uint4* x, int rs, int c, bool ok) {
+    return ld_gather(x + (size_t)c * rs, ok);
+}
+__device__ __forceinline__ uint4 ld_gather_row(const RhsRows& x, int, int c, bool ok) {
+    const int slot = ok ? __ldg(x.slot_map + c) : -1;
+    return ld_gather(x.rhs + slot * kLPR, slot >= 0);
+}
+
+template <class Src>
+__device__ __forceinline__ void group_row_dot_h(const int2* __restrict__ cv, int s, int e, const Src xh /* + lane */,
+                                                float (&acc)[8]) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] = 0.f;
     // kU independent 16-byte gathers in flight per lane; the ragged end of the row is a PREDICATED batch, not a
@@ -81,7 +114,7 @@ __device__ __forceinline__ void group_row_dot_h(const int2* __restrict__ cv, int
 #pragma unroll
         for (int j = 0; j < kU; ++j) c[j] = ld_cv(cv + i + j, i + j < e);
 #pragma unroll
-        for (int j = 0; j < kU; ++j) a[j] = ld_gather(xh + (size_t)c[j].x * kLPR, i + j < e);
+        for (int j = 0; j < kU; ++j) a[j] = ld_gather_row(xh, kLPR, c[j].x, i + j < e);
 #pragma unroll
         for (int j = 0; j < kU; ++j) fma8(acc, __int_as_float(c[j].y), a[j]);
     }
@@ -129,8 +162,8 @@ __device__ __forceinline__ void sync_signal(const SweepSync& sy) {
 // rhs / v32 are addressed through slot_map (null = dense).  Returns (in out[]) the value as
 // STORED (after fp16 rounding) so column sums match memory; MODE 1 + FINAL returns |value|.  RS: row stride in uint4 of
 // x0h / prevh / yh and of a dense rhs_h (kLPR; 2 kLPR when two states are interleaved row by row); compact rhs_h and v32
-// are per state.
-template <bool CHEB, int MODE, int RS = kLPR>
+// are per state.  PREV_RHS: prev is the rhs row itself (kX0AsPrev), zeros where the row has no slot.
+template <bool CHEB, int MODE, int RS = kLPR, bool PREV_RHS = false>
 __device__ __forceinline__ void row_epilogue_h(float (&acc)[8], int row, int lane, const int* __restrict__ slot_map,
                                                const uint4* __restrict__ rhs_h, const float4* __restrict__ v32,
                                                const float* __restrict__ col_scale, const uint4* x0h,
@@ -139,8 +172,8 @@ __device__ __forceinline__ void row_epilogue_h(float (&acc)[8], int row, int lan
     const size_t o = (size_t)row * RS + lane;
     const int slot = slot_map ? __ldg(slot_map + row) : row;
     if (MODE == 0) {
+        float r[8];
         if (slot >= 0) {
-            float r[8];
             h8_to_f(ld_stream16(rhs_h + (size_t)slot * (slot_map ? kLPR : RS) + lane), r);
 #pragma unroll
             for (int j = 0; j < 8; ++j) out[j] = fmaf(alpha, acc[j], r[j]);
@@ -150,7 +183,12 @@ __device__ __forceinline__ void row_epilogue_h(float (&acc)[8], int row, int lan
         }
         if (CHEB) {
             float p[8];
-            h8_to_f(ld_prev(prevh + o), p);
+            if (PREV_RHS) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) p[j] = slot >= 0 ? r[j] : 0.f;
+            } else {
+                h8_to_f(ld_prev(prevh + o), p);
+            }
             const float w1 = 1.f - w;
 #pragma unroll
             for (int j = 0; j < 8; ++j) out[j] = fmaf(w, out[j], w1 * p[j]);
@@ -236,7 +274,7 @@ struct SweepArgs {
 
 // Single-GPU sweep: one block of 64 rows per CTA.  (Kept free of the exchange code of k_sweep_h_push below: a block
 // loop with the staging / bulk-copy code behind a uniform branch slows the plain sweep down.)
-template <bool CHEB, int MODE, bool FINAL>
+template <bool CHEB, int MODE, bool FINAL, int X0C = kX0Dense>
 __global__ void __launch_bounds__(kThreads, 6)
 k_sweep_h(const SweepArgs a) {
     const int g = threadIdx.x / kLPR, l = threadIdx.x % kLPR;
@@ -250,9 +288,11 @@ k_sweep_h(const SweepArgs a) {
         if (e - s <= a.long_thresh) {
             float acc[8];
             uint4 packed;
-            group_row_dot_h(a.cv, s, e, a.xh + l, acc);
-            row_epilogue_h<CHEB, MODE>(acc, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh, a.prevh,
-                                       a.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out, packed);
+            if (X0C == kX0AsX) group_row_dot_h(a.cv, s, e, RhsRows{a.slot_map, a.rhs_h + l}, acc);
+            else group_row_dot_h(a.cv, s, e, a.xh + l, acc);
+            row_epilogue_h<CHEB, MODE, kLPR, X0C == kX0AsPrev>(acc, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32,
+                                                               a.col_scale, a.xh, a.prevh, a.yh, a.alpha, a.w, a.t,
+                                                               PeerOut(), a.overflow, out, packed);
         }
     }
     if (FINAL) block_colsum_h(out, a.partials + (size_t)blockIdx.x * kB);
@@ -263,8 +303,8 @@ k_sweep_h(const SweepArgs a) {
 // and the column-independent bytes (cv, row_ptr, row_order) are paid once per 64 columns.  Each state's sums keep
 // k_sweep_h's order: the same fma sequence per lane, the same epilogue and the same column-sum partials.
 constexpr int kRS2 = 2 * kLPR;          // row stride of the interleaved pair in uint4
-__device__ __forceinline__ void group_row_dot_h2(const int2* __restrict__ cv, int s, int e,
-                                                 const uint4* __restrict__ xa, const uint4* __restrict__ xb,
+template <class Src>
+__device__ __forceinline__ void group_row_dot_h2(const int2* __restrict__ cv, int s, int e, const Src xa, const Src xb,
                                                  float (&acc_a)[8], float (&acc_b)[8]) {
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc_a[j] = acc_b[j] = 0.f;
@@ -275,8 +315,8 @@ __device__ __forceinline__ void group_row_dot_h2(const int2* __restrict__ cv, in
         for (int j = 0; j < kU; ++j) c[j] = ld_cv(cv + i + j, i + j < e);
 #pragma unroll
         for (int j = 0; j < kU; ++j) {
-            a[j] = ld_gather(xa + (size_t)c[j].x * kRS2, i + j < e);
-            b[j] = ld_gather(xb + (size_t)c[j].x * kRS2, i + j < e);
+            a[j] = ld_gather_row(xa, kRS2, c[j].x, i + j < e);
+            b[j] = ld_gather_row(xb, kRS2, c[j].x, i + j < e);
         }
 #pragma unroll
         for (int j = 0; j < kU; ++j) {
@@ -287,8 +327,9 @@ __device__ __forceinline__ void group_row_dot_h2(const int2* __restrict__ cv, in
 }
 
 // 64 registers (4 CTAs per SM: 8 gathers in flight per lane, 8 K per SM against k_sweep_h's 6 K); FINAL keeps both
-// states' stored values for the column sums and takes 72 registers (3 CTAs per SM) rather than spill.
-template <bool CHEB, int MODE, bool FINAL>
+// states' stored values for the column sums and takes 72 registers (3 CTAs per SM) rather than spill.  With X0C ==
+// kX0AsX each state gathers its own compact first iterate: the passage slots are shared, the seed slots are not.
+template <bool CHEB, int MODE, bool FINAL, int X0C = kX0Dense>
 __global__ void __launch_bounds__(kThreads, FINAL ? 3 : 4)
 k_sweep_h2(const SweepArgs a, const SweepArgs b) {
     const int g = threadIdx.x / kLPR, l = threadIdx.x % kLPR;
@@ -302,11 +343,17 @@ k_sweep_h2(const SweepArgs a, const SweepArgs b) {
         if (e - s <= a.long_thresh) {
             float acc_a[8], acc_b[8];
             uint4 packed;
-            group_row_dot_h2(a.cv, s, e, a.xh + l, b.xh + l, acc_a, acc_b);
-            row_epilogue_h<CHEB, MODE, kRS2>(acc_a, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh,
-                                             a.prevh, a.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out_a, packed);
-            row_epilogue_h<CHEB, MODE, kRS2>(acc_b, a.row_base + r, l, b.slot_map, b.rhs_h, b.v32, b.col_scale, b.xh,
-                                             b.prevh, b.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out_b, packed);
+            if (X0C == kX0AsX)
+                group_row_dot_h2(a.cv, s, e, RhsRows{a.slot_map, a.rhs_h + l}, RhsRows{b.slot_map, b.rhs_h + l}, acc_a,
+                                 acc_b);
+            else group_row_dot_h2(a.cv, s, e, a.xh + l, b.xh + l, acc_a, acc_b);
+            constexpr bool PR = X0C == kX0AsPrev;
+            row_epilogue_h<CHEB, MODE, kRS2, PR>(acc_a, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale,
+                                                 a.xh, a.prevh, a.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out_a,
+                                                 packed);
+            row_epilogue_h<CHEB, MODE, kRS2, PR>(acc_b, a.row_base + r, l, b.slot_map, b.rhs_h, b.v32, b.col_scale,
+                                                 b.xh, b.prevh, b.yh, a.alpha, a.w, a.t, PeerOut(), a.overflow, out_b,
+                                                 packed);
         }
     }
     if (FINAL) {
@@ -393,15 +440,16 @@ k_sweep_h_push(const SweepArgs a, const PeerOut peers, const SweepSync sy) {
     sync_signal(sy);
 }
 
-template <int RS = kLPR>
+// Src: the state (const uint4*), or RhsRows for the compact first iterate
+template <int RS = kLPR, class Src = const uint4*>
 __global__ void __launch_bounds__(kThreads)
-k_sweep_long_segments_h(int n_seg, const int4* __restrict__ segs, const int2* __restrict__ cv,
-                        const uint4* __restrict__ xh, F8* __restrict__ seg_partial, const SweepSync sy) {
+k_sweep_long_segments_h(int n_seg, const int4* __restrict__ segs, const int2* __restrict__ cv, const Src xh,
+                        F8* __restrict__ seg_partial, const SweepSync sy) {
     sync_wait(sy);
-    segment_partial<LaneF16, kLPR, RS>(n_seg, segs, cv, nullptr, xh, seg_partial);
+    segment_partial<LaneF16, kLPR, RS, Src>(n_seg, segs, cv, nullptr, xh, seg_partial);
 }
 
-template <bool CHEB, int MODE, bool FINAL, int RS = kLPR>
+template <bool CHEB, int MODE, bool FINAL, int RS = kLPR, bool PREV_RHS = false>
 __global__ void __launch_bounds__(kThreads)
 k_sweep_long_finalize_h(int n_long, const int* __restrict__ long_rows, const int* __restrict__ long_seg_ptr,
                         const F8* __restrict__ seg_partial, const SweepArgs a, const PeerOut peers,
@@ -415,8 +463,8 @@ k_sweep_long_finalize_h(int n_long, const int* __restrict__ long_rows, const int
         const int r = __ldg(long_rows + k);
         F8 acc = segment_sum<LaneF16, kLPR>(long_seg_ptr, k, seg_partial + l);
         uint4 packed;
-        row_epilogue_h<CHEB, MODE, RS>(acc.v, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale, a.xh,
-                                       a.prevh, a.yh, a.alpha, a.w, a.t, peers, a.overflow, out, packed);
+        row_epilogue_h<CHEB, MODE, RS, PREV_RHS>(acc.v, a.row_base + r, l, a.slot_map, a.rhs_h, a.v32, a.col_scale,
+                                                 a.xh, a.prevh, a.yh, a.alpha, a.w, a.t, peers, a.overflow, out, packed);
     }
     if (FINAL) block_colsum_h(out, a.partials + (size_t)blockIdx.x * kB);
     sync_signal(sy);
@@ -551,7 +599,7 @@ k_rhs_seeds(int P, int nb, int q0, int slots_per_query, const int* __restrict__ 
     }
 }
 
-// rhs16[slot, :] = fp16(scale * Vc[slot, :]) for every slot, and the same row scattered into the dense
+// rhs16[slot, :] = fp16(scale * Vc[slot, :]) for every slot, and (x0 not null) the same row scattered into the dense
 // first iterate x0 (zeroed by the caller): x0[vertex(slot), :], rows x0_stride uint4 apart
 __global__ void __launch_bounds__(256)
 k_rhs_convert(int P, int n_slots, const int* __restrict__ passage_vid, const int* __restrict__ slot_vid,
@@ -560,13 +608,14 @@ k_rhs_convert(int P, int n_slots, const int* __restrict__ passage_vid, const int
     const int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x;       // one 8-column group
     const int slot = (int)(i >> 2), l = (int)(i & 3);
     if (slot >= n_slots) return;
-    const int vid = slot < P ? __ldg(passage_vid + slot) : __ldg(slot_vid + slot);
     const float4 a = __ldcs(Vc + 2 * i), b = __ldcs(Vc + 2 * i + 1);
     float f[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 #pragma unroll
     for (int j = 0; j < 8; ++j) f[j] *= __ldg(scale + l * 8 + j);
     const uint4 h = f_to_h8(f);
     rhs16[i] = h;
+    if (x0 == nullptr) return;
+    const int vid = slot < P ? __ldg(passage_vid + slot) : __ldg(slot_vid + slot);
     if (vid >= 0) x0[(size_t)vid * x0_stride + l] = h;
 }
 
@@ -681,6 +730,8 @@ int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO& io, float alpha
                 int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t st) {
     HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep: graph not loaded");
     HRAG_CHECK(kB <= g.max_batch, "mixed_sweep: segment partials too small for 32 columns");
+    HRAG_CHECK(io.x0c == kX0Dense || (io.slot_map && sync.flags == nullptr && mode == 0),
+               "mixed_sweep: the compact first iterate needs a compact rhs on a single GPU");
     const SweepGrid grid(g, kGPB);
     const SweepArgs a = sweep_args(g, io, alpha, w, t, overflow);
     SweepSync sy = sync;
@@ -693,26 +744,37 @@ int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO& io, float alpha
     sy.total_ctas = (unsigned)(grid_rows + grid.nb_long);
     F8* segp = reinterpret_cast<F8*>(g.seg_partial);
     if (g.n_long) {     // only waits: the segment kernel writes no exchanged rows
-        k_sweep_long_segments_h<><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, a.xh, segp, sy);
+        if (io.x0c == kX0AsX)
+            k_sweep_long_segments_h<kLPR, RhsRows><<<grid.nb_seg, kThreads, 0, st>>>(
+                g.n_seg, g.segs, g.cv, RhsRows{a.slot_map, a.rhs_h}, segp, sy);
+        else k_sweep_long_segments_h<><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, a.xh, segp, sy);
         count_launch();
     }
     SweepArgs al = a;
     al.partials = a.partials ? a.partials + (size_t)grid.nb_rows * kB : nullptr;
-    with_bools([&](auto cheb, auto resid, auto fin) {
-        if constexpr (!(cheb && resid)) {                // the residual (mode 1) has no Chebyshev form
+    with_bools([&](auto cheb, auto resid, auto fin, auto x0x, auto x0p) {
+        // the residual (mode 1) has no Chebyshev form; sweep 1 (x0 as x) is a plain sweep, sweep 2 (x0 as prev) a
+        // Chebyshev one
+        if constexpr (!(cheb && resid) && !(x0x && (cheb || resid)) && !(x0p && (!cheb || resid))) {
             constexpr int M = resid ? 1 : 0;
+            constexpr int X0C = x0x ? kX0AsX : x0p ? kX0AsPrev : kX0Dense;
             if (grid.nb_rows) {
-                if (sharded) k_sweep_h_push<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a, peers, sy);
-                else k_sweep_h<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a);
+                if constexpr (X0C == kX0Dense) {
+                    if (sharded) k_sweep_h_push<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a, peers, sy);
+                    else k_sweep_h<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a);
+                } else {
+                    k_sweep_h<cheb, M, fin, X0C><<<grid_rows, kThreads, 0, st>>>(a);
+                }
                 count_launch();
             }
             if (grid.nb_long) {
-                k_sweep_long_finalize_h<cheb, M, fin><<<grid.nb_long, kThreads, 0, st>>>(
+                k_sweep_long_finalize_h<cheb, M, fin, kLPR, X0C == kX0AsPrev><<<grid.nb_long, kThreads, 0, st>>>(
                     g.n_long, g.long_rows, g.long_seg_ptr, segp, al, peers, sy);
                 count_launch();
             }
         }
-    }, mode == 0 && io.prevh != nullptr, mode == 1, io.partials != nullptr);
+    }, mode == 0 && (io.prevh != nullptr || io.x0c == kX0AsPrev), mode == 1, io.partials != nullptr,
+       io.x0c == kX0AsX, io.x0c == kX0AsPrev);
     if (grid.nb_rows + grid.nb_long == 0 && sharded) HRAG_TRY(epoch_signal(sy, st));
     if (n_partials) *n_partials = grid.nb_rows + grid.nb_long;
     HRAG_CUDA(cudaGetLastError());
@@ -724,14 +786,17 @@ int mixed_sweep2(const PprGraph& g, int mode, const MixedSweepIO (&io)[2], float
     HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep2: graph not loaded");
     HRAG_CHECK(kB <= g.max_batch, "mixed_sweep2: segment partials too small for 32 columns");
     HRAG_CHECK((io[0].partials == nullptr) == (io[1].partials == nullptr), "mixed_sweep2: partials for both or neither");
+    HRAG_CHECK(io[0].x0c == io[1].x0c && (io[0].x0c == kX0Dense || (io[0].slot_map && io[1].slot_map && mode == 0)),
+               "mixed_sweep2: the compact first iterate needs a compact rhs for both states");
     const SweepGrid grid(g, kGPB);
     const SweepArgs a[2] = {sweep_args(g, io[0], alpha, w, t, overflow), sweep_args(g, io[1], alpha, w, t, overflow)};
     F8* segp = reinterpret_cast<F8*>(g.seg_partial);
-    with_bools([&](auto cheb, auto resid, auto fin) {
-        if constexpr (!(cheb && resid)) {
+    with_bools([&](auto cheb, auto resid, auto fin, auto x0x, auto x0p) {
+        if constexpr (!(cheb && resid) && !(x0x && (cheb || resid)) && !(x0p && (!cheb || resid))) {
             constexpr int M = resid ? 1 : 0;
+            constexpr int X0C = x0x ? kX0AsX : x0p ? kX0AsPrev : kX0Dense;
             if (grid.nb_rows) {
-                k_sweep_h2<cheb, M, fin><<<grid.nb_rows, kThreads, 0, st>>>(a[0], a[1]);
+                k_sweep_h2<cheb, M, fin, X0C><<<grid.nb_rows, kThreads, 0, st>>>(a[0], a[1]);
                 count_launch();
             }
             // long rows: the single-state segment and finalize kernels, once per state (seg_partial is reused in
@@ -739,14 +804,18 @@ int mixed_sweep2(const PprGraph& g, int mode, const MixedSweepIO (&io)[2], float
             for (int k = 0; k < 2 && grid.nb_long; ++k) {
                 SweepArgs al = a[k];
                 al.partials = al.partials ? al.partials + (size_t)grid.nb_rows * kB : nullptr;
-                k_sweep_long_segments_h<kRS2><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, al.xh, segp,
-                                                                               SweepSync());
-                k_sweep_long_finalize_h<cheb, M, fin, kRS2><<<grid.nb_long, kThreads, 0, st>>>(
+                if constexpr (X0C == kX0AsX)
+                    k_sweep_long_segments_h<kLPR, RhsRows><<<grid.nb_seg, kThreads, 0, st>>>(
+                        g.n_seg, g.segs, g.cv, RhsRows{al.slot_map, al.rhs_h}, segp, SweepSync());
+                else k_sweep_long_segments_h<kRS2><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, al.xh,
+                                                                                      segp, SweepSync());
+                k_sweep_long_finalize_h<cheb, M, fin, kRS2, X0C == kX0AsPrev><<<grid.nb_long, kThreads, 0, st>>>(
                     g.n_long, g.long_rows, g.long_seg_ptr, segp, al, PeerOut(), SweepSync());
                 count_launch(2);
             }
         }
-    }, mode == 0 && io[0].prevh != nullptr, mode == 1, io[0].partials != nullptr);
+    }, mode == 0 && (io[0].prevh != nullptr || io[0].x0c == kX0AsPrev), mode == 1, io[0].partials != nullptr,
+       io[0].x0c == kX0AsX, io[0].x0c == kX0AsPrev);
     if (n_partials) *n_partials = grid.nb_rows + grid.nb_long;
     HRAG_CUDA(cudaGetLastError());
     return 0;
@@ -785,9 +854,11 @@ int compact_prepare_rhs(const SeedTables& t, int nb, int q0, const float* S, int
     const int n_seed_slots = kB * slots_per_query;
     HRAG_CHECK(slots_per_query > 0, "compact_prepare_rhs: slots_per_query must be positive");
     const int nblk = compact_rhs_partial_rows(P);
-    HRAG_CHECK(x0_ld == kB || x0_ld == 2 * kB, "compact_prepare_rhs: x0 rows are 32 or 64 halves apart");
-    if (x0_ld == kB) HRAG_CUDA(cudaMemsetAsync(x0_dense, 0, (size_t)n_nodes * kB * 2, st));
-    else HRAG_CUDA(cudaMemset2DAsync(x0_dense, (size_t)x0_ld * 2, 0, kB * 2, (size_t)n_nodes, st));
+    if (x0_dense) {
+        HRAG_CHECK(x0_ld == kB || x0_ld == 2 * kB, "compact_prepare_rhs: x0 rows are 32 or 64 halves apart");
+        if (x0_ld == kB) HRAG_CUDA(cudaMemsetAsync(x0_dense, 0, (size_t)n_nodes * kB * 2, st));
+        else HRAG_CUDA(cudaMemset2DAsync(x0_dense, (size_t)x0_ld * 2, 0, kB * 2, (size_t)n_nodes, st));
+    }
     HRAG_CUDA(cudaMemsetAsync(Vc + (size_t)P * kB, 0, (size_t)n_seed_slots * kB * sizeof(float), st));
     k_rhs_passages<<<nblk, 256, 0, st>>>(P, nb, S, ldS, q0, minmax, pnw, Vc, partials);
     k_rhs_seeds<<<1, 1024, 0, st>>>(P, nb, q0, slots_per_query, seed_vid, seed_w, slot_map, slot_vid, Vc,

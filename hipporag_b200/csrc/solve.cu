@@ -169,12 +169,15 @@ static float cheb_step(int it, float alpha, double* w, T* a, T* c, T* prev, T** 
 
 // One sweep of the n sub-batches of a solve in layout L (n = 2: one paired walk over the interleaved buffers x, prev,
 // y).  in[k] holds sub-batch k's slot_map, rhs_h, v32 and col_scale; a dense rhs_h (slot_map null) is a buffer of L
-// like x.  final: the column-sum partials of sub-batch k go to h->mixed_part[k].
+// like x.  final: the column-sum partials of sub-batch k go to h->mixed_part[k].  x0c: MixedSweepIO::x0c (x or prev
+// is then null).
 static int mixed_sweep_n(hrag_t* h, const StateLayout& L, int n, int mode, const MixedSweepIO* in, const void* x,
-                         const void* prev, void* y, float alpha, float w, float t, bool final, int* n_part) {
+                         const void* prev, void* y, float alpha, float w, float t, bool final, int* n_part,
+                         int x0c = 0) {
     MixedSweepIO io[2];
     for (int k = 0; k < n; ++k) {
         io[k] = in[k];
+        io[k].x0c = x0c;
         if (!io[k].slot_map) io[k].rhs_h = L.part(io[k].rhs_h, k);
         io[k].xh = L.part(x, k);
         io[k].prevh = L.part(prev, k);
@@ -194,8 +197,9 @@ static int mixed_sums(hrag_t* h, int n, int n_part, double (MixedSums::*which)[3
 }
 
 // m Chebyshev sweeps of the fp16 solver on (I - aP) x = rhs for n sub-batches in layout L, first iterate x_first (= rhs
-// as a dense buffer of L); rhs[k] holds sub-batch k's rhs_h and its slot_map (null = dense).  Iterates alternate
-// between bufA and bufC; *result = the last one, its column sums land in the sub-batches' MixedSums' `which`.
+// as a dense buffer of L; null: the compact rhs itself, read through its slot map by sweeps 1 and 2); rhs[k] holds
+// sub-batch k's rhs_h and its slot_map (null = dense).  Iterates alternate between bufA and bufC; *result = the last
+// one, its column sums land in the sub-batches' MixedSums' `which`.
 static int mixed_cheb(hrag_t* h, const StateLayout& L, int n, const MixedSweepIO* rhs, void* x_first, void* bufA,
                       void* bufC, int m, float alpha, void** result, double (MixedSums::*which)[32]) {
     HRAG_CHECK(m >= 1, "mixed solver: sweep count must be >= 1");
@@ -204,7 +208,8 @@ static int mixed_cheb(hrag_t* h, const StateLayout& L, int n, const MixedSweepIO
     int n_part = 0;
     for (int it = 1; it <= m; ++it) {
         const float wf = cheb_step(it, alpha, &w, bufA, bufC, prev, &y);
-        HRAG_TRY(mixed_sweep_n(h, L, n, 0, rhs, x, prev, y, alpha, wf, 1.f, it == m, &n_part));
+        const int x0c = x_first || it > 2 ? 0 : it;      // 1: x is the compact rhs, 2: prev is
+        HRAG_TRY(mixed_sweep_n(h, L, n, 0, rhs, x, prev, y, alpha, wf, 1.f, it == m, &n_part, x0c));
         prev = x;
         x = y;
         h->stats.ppr_sweeps += n;
@@ -270,10 +275,12 @@ static int dev_ppr_mixed_body(hrag_t* h, const SweepPlan& plan, float alpha, int
         resid[k].col_scale = in[k].scale;
         corr[k].rhs_h = L.R;
     }
+    // x0_dense is also the correction's first work buffer, which its first sweep overwrites in full
     void* x0_dense = in[0].x0_dense;
     void* x0 = nullptr;
     void* d = nullptr;
-    HRAG_TRY(mixed_cheb(h, L, n, first, x0_dense, L.A, L.C, plan.m1, alpha, &x0, &MixedSums::x0));
+    HRAG_TRY(mixed_cheb(h, L, n, first, in[0].x0_compact ? nullptr : x0_dense, L.A, L.C, plan.m1, alpha, &x0,
+                        &MixedSums::x0));
     void* other = (x0 == L.A) ? L.C : L.A;
     int n_part = 0;
     HRAG_TRY(mixed_sweep_n(h, L, n, 1, resid, x0, nullptr, L.R, alpha, 1.f, kMixedT, true, &n_part));
@@ -359,12 +366,14 @@ int ensure_stage_b_mixed(hrag_t* h, int Bq, int k_facts) {
 }
 
 // Two streams: stream2 builds solve i+1's compact right-hand sides (passage weights + phrase seeds on P + 2048 slots,
-// column scales, the fp16 copy and the dense first iterate) while `stream` runs the sweeps of solve i.  Solve i (one
-// sub-batch, or a pair) uses the sets of parity i & 1: set p, and p + 2 for the second sub-batch of a pair, and the
-// first iterate x0[p] of its layout.
+// column scales and the fp16 copy) while `stream` runs the sweeps of solve i.  Solve i (one sub-batch, or a pair) uses
+// the sets of parity i & 1: set p, and p + 2 for the second sub-batch of a pair, and the buffer x0[p] of its layout.
+// On one GPU the first solve reads its first iterate compactly (MixedRhs::x0_compact); node-range sharding, whose
+// peers exchange the rows of every sweep's input, and hrag_debug_dense_first_sweep scatter it into x0[p] first.
 int stage_b_mixed(hrag_t* h, const SweepPlan& plan, int Bq, float* S, int64_t ldS, const float2* mm_pass, float pnw,
                   float damping) {
     const bool pairs = solve_in_pairs(h, Bq);
+    const bool x0_compact = h->world == 1 && !h->debug_dense_first_sweep;
     if (plan.check) h->check_tol = std::max(h->check_tol, plan.tol), h->check_kappa = plan.kappa;
     HRAG_CUDA(cudaEventRecord(h->ev_inputs, h->stream));            // S, min/max, seed lists are ready
     HRAG_CUDA(cudaStreamWaitEvent(h->stream2, h->ev_inputs, 0));
@@ -381,6 +390,7 @@ int stage_b_mixed(hrag_t* h, const SweepPlan& plan, int Bq, float* S, int64_t ld
             const int qk = q0 + 32 * k;
             nb[k] = std::min(32, Bq - qk);
             in[k].x0_dense = L.x0[par];
+            in[k].x0_compact = x0_compact;
             in[k].slot_map = set.slot_map.as<int>();
             in[k].Vexact = set.Vc.as<float>();
             in[k].rhs16 = set.R16.p;
@@ -388,7 +398,8 @@ int stage_b_mixed(hrag_t* h, const SweepPlan& plan, int Bq, float* S, int64_t ld
             in[k].vsum = set.vsum.as<double>();
             HRAG_TRY(compact_prepare_rhs(h->t, nb[k], qk, S, ldS, mm_pass, pnw, kSeedSlots, h->seed_vid.as<int>(),
                                          h->seed_w.as<double>(), damping, set.slot_map.as<int>(),
-                                         set.slot_vid.as<int>(), set.Vc.as<float>(), set.R16.p, L.part(L.x0[par], k),
+                                         set.slot_vid.as<int>(), set.Vc.as<float>(), set.R16.p,
+                                         x0_compact ? nullptr : L.part(L.x0[par], k),
                                          L.ld, (int64_t)h->g.n_global, h->prep_scratch.as<float>(),
                                          set.vsum.as<double>(), set.scale.as<float>(), h->stream2));
         }
@@ -610,8 +621,10 @@ int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float
     HRAG_CHECK(h->g.n_global > 0, "hrag_bench_sweep: graph not loaded");
     HRAG_CUDA(cudaSetDevice(h->device));
     // fp16-state sweep (Chebyshev form), B = 32: 2 = dense rhs, 3 = compact rhs, 4 = the paired sweep of two
-    // compact-rhs sub-batches ([N, 2, 32] state), timed per paired sweep (64 columns)
-    const bool paired = method == 4;
+    // compact-rhs sub-batches ([N, 2, 32] state), timed per paired sweep (64 columns); 5 / 6 = the paired first sweep
+    // of a solve (plain), gathering the dense first iterate x0 (5) or the compact rhs through the slot maps (6)
+    const bool first = method == 5 || method == 6;
+    const bool paired = method == 4 || first;
     const bool mixed = method == 2 || method == 3 || paired;
     HRAG_CHECK(!paired || h->world == 1, "hrag_bench_sweep: the paired sweep runs on a single-GPU handle");
     const bool cheb = method == HRAG_PPR_CHEBYSHEV;
@@ -636,7 +649,7 @@ int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float
         A = L.A, C = L.C;
         if (paired) {
             HRAG_TRY(ensure_state_pair(h));
-            for (void* p : {h->pair.A, h->pair.C}) HRAG_CUDA(cudaMemsetAsync(p, 0x2c, 2 * hb, h->stream));
+            for (void* p : {h->pair.x0[0], h->pair.A, h->pair.C}) HRAG_CUDA(cudaMemsetAsync(p, 0x2c, 2 * hb, h->stream));
             A = h->pair.A, C = h->pair.C;
         }
     } else {
@@ -657,7 +670,11 @@ int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float
             void* x = (i & 1) ? C : A;
             void* y = (i & 1) ? A : C;
             float* yf = static_cast<float*>(y);
-            if (mixed) {
+            if (first) {
+                const bool dense = method == 5;
+                HRAG_TRY(mixed_sweep_n(h, h->pair, 2, 0, rhs, dense ? h->pair.x0[0] : nullptr, nullptr, y, 0.5f, 1.f,
+                                       1.f, false, nullptr, dense ? 0 : 1));
+            } else if (mixed) {
                 HRAG_TRY(mixed_sweep_n(h, paired ? h->pair : h->single, paired ? 2 : 1, 0, rhs, x, y, y, 0.5f, 1.07f,
                                        1.f, false, nullptr));
             } else {

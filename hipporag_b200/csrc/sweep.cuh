@@ -106,17 +106,21 @@ struct LaneF64 {
 // lane (the sweep is bound by gather latency x bandwidth, not by FMA issue); each lane sums in non-zero order.
 // S = 1 walks a whole short row; S = 32 / LPR is one group's share of a long-row segment.  x is already + lane.
 // (The bound is written `+ 1 <=`: nvcc unrolls the `i + 3 * S < e` form 4x more at S = 1, a larger k_sweep_rows.)
-// RS: the state's row stride in X units (LPR unless two states are interleaved row by row).
-template <class L, int LPR, int S, int RS = LPR>
+// RS: the state's row stride in X units (LPR unless two states are interleaved row by row).  x is the state itself, or
+// any source with a gather_row overload (ppr_mixed.cu reads a compact first iterate through its slot map).
+template <int RS, class X>
+__device__ __forceinline__ X gather_row(const X* __restrict__ x, int col) { return __ldg(x + (size_t)col * RS); }
+
+template <class L, int LPR, int S, int RS = LPR, class Src = const typename L::X*>
 __device__ __forceinline__ typename L::Acc row_walk(const int2* __restrict__ cv, const float* __restrict__ lo, int i,
-                                                    int e, const typename L::X* __restrict__ x) {
+                                                    int e, const Src x) {
     typename L::Acc acc = L::zero();
     for (; i + 3 * S + 1 <= e; i += 4 * S) {
         const int2 c0 = __ldg(cv + i), c1 = __ldg(cv + i + S), c2 = __ldg(cv + i + 2 * S), c3 = __ldg(cv + i + 3 * S);
-        const auto a0 = __ldg(x + (size_t)c0.x * RS);
-        const auto a1 = __ldg(x + (size_t)c1.x * RS);
-        const auto a2 = __ldg(x + (size_t)c2.x * RS);
-        const auto a3 = __ldg(x + (size_t)c3.x * RS);
+        const auto a0 = gather_row<RS>(x, c0.x);
+        const auto a1 = gather_row<RS>(x, c1.x);
+        const auto a2 = gather_row<RS>(x, c2.x);
+        const auto a3 = gather_row<RS>(x, c3.x);
         L::fma(acc, L::coef(c0, lo, i), a0);
         L::fma(acc, L::coef(c1, lo, i + S), a1);
         L::fma(acc, L::coef(c2, lo, i + 2 * S), a2);
@@ -124,22 +128,22 @@ __device__ __forceinline__ typename L::Acc row_walk(const int2* __restrict__ cv,
     }
     for (; i < e; i += S) {
         const int2 c = __ldg(cv + i);
-        L::fma(acc, L::coef(c, lo, i), __ldg(x + (size_t)c.x * RS));
+        L::fma(acc, L::coef(c, lo, i), gather_row<RS>(x, c.x));
     }
     return acc;
 }
 
 // Body of the segment kernels: warp w of the grid sums segment w of the long rows; the groups of the warp are then
 // added by butterfly and the warp's LPR lane slices go to seg_partial[w].
-template <class L, int LPR, int RS = LPR>
+template <class L, int LPR, int RS = LPR, class Src = const typename L::X*>
 __device__ __forceinline__ void segment_partial(int n_seg, const int4* __restrict__ segs, const int2* __restrict__ cv,
-                                                const float* __restrict__ lo, const typename L::X* __restrict__ x,
+                                                const float* __restrict__ lo, const Src x,
                                                 typename L::Acc* __restrict__ seg_partial) {
     const int warp = (blockIdx.x * kThreads + threadIdx.x) >> 5;
     if (warp >= n_seg) return;
     const int lane = threadIdx.x & 31;
     const int4 sg = __ldg(segs + warp);
-    typename L::Acc acc = row_walk<L, LPR, 32 / LPR, RS>(cv, lo, sg.y + lane / LPR, sg.z, x + lane % LPR);
+    typename L::Acc acc = row_walk<L, LPR, 32 / LPR, RS, Src>(cv, lo, sg.y + lane / LPR, sg.z, x + lane % LPR);
 #pragma unroll
     for (int off = LPR; off < 32; off <<= 1) L::shfl_xor_add(acc, off);
     if (lane < LPR) seg_partial[(size_t)warp * LPR + lane] = acc;

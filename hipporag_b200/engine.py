@@ -555,6 +555,11 @@ class Engine:
         retrieve_resident, n < 0 runs retrieve_resident's chunks without the overlap, 0 restores the defaults."""
         _lib.check(self._lib.hrag_debug_sim_ctas(self._h, int(n)))
 
+    def debug_dense_first_sweep(self, on: bool = True):
+        """Make stage B's mixed solves build and sweep the dense first iterate instead of reading the compact right-hand
+        side through the slot map (tests, benchmarks: both give the same bytes); False restores the default."""
+        _lib.check(self._lib.hrag_debug_dense_first_sweep(self._h, 1 if on else 0))
+
     def debug_scores(self, which: int) -> np.ndarray:
         cols = self.n_facts if which == 0 else self.n_passages
         buf = np.empty(1024 * max(cols, 1), dtype=np.float32)

@@ -315,7 +315,9 @@ int hrag_knn_index_clear(hrag_t* h);
 /* K1 micro-benchmark: runs `sweeps` SpMM sweeps at batch width B on resident synthetic
  * state and returns the average milliseconds per sweep (CUDA events on the launch stream).
  * method: 0 power / 1 Chebyshev (fp32 state), 2 fp16 state with a dense rhs, 3 fp16 state with the
- * compact rhs of stage B (needs hrag_load_tables). */
+ * compact rhs of stage B (needs hrag_load_tables), 4 the paired sweep of two such sub-batches ([N, 2, 32] state, time
+ * per paired sweep); 5 / 6 the paired FIRST sweep of a stage-B solve (plain, no prev), 5 gathering the dense first
+ * iterate, 6 the compact rhs through the slot maps of the passages. */
 int hrag_bench_sweep(hrag_t* h, int32_t B, int32_t sweeps, int32_t method, float* ms_per_sweep);
 
 /* The CUDA stream (cudaStream_t) every call of this handle is ordered on: a call starts after the work already on
@@ -351,6 +353,10 @@ int hrag_debug_keep_scores(hrag_t* h, int keep);
  * CTAs instead of the count derived from the shapes; n < 0: hrag_retrieve_resident runs its chunks one after the
  * other without the overlap; n = 0 restores the defaults. */
 int hrag_debug_sim_ctas(hrag_t* h, int n);
+/* on != 0: stage B's mixed solves scatter their right-hand side into a dense first iterate and sweep it, as
+ * node-range-sharded handles do, instead of reading it through the slot map (tests and benchmarks compare the two
+ * forms; the results are the same bit for bit); 0 restores the default. */
+int hrag_debug_dense_first_sweep(hrag_t* h, int on);
 
 #ifdef __cplusplus
 }
