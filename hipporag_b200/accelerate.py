@@ -173,7 +173,7 @@ def _resident_knn_applies(query_ids, key_ids, query_vecs, key_vecs, thr: float) 
 
 def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_workers: int = 1,
                filter_chunk: int = 256, ppr_tol: float = 0.0, cache: bool = True, run_ppr_fp64: bool = False,
-               incremental: bool = False, **engine_opts):
+               incremental: bool = False, fact_device_bytes: Optional[int] = None, **engine_opts):
     """Rebinds the hot-path methods of ``rag`` (a reference ``HippoRAG`` instance) in place.
 
     ``filter_workers > 1`` (SURVEY.md 8(f)-1) runs the per-query recognition-memory filter calls (LLM HTTP
@@ -202,6 +202,11 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     "unchanged" or "per-call").  Incremental updates do not
     write the binary cache: the next cold start rebuilds it, as after any change today.  The default
     (``incremental=False``) loads the host-built CSR and reloads everything after ``index()`` / ``delete()``.
+    ``fact_device_bytes`` (``Engine.set_fact_memory``): device memory the fact planes may take; a fact matrix larger
+    than that is kept in pinned host memory and streamed through the GPU by every stage-A call, with the same results.
+    Stage A then streams the planes once per call, so ``filter_workers > 1`` streams them once per ``filter_chunk``
+    queries: give it a large ``filter_chunk``.  Host planes cannot be updated in place: with ``incremental=True``
+    every ``index()`` / ``delete()`` takes the full reload.
     ``engine_opts`` go to ``Engine.set_options``.
     """
     from hipporag.utils.misc_utils import QuerySolution
@@ -222,6 +227,8 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         elif incremental and not state.get("mutable_set"):
             state["engine"].set_mutable()
         state["mutable_set"] = incremental
+        if fact_device_bytes is not None:     # before every load, which is what applies it
+            state["engine"].set_fact_memory(fact_device_bytes)
         return state["engine"]
 
     def _embeddings(self):

@@ -36,7 +36,8 @@ int sim_dispatch(hrag_t* h, const float* dQ, int Bq, int which, float* S, int64_
 
 constexpr int kFusedTopK = 8;     // candidates the GEMM epilogue / row_minmax_topk keep in registers
 bool fused_stage_a(hrag_t* h, int k) {   // tensor-core modes select facts in the GEMM epilogue (no score matrix)
-    return h->sim_mode != HRAG_SIM_FP32 && h->emb[0].hi.p != nullptr && !h->keep_fact_scores && k <= kFusedTopK;
+    return h->sim_mode != HRAG_SIM_FP32 && (h->emb[0].hi.p != nullptr || h->fplanes.held()) && !h->keep_fact_scores &&
+           k <= kFusedTopK;
 }
 
 int64_t chunk_a(hrag_t* h, int k) {
@@ -250,7 +251,8 @@ int dev_stage_b_solve_f64(hrag_t* h, int Bq, const float* S, const float2* mm_pa
 int overlap_ctas(const hrag_t* h, int Bq, const SweepPlan& plan) {
     constexpr double kGemmFlopPerSmMs = 2.49e9, kSweepNnzPerMs = 3.80e7;
     const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
-    const double gemm_flop = 2.0 * n_seg * Bq * (double)(h->emb[0].rows + h->emb[1].rows) * h->dim;
+    const int64_t fact_rows = h->fplanes.held() ? 0 : h->emb[0].rows;   // streamed planes: stage A ran up front
+    const double gemm_flop = 2.0 * n_seg * Bq * (double)(fact_rows + h->emb[1].rows) * h->dim;
     const int64_t sweeps = plan.mixed ? (int64_t)(plan.m1 + 1 + plan.m2) * ceil_div(Bq, 32)
                                       : (int64_t)plan.iters * ceil_div(Bq, round_batch(std::min(h->ppr_batch, Bq)));
     const double t_sweep = (double)sweeps * (double)h->g.nnz / kSweepNnzPerMs;
@@ -412,7 +414,10 @@ int hrag_stage_a(hrag_t* h, int32_t B, const float* q_fact, int32_t k, int32_t* 
     HRAG_TRY(h->d_top_idx.ensure((size_t)std::max(B, 1) * k * sizeof(int)));
     HRAG_TRY(h->d_top_score.ensure((size_t)std::max(B, 1) * k * sizeof(float)));
     HRAG_TRY(h->d_nvalid.ensure((size_t)std::max(B, 1) * sizeof(int)));
-    for (int64_t q0 = 0; q0 < B; q0 += chunk) {
+    if (h->fplanes.held())   // fact planes in host memory: one pass over them per fact_stream_pass_cap queries
+        HRAG_TRY(fact_stream_stage_a(h, B, q_fact, false, k, h->d_top_idx.as<int>(), h->d_top_score.as<float>(),
+                                     h->d_nvalid.as<int>()));
+    for (int64_t q0 = 0; q0 < B && !h->fplanes.held(); q0 += chunk) {
         const int nb = (int)std::min<int64_t>(chunk, B - q0);
         HRAG_TRY(h2d(h, h->d_q.p, q_fact + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
         HRAG_TRY(dev_stage_a(h, nb, h->d_q.as<float>(), k, h->d_top_idx.as<int>() + q0 * k,
@@ -496,22 +501,35 @@ int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const fl
         HRAG_TRY(top_score[s]->ensure((size_t)chunk * k * sizeof(float)));
         HRAG_TRY(nvalid[s]->ensure((size_t)chunk * sizeof(int)));
     }
+    // fact planes in host memory: stage A of the whole call first, in one pass over the planes (per
+    // fact_stream_pass_cap queries), into fs_top_* [B, k]; the chunks below then skip their stage A
+    const bool streamed = h->fplanes.held();
+    if (streamed) {
+        HRAG_TRY(h->fs_top_idx.ensure((size_t)std::max(B, 1) * k * sizeof(int)));
+        HRAG_TRY(h->fs_top_score.ensure((size_t)std::max(B, 1) * k * sizeof(float)));
+        HRAG_TRY(h->fs_nvalid.ensure((size_t)std::max(B, 1) * sizeof(int)));
+        HRAG_TRY(fact_stream_stage_a(h, B, d_q_fact, true, k, h->fs_top_idx.as<int>(), h->fs_top_score.as<float>(),
+                                     h->fs_nvalid.as<int>()));
+    }
     // chunk c's similarity part on stream sim_s into slot c % 2 (stage A, then the passage GEMM + min/max)
     auto slot = [&](int64_t c) { return overlap ? (int)(c & 1) : 0; };
     auto similarity = [&](int64_t c, cudaStream_t sim_s, int n_ctas) -> int {
         const int64_t q0 = c * chunk;
         const int nb = (int)std::min<int64_t>(chunk, B - q0), s = slot(c);
-        HRAG_TRY(dev_stage_a(h, nb, d_q_fact + (size_t)q0 * h->dim, k, top_idx[s]->as<int>(), top_score[s]->as<float>(),
-                             nvalid[s]->as<int>(), sim_s, n_ctas));
+        if (!streamed)
+            HRAG_TRY(dev_stage_a(h, nb, d_q_fact + (size_t)q0 * h->dim, k, top_idx[s]->as<int>(),
+                                 top_score[s]->as<float>(), nvalid[s]->as<int>(), sim_s, n_ctas));
         return dev_stage_b_sim(h, nb, d_q_pass + (size_t)q0 * h->dim, *S_pass[s], *mm_pass[s], sim_s, n_ctas);
     };
     // chunk c's solve part on `stream` (identity recognition-memory filter: the candidates are the kept facts)
     auto solve = [&](int64_t c) -> int {
         const int64_t q0 = c * chunk;
         const int nb = (int)std::min<int64_t>(chunk, B - q0), s = slot(c);
-        return dev_stage_b_solve(h, nb, S_pass[s]->as<float>(), mm_pass[s]->as<float2>(), top_idx[s]->as<int>(),
-                                 top_score[s]->as<float>(), k, nullptr, damping, passage_node_weight, link_top_k, topk,
-                                 iters, tol, d_out_ids + q0 * topk, d_out_scores + q0 * topk);
+        const int* kept_idx = streamed ? h->fs_top_idx.as<int>() + q0 * k : top_idx[s]->as<int>();
+        const float* kept_score = streamed ? h->fs_top_score.as<float>() + q0 * k : top_score[s]->as<float>();
+        return dev_stage_b_solve(h, nb, S_pass[s]->as<float>(), mm_pass[s]->as<float2>(), kept_idx, kept_score, k,
+                                 nullptr, damping, passage_node_weight, link_top_k, topk, iters, tol,
+                                 d_out_ids + q0 * topk, d_out_scores + q0 * topk);
     };
     // one chunk, node-range sharding (its all-gathers and spin-waiting sweeps must not share SMs), or hrag_debug_sim_ctas
     if (!overlap) {
@@ -558,7 +576,8 @@ int hrag_similarity(hrag_t* h, int which, int32_t B, const float* q, float* out)
     for (int64_t q0 = 0; q0 < B; q0 += chunk) {
         const int nb = (int)std::min<int64_t>(chunk, B - q0);
         HRAG_TRY(h2d(h, h->d_q.p, q + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
-        HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld, h->stream, h->num_sms));
+        if (which == 0 && h->fplanes.held()) HRAG_TRY(fact_stream_scores(h, nb, h->d_q.as<float>(), Sb.as<float>(), ld));
+        else HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld, h->stream, h->num_sms));
         HRAG_TRY(row_minmax_topk(Sb.as<float>(), nb, M, ld, 0, mm.as<float2>(), nullptr, nullptr, nullptr, h->stream));
         HRAG_TRY(minmax_apply(Sb.as<float>(), nb, M, ld, mm.as<float2>(), h->stream));
         HRAG_CUDA(cudaMemcpy2DAsync(out + (size_t)q0 * M, (size_t)M * sizeof(float), Sb.p, (size_t)ld * sizeof(float),
@@ -589,7 +608,10 @@ int hrag_topk_similarity(hrag_t* h, int which, int32_t B, const float* q, int32_
         HRAG_TRY(h2d(h, h->d_q.p, q + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
         {
             StageTimer tm(h, which == 0 ? ST_SIM_FACT : ST_SIM_PASS);
-            HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld, h->stream, h->num_sms));
+            if (which == 0 && h->fplanes.held())
+                HRAG_TRY(fact_stream_scores(h, nb, h->d_q.as<float>(), Sb.as<float>(), ld));
+            else
+                HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld, h->stream, h->num_sms));
         }
         {
             StageTimer tm(h, ST_TOPK);
@@ -607,6 +629,9 @@ int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float mi
                        int32_t* out_ids, float* out_scores, int32_t* n_found) {
     HRAG_CHECK(h && q && out_ids && out_scores && n_found && (which == 0 || which == 1), "hrag_knn_threshold: bad arguments");
     HRAG_CHECK(kmax >= 1 && kmax <= kCandidateCap && B >= 0, "hrag_knn_threshold: kmax must be in [1, 512]");
+    HRAG_CHECK(which == 1 || !h->fplanes.held(),
+               "hrag_knn_threshold: the fact planes are held in host memory (hrag_set_fact_memory); the threshold "
+               "search runs on resident planes only");
     HRAG_CHECK(h->dim > 0 && h->emb[which].rows > 0 && h->emb[which].hi.p != nullptr,
                "hrag_knn_threshold: embeddings not loaded (needs the tensor-core layout: dim % 8 == 0)");
     HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, "hrag_knn_threshold: the threshold epilogue lives in the tensor-core kernel");

@@ -1,0 +1,337 @@
+// Fact matrices larger than the device budget of hrag_set_fact_memory: the bf16 hi / lo fact planes live in pinned
+// host memory and stream through a device ring of two slices while stage A runs.  A copy stream fills one half of the
+// ring with slice s + 1 while the similarity GEMM (K2, unchanged) reads slice s from the other half; events order the
+// two.  One call streams the planes once for all of its queries: slices are the outer loop, query chunks the inner.
+//
+// Results are bit for bit those of the resident planes: K2's accumulator for a (query, fact) pair does not depend on
+// the tile the fact falls in, and a slice starts on a 256-row tile boundary.  The fused top-8 path merges each slice's
+// per-tile lists with the slice's first row as index offset and folds the per-slice lists into a running one with the
+// same kernel the fact-sharded stage A uses across ranks (merge_minmax_topk_ex); the materialised path (k > 8, or
+// hrag_debug_keep_scores) takes each slice's exact top-k and (min, max) and folds them with fold_topk (select.cu).
+#include <algorithm>
+
+#include "handle.h"
+
+namespace hrag {
+
+int split_queries(hrag_t* h, const float* dQ, int Bq, cudaStream_t s);   // api.cu
+int64_t pad4(int64_t x);                                                  // api.cu
+
+namespace {
+
+constexpr int64_t kSliceAlign = 256;                // K2's tile width: every slice boundary is a tile boundary
+constexpr int kPassChunk = 1024;                     // queries per K2 launch, as in the resident fused stage A
+constexpr size_t kPassSplitBytes = size_t(256) << 20;   // bound on one pass's query splits (bf16 hi + lo)
+constexpr int kFusedK = 8;                           // the fused epilogue's list length
+
+const char* kNoFp32 = "similarity: the fact planes are held in host memory (hrag_set_fact_memory) and no fp32 copy "
+                      "of the fact rows is kept; only the tensor-core modes are available";
+
+// Walks the slices of the host planes on `stream`: body(s, first row, rows, hi, lo) reads slice s from its ring half
+// while the copy stream fills the other half with slice s + 1.  `both`: stream the lo plane too (HRAG_SIM_BF16 reads
+// only hi).  Every copy is joined into `stream` before its slice is read, so the caller's later work on `stream` sees
+// the whole walk.
+template <class Body> int stream_slices(hrag_t* h, bool both, Body body) {
+    FactPlanes& fp = h->fplanes;
+    const int64_t d = h->dim, S = fp.slice_rows, F = h->emb[0].rows;
+    const int64_t n_slices = ceil_div(F, S);
+    const size_t half_bytes = (size_t)S * d * 4;
+    char* ring = fp.ring.as<char>();
+    auto copy = [&](int64_t s) -> int {
+        const int64_t r0 = s * S, n = std::min(S, F - r0);
+        const int half = (int)(s & 1);
+        char* dst = ring + half * half_bytes;
+        HRAG_CUDA(cudaStreamWaitEvent(fp.copy, fp.freed[half], 0));   // the last read of this half is done
+        HRAG_CUDA(cudaMemcpyAsync(dst, static_cast<char*>(fp.hi) + (size_t)r0 * d * 2, (size_t)n * d * 2,
+                                  cudaMemcpyHostToDevice, fp.copy));
+        if (both)
+            HRAG_CUDA(cudaMemcpyAsync(dst + (size_t)S * d * 2, static_cast<char*>(fp.lo) + (size_t)r0 * d * 2,
+                                      (size_t)n * d * 2, cudaMemcpyHostToDevice, fp.copy));
+        h->stats.h2d_bytes += (int64_t)n * d * 2 * (both ? 2 : 1);
+        HRAG_CUDA(cudaEventRecord(fp.loaded[half], fp.copy));
+        return 0;
+    };
+    for (int i = 0; i < 2; ++i) HRAG_CUDA(cudaEventRecord(fp.freed[i], h->stream));   // after the earlier reads
+    HRAG_TRY(copy(0));
+    for (int64_t s = 0; s < n_slices; ++s) {
+        if (s + 1 < n_slices) HRAG_TRY(copy(s + 1));
+        const int half = (int)(s & 1);
+        HRAG_CUDA(cudaStreamWaitEvent(h->stream, fp.loaded[half], 0));
+        const char* e_hi = ring + half * half_bytes;
+        HRAG_TRY(body(s, s * S, std::min(S, F - s * S), e_hi, e_hi + (size_t)S * d * 2));
+        HRAG_CUDA(cudaEventRecord(fp.freed[half], h->stream));
+    }
+    return 0;
+}
+
+}  // namespace
+
+void FactPlanes::release() {
+    if (copy) cudaStreamSynchronize(copy);
+    if (hi) cudaFreeHost(hi);
+    if (lo) cudaFreeHost(lo);
+    hi = lo = nullptr;
+    plane_bytes = 0;
+    slice_rows = 0;
+    ring.reset();
+    run_mm.reset();
+    run_keys.reset();
+    sl_ids.reset();
+    sl_scores.reset();
+    sl_mm.reset();
+    tail.reset();
+    for (int i = 0; i < 2; ++i) {
+        if (loaded[i]) cudaEventDestroy(loaded[i]);
+        if (freed[i]) cudaEventDestroy(freed[i]);
+        loaded[i] = freed[i] = nullptr;
+    }
+    if (copy) cudaStreamDestroy(copy);
+    copy = nullptr;
+}
+
+int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows) {
+    *slice_rows = 0;
+    const int64_t plane_bytes = rows * (int64_t)dim * 4;   // hi + lo
+    if (h->fact_budget <= 0 || plane_bytes <= h->fact_budget) return 0;
+    HRAG_CHECK(h->world == 1, who + ": fact planes in host memory (hrag_set_fact_memory) serve one GPU only; a "
+                                    "node-range-sharded handle (world > 1) keeps its fact slice resident");
+    HRAG_CHECK(dim % 8 == 0, who + ": fact planes in host memory need dim % 8 == 0 (the tensor-core layout)");
+    const int64_t slice = h->fact_budget / (2 * (int64_t)dim * 4) / kSliceAlign * kSliceAlign;
+    HRAG_CHECK(slice >= kSliceAlign,
+               who + ": hrag_set_fact_memory budget of " + std::to_string(h->fact_budget) + " bytes is below the " +
+                   std::to_string(2 * kSliceAlign * dim * 4) + " bytes of a ring of two 256-row slices at dim " +
+                   std::to_string(dim));
+    *slice_rows = slice;
+    return 0;
+}
+
+int fact_planes_alloc(hrag_t* h, int64_t slice_rows) {
+    FactPlanes& fp = h->fplanes;
+    fp.release();
+    const int64_t d = h->dim, F = h->emb[0].rows;
+    fp.plane_bytes = (size_t)F * d * 2;
+    HRAG_CUDA(cudaHostAlloc(&fp.hi, fp.plane_bytes, cudaHostAllocDefault));
+    HRAG_CUDA(cudaHostAlloc(&fp.lo, fp.plane_bytes, cudaHostAllocDefault));
+    fp.slice_rows = slice_rows;
+    HRAG_TRY(fp.ring.ensure((size_t)2 * slice_rows * d * 4));
+    HRAG_CUDA(cudaStreamCreateWithFlags(&fp.copy, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; ++i) {
+        HRAG_CUDA(cudaEventCreateWithFlags(&fp.loaded[i], cudaEventDisableTiming));
+        HRAG_CUDA(cudaEventCreateWithFlags(&fp.freed[i], cudaEventDisableTiming));
+    }
+    return 0;
+}
+
+// Ring half 0 stages up to slice_rows fp32 rows (slice_rows x dim x 4 bytes: exactly one half), half 1 takes their
+// split (hi rows, then lo rows), which goes back to the pinned planes.  split_bf16 is element-wise, so the planes are
+// byte for byte those of a resident load.
+int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool src_on_device) {
+    FactPlanes& fp = h->fplanes;
+    const int64_t d = h->dim, S = fp.slice_rows;
+    char* stage = fp.ring.as<char>();
+    char* split = stage + (size_t)S * d * 4;
+    for (int64_t r = 0; r < n; r += S) {
+        const int64_t m = std::min(S, n - r);
+        const size_t ne = (size_t)m * d;
+        const float* x = src + (size_t)r * d;
+        if (!src_on_device) {
+            HRAG_CUDA(cudaMemcpyAsync(stage, x, ne * 4, cudaMemcpyHostToDevice, h->stream));
+            x = reinterpret_cast<const float*>(stage);
+        }
+        HRAG_TRY(split_bf16(x, (int64_t)ne, split, split + (size_t)S * d * 2, h->stream));
+        const size_t at = (size_t)(row0 + r) * d * 2;
+        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(fp.hi) + at, split, ne * 2, cudaMemcpyDeviceToHost, h->stream));
+        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(fp.lo) + at, split + (size_t)S * d * 2, ne * 2,
+                                  cudaMemcpyDeviceToHost, h->stream));
+    }
+    HRAG_CUDA(cudaStreamSynchronize(h->stream));
+    return 0;
+}
+
+// Queries per pass: their bf16 hi / lo splits (dim x 4 bytes each) stay on the device for the whole pass and are
+// bounded by kPassSplitBytes (256 MB): 65,536 queries at dim 1024, 16,384 at dim 4096.  A call with more queries
+// streams the planes once per pass.
+int64_t fact_stream_pass_cap(const hrag_t* h) {
+    const int64_t per_query = 4 * (int64_t)std::max(h->dim, 1);
+    return std::max<int64_t>(kPassChunk, (int64_t)kPassSplitBytes / per_query / kPassChunk * kPassChunk);
+}
+
+int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* d_top_idx,
+                        float* d_top_score, int* d_nvalid) {
+    FactPlanes& fp = h->fplanes;
+    HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, std::string("stage A ") + kNoFp32);
+    h->last_fact_rows = 0;
+    if (B == 0) return 0;
+    const int64_t F = h->emb[0].rows, d = h->dim, S = fp.slice_rows;
+    const int64_t n_slices = ceil_div(F, S);
+    const bool fused = !h->keep_fact_scores && k <= kFusedK;
+    const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
+    const int n_ctas = h->debug_sim_ctas > 0 ? h->debug_sim_ctas : h->num_sms;
+    const int64_t cap = fact_stream_pass_cap(h);
+    const int64_t Bmax = std::min<int64_t>(cap, B);
+    // query chunk of one K2 launch: the fused partials are 72 B per (query, tile of the slice); a materialised slice
+    // row is pad4(slice_rows) floats (the resident rule of chunk_a, per slice instead of per matrix)
+    const int64_t ldS = pad4(S);
+    const int64_t chunk = fused ? kPassChunk
+                                : std::max<int64_t>(1, std::min<int64_t>((int64_t)(4e9 / (4.0 * (double)ldS)),
+                                                                         kPassChunk));
+    const int64_t cb = std::min<int64_t>(chunk, Bmax);
+    HRAG_TRY(h->q_hi.ensure((size_t)Bmax * d * 2));
+    HRAG_TRY(h->q_lo.ensure((size_t)Bmax * d * 2));
+    if (!q_on_device) HRAG_TRY(h->d_q.ensure((size_t)std::min<int64_t>(kPassChunk, Bmax) * d * 4));
+    if (fused) {
+        const int nt = sim_tc_n_tiles(S);
+        HRAG_TRY(h->part_mm.ensure((size_t)cb * nt * sizeof(float2)));
+        HRAG_TRY(h->part_keys.ensure((size_t)cb * nt * 8 * sizeof(uint64_t)));
+        HRAG_TRY(h->part_bound.ensure((size_t)cb * sizeof(uint64_t)));
+        HRAG_TRY(h->mm_fact.ensure((size_t)Bmax * sizeof(float2)));
+        HRAG_TRY(fp.run_mm.ensure((size_t)3 * Bmax * sizeof(float2)));     // slots: running x 2, this slice
+        HRAG_TRY(fp.run_keys.ensure((size_t)3 * Bmax * 8 * sizeof(uint64_t)));
+    } else {
+        HRAG_TRY(h->S_fact.ensure((size_t)cb * ldS * sizeof(float)));
+        HRAG_TRY(fp.sl_ids.ensure((size_t)cb * k * sizeof(int)));
+        HRAG_TRY(fp.sl_scores.ensure((size_t)cb * k * sizeof(float)));
+        HRAG_TRY(fp.sl_mm.ensure((size_t)cb * sizeof(float2)));
+        HRAG_TRY(fp.run_mm.ensure((size_t)Bmax * sizeof(float2)));
+    }
+    const char* q_hi = h->q_hi.as<char>();
+    const char* q_lo = h->q_lo.as<char>();
+    for (int64_t p0 = 0; p0 < B; p0 += cap) {
+        const int64_t Bp = std::min<int64_t>(cap, B - p0);
+        {   // the pass's query splits, once
+            StageTimer tm(h, ST_SIM_FACT);
+            for (int64_t q0 = 0; q0 < Bp; q0 += kPassChunk) {
+                const int64_t nb = std::min<int64_t>(kPassChunk, Bp - q0);
+                const float* x = q + (size_t)(p0 + q0) * d;
+                if (!q_on_device) {
+                    HRAG_TRY(h2d(h, h->d_q.p, x, (size_t)nb * d * 4));
+                    x = h->d_q.as<float>();
+                }
+                HRAG_TRY(split_bf16(x, nb * d, h->q_hi.as<char>() + (size_t)q0 * d * 2,
+                                    h->q_lo.as<char>() + (size_t)q0 * d * 2, h->stream));
+            }
+        }
+        float2* run_mm = fp.run_mm.as<float2>();
+        uint64_t* run_keys = fp.run_keys.as<uint64_t>();
+        int cur = 0;   // fused: the running slot (0 or 1); slot 2 takes the slice being folded in
+        auto body = [&](int64_t s, int64_t r0, int64_t ns, const void* e_hi, const void* e_lo) -> int {
+            const bool last = s == n_slices - 1;
+            for (int64_t q0 = 0; q0 < Bp; q0 += chunk) {
+                const int nb = (int)std::min<int64_t>(chunk, Bp - q0);
+                const int64_t o = p0 + q0;   // output row
+                const void* qh = q_hi + (size_t)q0 * d * 2;
+                const void* ql = q_lo + (size_t)q0 * d * 2;
+                if (fused) {
+                    const int nt = sim_tc_n_tiles(ns);
+                    {
+                        StageTimer tm(h, ST_SIM_FACT);
+                        HRAG_TRY(sim_tc(qh, ql, nb, e_hi, e_lo, ns, (int)d, n_seg, nullptr, 0, h->part_mm.as<float2>(),
+                                        h->part_keys.as<uint64_t>(), h->part_bound.as<uint64_t>(), n_ctas, h->stream));
+                    }
+                    StageTimer tm(h, ST_SEL_FACT);
+                    const float2* pmm = h->part_mm.as<float2>();
+                    const uint64_t* pkeys = h->part_keys.as<uint64_t>();
+                    if (n_slices == 1) {
+                        HRAG_TRY(merge_minmax_topk_ex(pmm, pkeys, nb, nt, nt, 1, 0, F, k, h->mm_fact.as<float2>() + q0,
+                                                      d_top_idx + o * k, d_top_score + o * k, d_nvalid + o, nullptr,
+                                                      h->stream));
+                        continue;
+                    }
+                    // this slice's 8 best (global rows) and (min, max): into the running slot for the first slice,
+                    // else into slot 2, then folded with the running slot into the other one -- or, after the
+                    // last slice, into the normalised outputs, exactly as the sharded path merges its ranks' lists
+                    const int tgt = s == 0 ? cur : 2;
+                    HRAG_TRY(merge_minmax_topk_ex(pmm, pkeys, nb, nt, nt, 1, r0, ns, kFusedK,
+                                                  run_mm + tgt * Bp + q0, nullptr, nullptr, nullptr,
+                                                  run_keys + (size_t)(tgt * Bp + q0) * 8, h->stream));
+                    if (s == 0) continue;
+                    const int nxt = 1 - cur;
+                    const float2* amm = run_mm + cur * Bp + q0;
+                    const uint64_t* akeys = run_keys + (size_t)(cur * Bp + q0) * 8;
+                    if (last)
+                        HRAG_TRY(merge_minmax_topk_ex(amm, akeys, nb, 2, 1, (2 - cur) * Bp, 0, F, k,
+                                                      h->mm_fact.as<float2>() + q0, d_top_idx + o * k,
+                                                      d_top_score + o * k, d_nvalid + o, nullptr, h->stream));
+                    else
+                        HRAG_TRY(merge_minmax_topk_ex(amm, akeys, nb, 2, 1, (2 - cur) * Bp, 0, F, kFusedK,
+                                                      run_mm + nxt * Bp + q0, nullptr, nullptr, nullptr,
+                                                      run_keys + (size_t)(nxt * Bp + q0) * 8, h->stream));
+                } else {
+                    float* Sf = h->S_fact.as<float>();
+                    {
+                        StageTimer tm(h, ST_SIM_FACT);
+                        HRAG_TRY(sim_tc(qh, ql, nb, e_hi, e_lo, ns, (int)d, n_seg, Sf, ldS, nullptr, nullptr, nullptr,
+                                        n_ctas, h->stream));
+                    }
+                    StageTimer tm(h, ST_SEL_FACT);
+                    HRAG_TRY(row_minmax_topk(Sf, nb, ns, ldS, 0, fp.sl_mm.as<float2>(), nullptr, nullptr, nullptr,
+                                             h->stream));
+                    HRAG_TRY(row_topk(Sf, nb, ns, ldS, k, fp.sl_ids.as<int>(), fp.sl_scores.as<float>(), h->stream));
+                    HRAG_TRY(fold_topk(nb, k, r0, fp.sl_ids.as<int>(), fp.sl_scores.as<float>(),
+                                       fp.sl_mm.as<float2>(), d_top_idx + o * k, d_top_score + o * k,
+                                       run_mm + q0, s == 0, h->stream));
+                }
+            }
+            if (fused && s > 0) cur = 1 - cur;
+            return 0;
+        };
+        HRAG_TRY(stream_slices(h, n_seg == 4, body));
+        if (!fused) {
+            StageTimer tm(h, ST_SEL_FACT);
+            HRAG_TRY(topk_normalize((int)Bp, k, F, run_mm, d_top_idx + p0 * k, d_top_score + p0 * k, d_nvalid + p0,
+                                    h->stream));
+        }
+    }
+    return 0;
+}
+
+// K2 writes a score tile up to its 256-column end, clipped at ldS columns from the pointer it is given.  A slice that
+// ends on a tile boundary therefore writes in place (S + its first row); a ragged last slice would spill into the
+// next row, so it goes through `tail` [nb, pad4(rows)] and a 2-D copy.
+int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ldS) {
+    HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, kNoFp32);
+    FactPlanes& fp = h->fplanes;
+    const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
+    const int64_t F = h->emb[0].rows, last_rows = F - (ceil_div(F, fp.slice_rows) - 1) * fp.slice_rows;
+    HRAG_TRY(split_queries(h, d_q, nb, h->stream));
+    if (last_rows % kSliceAlign) HRAG_TRY(fp.tail.ensure((size_t)nb * pad4(last_rows) * sizeof(float)));
+    return stream_slices(h, n_seg == 4, [&](int64_t, int64_t r0, int64_t ns, const void* e_hi, const void* e_lo) {
+        const bool ragged = ns % kSliceAlign != 0;
+        float* out = ragged ? fp.tail.as<float>() : S + r0;
+        const int64_t ld = ragged ? pad4(ns) : ldS;
+        HRAG_TRY(sim_tc(h->q_hi.p, h->q_lo.p, nb, e_hi, e_lo, ns, h->dim, n_seg, out, ld, nullptr, nullptr, nullptr,
+                        h->num_sms, h->stream));
+        if (ragged)
+            HRAG_CUDA(cudaMemcpy2DAsync(S + r0, (size_t)ldS * sizeof(float), out, (size_t)ld * sizeof(float),
+                                        (size_t)ns * sizeof(float), (size_t)nb, cudaMemcpyDeviceToDevice, h->stream));
+        return 0;
+    });
+}
+
+}  // namespace hrag
+
+using namespace hrag;
+
+extern "C" {
+
+int hrag_set_fact_memory(hrag_t* h, int64_t max_device_bytes) {
+    HRAG_CHECK(h, "hrag_set_fact_memory: null handle");
+    HRAG_CHECK(max_device_bytes >= 0, "hrag_set_fact_memory: the budget must be >= 0 bytes (0 = no limit)");
+    HRAG_CHECK(h->world == 1 || max_device_bytes == 0,
+               "hrag_set_fact_memory: fact planes in host memory serve one GPU only; a node-range-sharded handle "
+               "(world > 1) keeps its fact slice resident");
+    h->fact_budget = max_device_bytes;
+    return 0;
+}
+
+int hrag_fact_planes_info(hrag_t* h, int* on_host, int64_t* slice_rows, int64_t* device_bytes, int64_t* host_bytes) {
+    HRAG_CHECK(h && on_host && slice_rows && device_bytes && host_bytes, "hrag_fact_planes_info: null argument");
+    const FactPlanes& fp = h->fplanes;
+    *on_host = fp.held() ? 1 : 0;
+    *slice_rows = fp.slice_rows;
+    *device_bytes = fp.held() ? (int64_t)fp.ring.cap : (int64_t)(h->emb[0].hi.cap + h->emb[0].lo.cap);
+    *host_bytes = fp.held() ? 2 * (int64_t)fp.plane_bytes : 0;
+    return 0;
+}
+
+}  // extern "C"

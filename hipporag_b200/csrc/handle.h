@@ -8,6 +8,8 @@
 //             + edges src/dst int32[E], w fp64[E]: the COO list as given, mutable handles only (index_update.cu)
 //   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N]                                         (resident)
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
+//             facts over the hrag_set_fact_memory budget: the planes in pinned host memory, and on the device a
+//             ring of two slices (fact_stream.cu) of at most the budget
 //   knn       self-KNN index (knn_index.cu): bf16 hi/lo [entities, d] x 2, ids / scores [entities, pad4(kmax + 1)]
 //             (only after hrag_knn_index_update; independent of the retrieval index)
 //   state     mixed solver: x0[2], A, C, R [N, 32] fp16 in one IPC-exportable slab, and for paired solves the same
@@ -119,6 +121,29 @@ struct KnnIndex {
 };
 constexpr int kKnnComplete = 1, kKnnRefill = 2;
 
+// Fact planes held in pinned host memory (hrag_set_fact_memory with a budget below rows x dim x 4 bytes;
+// fact_stream.cu): hi / lo [rows, dim] bf16 each, byte for byte what a resident load builds, streamed through a
+// device ring of two halves, each slice_rows rows of hi then lo.  `copy` carries the ring uploads; loaded[i] marks
+// half i filled, freed[i] the last read of half i on `stream`.  Owned: freed by release().
+struct FactPlanes {
+    void *hi = nullptr, *lo = nullptr;   // pinned (cudaHostAlloc)
+    size_t plane_bytes = 0;              // of one of them
+    int64_t slice_rows = 0;              // a multiple of 256, the K2 tile width
+    Buf ring;                            // 2 halves, each hi [slice_rows, dim] then lo [slice_rows, dim] bf16
+    // a pass's per-query state: fused, (min, max) [3, B] and 8 keys [3, B, 8] (two running slots and this slice's);
+    // materialised, the running (min, max) [B] and one chunk's slice top-k sl_ids / sl_scores [chunk, k], sl_mm
+    Buf run_mm, run_keys, sl_ids, sl_scores, sl_mm;
+    Buf tail;                            // hrag_similarity's scores of a ragged last slice (fact_stream_scores)
+    cudaStream_t copy = nullptr;
+    cudaEvent_t loaded[2] = {nullptr, nullptr}, freed[2] = {nullptr, nullptr};
+    FactPlanes() = default;
+    FactPlanes(const FactPlanes&) = delete;
+    FactPlanes& operator=(const FactPlanes&) = delete;
+    ~FactPlanes() { release(); }
+    void release();
+    bool held() const { return hi != nullptr; }
+};
+
 }  // namespace hrag
 
 namespace hrag {
@@ -180,6 +205,8 @@ struct hrag_handle {
     hrag::SeedTables t;                // view of `tables`
     hrag::TableMem tables;
     hrag::EmbMem emb[2];
+    int64_t fact_budget = 0;           // hrag_set_fact_memory: device bytes the fact planes may take (0 = no limit)
+    hrag::FactPlanes fplanes;          // the fact planes in pinned host memory when they exceed fact_budget
     hrag::KnnIndex knn;                // hrag_knn_index_update: the synonymy KNN of the entities, kept between calls
     int num_sms = 132;
     int64_t fact_row_lo = 0;        // first global fact row of the local slice
@@ -222,6 +249,7 @@ struct hrag_handle {
     hrag::Buf S_fact, S_pass, mm_fact, mm_pass, mode, seed_vid, seed_w, q_hi, q_lo, part_mm, part_keys;
     hrag::Buf part_bound;                 // fused stage A: [Bq] per-query bound on the 8th best key (sim_tc's scratch)
     hrag::Buf xr_mm, xr_keys;             // fact-sharded stage A: [world, Bq] min/max and [world, Bq, 8] best keys
+    hrag::Buf fs_top_idx, fs_top_score, fs_nvalid;   // hrag_retrieve_resident on host fact planes: stage A [B, k]
     hrag::Buf d_q, d_q2, d_top_idx, d_top_score, d_nvalid, d_kept_idx, d_kept_score, d_dpr, d_out_ids, d_out_scores;
     hrag::Buf d_reset, d_scores;
     // second slot of what stream_sim hands to `stream` in hrag_retrieve_resident (slot 0: d_top_*, d_nvalid,
@@ -357,6 +385,22 @@ int compact_rows(hrag_t* h, void* base, size_t row_bytes, int64_t n_new, int64_t
                  Buf& staging);
 // out row r = base row row_src[r] (device), r < n_rows, on h->stream; row_bytes % 16 == 0.
 int gather_rows(hrag_t* h, const void* base, size_t row_bytes, const int* row_src, int64_t n_rows, void* out);
+
+// fact_stream.cu: the fact planes in pinned host memory, streamed through a device ring.
+// fact_planes_plan, before a fact load touches the handle: *slice_rows = 0 when the planes of `rows` x `dim` stay
+// resident, else the rows of one ring slice; rejects a budget below two 256-row slices, sharded handles and
+// dim % 8 != 0.  fact_planes_alloc, after reset_embeddings: the pinned planes and the ring for the handle's fact rows.
+int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows);
+int fact_planes_alloc(hrag_t* h, int64_t slice_rows);
+// Fills host plane rows [row0, row0 + n) from fp32 rows (host or device), split through the ring.
+int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool src_on_device);
+// Stage A of B queries (host or device fp32 [B, dim]) in passes of at most fact_stream_pass_cap queries, each
+// streaming the planes once: the outputs of dev_stage_a, bit for bit, for all B queries (device [B, k], [B]).
+int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* d_top_idx,
+                        float* d_top_score, int* d_nvalid);
+// Raw fact scores of nb (<= 1024) device queries into S [nb, ldS], the planes streamed once.
+int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ldS);
+int64_t fact_stream_pass_cap(const hrag_t* h);
 
 int exchange_rows(hrag_t* h, float* y, int B);
 int p2p_wait(hrag_t* h);

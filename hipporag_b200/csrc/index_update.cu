@@ -210,6 +210,8 @@ bool has_split(const hrag_t* h) { return h->dim % 8 == 0; }
 int check_updatable(hrag_t* h, const std::string& who) {
     HRAG_CHECK(h, who + ": null handle");
     HRAG_CHECK(h->world == 1, who + ": a node-range-sharded handle (world > 1) cannot be updated in place; reload it");
+    HRAG_CHECK(!h->fplanes.held(), who + ": the fact planes are held in host memory (hrag_set_fact_memory) and cannot "
+                                         "be updated in place; reload the index");
     HRAG_CHECK(h->g.cv, who + ": no graph loaded");
     HRAG_CHECK(h->mutable_index, who + ": the handle is not mutable: call hrag_set_mutable(h, 1) before the graph is "
                                        "loaded through hrag_load_graph_coo or hrag_load_graph_coo_device");
@@ -565,8 +567,10 @@ int hrag_debug_index(hrag_t* h, int plane, void* host_out, int64_t max_bytes, in
     const SeedTables& t = h->t;
     const EdgeList& E = h->graph.edges;
     const int64_t d = h->dim, F = h->emb[0].rows, P = h->emb[1].rows;
+    const bool host = h->fplanes.held();   // fact planes in pinned host memory (hrag_set_fact_memory)
     const void* src[13] = {t.passage_vid, t.fact_subj_vid, t.fact_obj_vid, t.ent_chunk_count,
-                           h->emb[0].hi.p, h->emb[0].lo.p, h->emb[1].hi.p, h->emb[1].lo.p,
+                           host ? h->fplanes.hi : h->emb[0].hi.p, host ? h->fplanes.lo : h->emb[0].lo.p,
+                           h->emb[1].hi.p, h->emb[1].lo.p,
                            h->emb[0].f32, h->emb[1].f32, E.src.p, E.dst.p, E.w.p};
     const int64_t bytes[13] = {4 * (int64_t)t.n_passages, 4 * t.n_facts, 4 * t.n_facts,
                                t.ent_chunk_count ? 4 * (int64_t)t.n_nodes : 0,
@@ -577,7 +581,7 @@ int hrag_debug_index(hrag_t* h, int plane, void* host_out, int64_t max_bytes, in
     HRAG_CHECK(*n_written <= max_bytes, "hrag_debug_index: host buffer too small");
     HRAG_CUDA(cudaSetDevice(h->device));
     HRAG_CUDA(cudaStreamSynchronize(h->stream));
-    if (*n_written) HRAG_CUDA(cudaMemcpy(host_out, src[plane], (size_t)*n_written, cudaMemcpyDeviceToHost));
+    if (*n_written) HRAG_CUDA(cudaMemcpy(host_out, src[plane], (size_t)*n_written, cudaMemcpyDefault));
     return 0;
 }
 

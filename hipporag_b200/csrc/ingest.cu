@@ -100,6 +100,7 @@ int load_graph_coo_impl(hrag_t* h, const std::string& who, int64_t n_nodes, int6
 // sharding gives rank r the fact rows [r * ceil(F / world), ...)); returns the first of them.
 int64_t reset_embeddings(hrag_t* h, int which, int64_t rows, int32_t dim) {
     h->emb[which] = EmbMem{};
+    if (which == 0) h->fplanes.release();
     h->dim = dim;
     int64_t lo = 0, hi = rows;
     if (which == 0) {
@@ -186,10 +187,20 @@ int hrag_load_embeddings(hrag_t* h, int which, int64_t rows, int32_t dim, const 
     HRAG_CHECK(rows == 0 || emb != nullptr, "hrag_load_embeddings: null embeddings");
     HRAG_CHECK(h->dim == 0 || h->dim == dim || h->emb[1 - which].rows == 0,
                "hrag_load_embeddings: fact and passage embeddings must share dim");
+    int64_t slice_rows = 0;   // > 0: the fact planes go to pinned host memory (hrag_set_fact_memory)
+    if (which == 0) HRAG_TRY(fact_planes_plan(h, "hrag_load_embeddings", rows, dim, &slice_rows));
+    HRAG_CHECK(!slice_rows || !on_device,
+               "hrag_load_embeddings: the fact planes exceed the hrag_set_fact_memory budget and go to host memory; "
+               "pass the fp32 fact rows from host memory (on the device they would take the memory the budget keeps "
+               "free)");
     HRAG_CUDA(cudaSetDevice(h->device));
     emb += (size_t)reset_embeddings(h, which, rows, dim) * dim;
     EmbMem& e = h->emb[which];
     if (e.rows == 0) return 0;
+    if (slice_rows) {   // no fp32 copy is kept, as with the streamed loader
+        HRAG_TRY(fact_planes_alloc(h, slice_rows));
+        return fact_planes_fill(h, 0, e.rows, emb, false);
+    }
     if (on_device) e.f32 = emb;   // caller keeps it alive
     else HRAG_TRY(e.own.upload(emb, (size_t)e.rows * dim, &e.f32));
     if (dim % 8 == 0) {   // bf16 hi/lo split for the tensor-core similarity kernel
@@ -207,8 +218,11 @@ int hrag_load_embeddings_begin(hrag_t* h, int which, int64_t rows, int32_t dim) 
     HRAG_CHECK(rows > 0 && dim > 0 && dim % 8 == 0, "hrag_load_embeddings_begin: rows > 0 and dim a multiple of 8");
     HRAG_CHECK(h->dim == 0 || h->dim == dim || h->emb[1 - which].rows == 0,
                "hrag_load_embeddings_begin: fact and passage embeddings must share dim");
+    int64_t slice_rows = 0;
+    if (which == 0) HRAG_TRY(fact_planes_plan(h, "hrag_load_embeddings_begin", rows, dim, &slice_rows));
     HRAG_CUDA(cudaSetDevice(h->device));
     reset_embeddings(h, which, rows, dim);
+    if (slice_rows) return fact_planes_alloc(h, slice_rows);
     const size_t n = (size_t)std::max<int64_t>(h->emb[which].rows, 1) * dim;
     HRAG_TRY(h->emb[which].hi.ensure(n * 2));
     HRAG_TRY(h->emb[which].lo.ensure(n * 2));
@@ -218,7 +232,8 @@ int hrag_load_embeddings_begin(hrag_t* h, int which, int64_t rows, int32_t dim) 
 int hrag_load_embeddings_chunk(hrag_t* h, int which, int64_t row0, int64_t n_rows, const float* emb, int on_device) {
     HRAG_CHECK(h && (which == 0 || which == 1) && emb, "hrag_load_embeddings_chunk: bad arguments");
     const EmbMem& e = h->emb[which];
-    HRAG_CHECK(e.hi.p != nullptr && e.f32 == nullptr,
+    const bool host_planes = which == 0 && h->fplanes.held();
+    HRAG_CHECK((e.hi.p != nullptr || host_planes) && e.f32 == nullptr,
                "hrag_load_embeddings_chunk: call hrag_load_embeddings_begin first");
     HRAG_CUDA(cudaSetDevice(h->device));
     const int64_t lo = which == 0 ? h->fact_row_lo : 0, hi = lo + e.rows;
@@ -228,6 +243,7 @@ int hrag_load_embeddings_chunk(hrag_t* h, int which, int64_t row0, int64_t n_row
     if (a >= b) return 0;
     const size_t n = (size_t)(b - a) * h->dim;
     const float* src = emb + (size_t)(a - row0) * h->dim;
+    if (host_planes) return fact_planes_fill(h, a, b - a, src, on_device != 0);
     if (!on_device) {
         HRAG_TRY(h->d_reset.ensure(n * sizeof(float)));                          // staging
         HRAG_CUDA(cudaMemcpyAsync(h->d_reset.p, src, n * sizeof(float), cudaMemcpyHostToDevice, h->stream));

@@ -190,6 +190,14 @@ int row_minmax_topk(const float* S, int rows, int64_t M, int64_t ld, int k, floa
 int topk_normalize(int rows, int k, int64_t M, const float2* minmax, const int* ids, float* scores, int* n_valid,
                    cudaStream_t stream);
 
+// Folds one slice of the columns into a running selection over the columns before it (fact planes streamed slice by
+// slice, fact_stream.cu): slice_ids / slice_scores [rows, k] are row_topk's output over the slice (ids local, -1 =
+// none; raw scores), slice_mm its (min, max).  run_ids / run_scores / run_mm (global ids) become the exact k best
+// (score desc, index asc) of both and the (min, max) of both; first != 0 starts the running selection from the slice
+// alone.  k <= 32; the slice's columns all follow the running ones.
+int fold_topk(int rows, int k, int64_t idx_offset, const int* slice_ids, const float* slice_scores,
+              const float2* slice_mm, int* run_ids, float* run_scores, float2* run_mm, int first, cudaStream_t stream);
+
 // In place: S[row, :M] <- min-max normalised with minmax[row] (all-equal -> 1).
 int minmax_apply(float* S, int rows, int64_t M, int64_t ld, const float2* minmax, cudaStream_t stream);
 

@@ -373,7 +373,55 @@ k_topk_normalize(int rows, int k, int64_t M, const float2* __restrict__ minmax, 
     if (j == 0) n_valid[row] = (int)((int64_t)k < M ? k : M);
 }
 
+// One thread per row: merges the running k best with a later slice's k best by rank key.  Both lists are sorted by
+// rank key, so one pass of two cursors picks the k best; an equal score resolves to the lower global row, which is
+// the running list's since every slice row follows the rows folded before it.
+constexpr int kFoldMaxK = 32;
+__global__ void __launch_bounds__(128)
+k_fold_topk(int rows, int k, uint32_t idx_offset, const int* __restrict__ slice_ids,
+            const float* __restrict__ slice_scores, const float2* __restrict__ slice_mm, int* run_ids,
+            float* run_scores, float2* run_mm, int first) {
+    const int row = blockIdx.x * 128 + threadIdx.x;
+    if (row >= rows) return;
+    const size_t base = (size_t)row * k;
+    uint64_t a[kFoldMaxK], b[kFoldMaxK];   // running, slice (0 = none)
+    for (int j = 0; j < k; ++j) {
+        const int ia = first ? -1 : run_ids[base + j];
+        const int ib = slice_ids[base + j];
+        a[j] = ia >= 0 ? rank_key(run_scores[base + j], (uint32_t)ia) : 0ull;
+        b[j] = ib >= 0 ? rank_key(slice_scores[base + j], (uint32_t)ib + idx_offset) : 0ull;
+    }
+    int i = 0, j = 0;
+    for (int o = 0; o < k; ++o) {
+        const uint64_t ka = i < k ? a[i] : 0ull, kb = j < k ? b[j] : 0ull;
+        const uint64_t pick = ka >= kb ? ka : kb;
+        if (ka >= kb) ++i; else ++j;
+        run_ids[base + o] = pick ? (int)key_index(pick) : -1;
+        run_scores[base + o] = pick ? key_score(pick) : 0.f;
+    }
+    const float2 s = slice_mm[row];
+    if (first) {
+        run_mm[row] = s;
+    } else {
+        const float2 r = run_mm[row];
+        run_mm[row] = make_float2(fminf(r.x, s.x), fmaxf(r.y, s.y));
+    }
+}
+
 }  // namespace
+
+int fold_topk(int rows, int k, int64_t idx_offset, const int* slice_ids, const float* slice_scores,
+              const float2* slice_mm, int* run_ids, float* run_scores, float2* run_mm, int first, cudaStream_t stream) {
+    HRAG_CHECK(k >= 1 && k <= kFoldMaxK, "fold_topk: k must be in [1, 32]");
+    HRAG_CHECK(idx_offset >= 0 && idx_offset < (int64_t)0xffffffff, "fold_topk: bad index offset");
+    if (rows == 0) return 0;
+    k_fold_topk<<<(unsigned)ceil_div((int64_t)rows, 128), 128, 0, stream>>>(rows, k, (uint32_t)idx_offset, slice_ids,
+                                                                            slice_scores, slice_mm, run_ids,
+                                                                            run_scores, run_mm, first);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
 
 int sort_candidates(const uint64_t* cand_keys, const int* cand_count, int rows, int cap, int kmax, int* out_ids,
                     float* out_scores, int* n_found, cudaStream_t stream) {

@@ -123,13 +123,16 @@ def _stage_b_inputs(q_pass, kept_idx, kept_score, dpr_only):
 class Engine:
     """One handle = one H100.  Not thread-safe (like the reference's ``HippoRAG`` object)."""
 
-    def __init__(self, device: int = 0, shard_mode: int = 0, mutable: bool = False):
+    def __init__(self, device: int = 0, shard_mode: int = 0, mutable: bool = False, fact_device_bytes: int = 0):
+        """``fact_device_bytes`` > 0 caps the device memory of the fact planes (``set_fact_memory``)."""
         self._lib = _lib.load()
         self._h = C.c_void_p()
         dev = (C.c_int * 1)(device)
         _lib.check(self._lib.hrag_create(dev, 1, shard_mode, C.byref(self._h)))
         if mutable:
             self.set_mutable()
+        if fact_device_bytes:
+            self.set_fact_memory(fact_device_bytes)
         self.device = device
         self.rank, self.world = 0, 1
         self.n_nodes = 0
@@ -178,6 +181,23 @@ class Engine:
         """Before ``load_graph``: keep the edge list on the device (16 bytes per edge), which ``append`` and
         ``delete`` need (``hrag_set_mutable``)."""
         _lib.check(self._lib.hrag_set_mutable(self._h, 1 if on else 0))
+
+    def set_fact_memory(self, max_device_bytes: int):
+        """Before the fact embeddings are loaded: the device bytes their bf16 hi / lo planes (rows x dim x 4 bytes) may
+        take (``hrag_set_fact_memory``; 0 = no limit).  A larger fact matrix is kept in pinned host memory and
+        streamed through a device ring of at most this many bytes (two slices of a multiple of 256 rows), with
+        results bit for bit those of resident planes.  Host planes rule out ``sim_mode=HRAG_SIM_FP32`` for the facts,
+        device fact embeddings, ``knn_threshold`` on the facts and in-place updates."""
+        _lib.check(self._lib.hrag_set_fact_memory(self._h, int(max_device_bytes)))
+
+    def fact_planes_info(self) -> dict:
+        """Where the last fact load put the planes: ``on_host``, the ring's ``slice_rows`` (0 when resident), the
+        planes' ``device_bytes`` (the ring when on the host) and the pinned ``host_bytes``."""
+        on_host, slice_rows, dev, host = C.c_int(), C.c_int64(), C.c_int64(), C.c_int64()
+        _lib.check(self._lib.hrag_fact_planes_info(self._h, C.byref(on_host), C.byref(slice_rows), C.byref(dev),
+                                                   C.byref(host)))
+        return {"on_host": int(on_host.value), "slice_rows": int(slice_rows.value), "device_bytes": int(dev.value),
+                "host_bytes": int(host.value)}
 
     def _check_device_edges(self, edge_src, edge_dst, edge_w) -> bool:
         """True for three CUDA tensors (checked, and ready to read on the library's stream), False for host arrays."""

@@ -145,6 +145,24 @@ int hrag_load_embeddings_begin(hrag_t* h, int which, int64_t rows, int32_t dim);
 int hrag_load_embeddings_chunk(hrag_t* h, int which, int64_t row0, int64_t n_rows, const float* emb,
                                int on_device);
 
+/* Device memory of the fact planes (the bf16 hi / lo planes of fact_embeddings, HippoRAG.py:1345, that stage A's
+ * similarity reads, rows x dim x 4 bytes), set before the fact embeddings are loaded and applied by every later fact
+ * load.  0 (the default) or a budget of at least the planes keeps them resident.  A smaller budget keeps them in
+ * library-owned pinned host memory, byte for byte the planes a resident load builds, and streams them through a
+ * device ring of at most max_device_bytes: two slices, each a multiple of 256 rows (a budget below two 256-row slices,
+ * 2 x 256 x dim x 4 bytes, fails the load).  Every entry then returns bit for bit what the resident planes give:
+ * hrag_stage_a streams the planes once per call (per 256 MB of bf16 query splits: 65,536 queries at dim 1024), as does
+ * the stage A of hrag_retrieve_resident, which runs for the whole call before its chunks (the get_fact_scores /
+ * rerank_facts of HippoRAG.py:459-470 for all queries); hrag_similarity / hrag_topk_similarity (which = 0) stream
+ * them once per query chunk.  With host planes: no fp32 fact rows are kept (HRAG_SIM_FP32 is unavailable for the
+ * facts, as after a streamed upload); hrag_load_embeddings rejects fact rows on the device; hrag_knn_threshold
+ * (which = 0), the update entries and sharded handles (world > 1) are rejected; h2d_bytes counts the streamed plane
+ * bytes.  A reload or hrag_destroy frees the pinned memory.  The passage planes are always resident. */
+int hrag_set_fact_memory(hrag_t* h, int64_t max_device_bytes);
+/* What the last fact load chose: on_host (1 = pinned host planes), the ring's slice_rows (0 when resident), the
+ * device bytes of the fact planes (the ring, or the resident planes) and the pinned host bytes (0 when resident). */
+int hrag_fact_planes_info(hrag_t* h, int* on_host, int64_t* slice_rows, int64_t* device_bytes, int64_t* host_bytes);
+
 /* Incremental updates of a loaded index: what HippoRAG.index() (HippoRAG.py:262-335: the stores append, igraph
  * add_vertices / add_edges, :1187, :1220) and HippoRAG.delete() (:337-411: the stores pop in place, igraph
  * delete_vertices compacts in order, :408) do to the arrays this handle mirrors, applied on the device without a

@@ -49,6 +49,13 @@ ent /= 8
 m.knn_index_update(ent, None, 0.375, 128)
 m.knn_index_update(np.concatenate([ent[3:], ent[:40]]), np.arange(3, 1500), 0.375, 128)
 m.knn_index_read()
+# fact planes in pinned host memory (fact_stream.cu): a 256-row-slice ring, fused and materialised stage A, similarity
+f = hb.B200Retriever(kg.n_nodes, src, dst, w, kg.passage_vid, kg.fact_subj_vid, kg.fact_obj_vid, kg.ent_chunk_count,
+                     fe, pe, engine=hb.Engine(0, fact_device_bytes=2 * 256 * d * 4)).engine
+f.stage_a(qf, 5)
+f.stage_a(qf, 10)
+f.similarity(0, qf[:3])
+f.topk_similarity(0, qf[:3], 40)
 print("driver ok", ids.shape)
 PY
 compute-sanitizer --tool $TOOL --error-exitcode 7 python /tmp/hrag_sanitize_driver.py 2>&1 | tail -15
