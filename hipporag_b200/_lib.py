@@ -62,6 +62,11 @@ SIGNATURES = {
     "hrag_index_reserve": (C.c_int, [_p, _i64, _i64, _i64, _i64]),
     "hrag_index_append": (C.c_int, [_p, _i64, _i64, _p, _p, _p, _i64, _p, _i64, _p, _p, _p, _i32, _p, _p, C.c_int]),
     "hrag_index_delete": (C.c_int, [_p, _i64, _p, _i64, _p, _p]),
+    "hrag_index_export": (C.c_int, [_p, _p, _i64, C.POINTER(_i64)]),
+    "hrag_index_unexport": (C.c_int, [_p]),
+    "hrag_index_attach": (C.c_int, [_p, _p, _i64]),
+    "hrag_index_detach": (C.c_int, [_p]),
+    "hrag_index_share_info": (C.c_int, [_p, C.POINTER(C.c_int), C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
     "hrag_set_options": (C.c_int, [_p, C.c_int, C.c_int, C.c_int, C.c_int]),
     "hrag_set_ppr_precision": (C.c_int, [_p, C.c_int, C.c_int, C.c_int]),
     "hrag_stage_a": (C.c_int, [_p, _i32, _p, _i32, _p, _p, _p]),

@@ -21,6 +21,8 @@ What is rebound (all paths under the reference's ``src/hipporag/``):
 * ``index`` / ``delete`` (``:262``, ``:337``) -- additionally invalidate the device state
   (``index`` forgets to clear ``ready_to_retrieve`` in the reference); with ``incremental=True`` the next prepare
   applies the change to the device in place when it is an append or an ordered delete;
+* with ``attach=`` (a blob from ``share(owner_rag)`` in another process) ``prepare_retrieval_objects`` maps the
+  owner's index on the same GPU instead of uploading one, and ``index`` / ``delete`` raise;
 * ``add_synonymy_edges`` (``:959-1020``) -- runs unchanged, but the ``retrieve_knn`` it calls
   (``utils/embed_utils.py:6-94``, imported into ``HippoRAG.py:35``) is the engine's fused
   threshold KNN for the duration of the call (``hipporag_b200/knn.py``); with ``incremental=True`` the self-KNN stays
@@ -33,7 +35,9 @@ The engine never falls back to the CPU: if the CUDA library or an H100 is missin
 """
 from __future__ import annotations
 
+import json
 import logging
+import struct
 import time
 import types
 from typing import Dict, List, Optional, Tuple
@@ -45,6 +49,45 @@ from .engine import Engine
 
 logger = logging.getLogger(__name__)
 MAX_LINKING_TOP_K = 32          # kMaxKeptFacts of the library (csrc/kernels.h)
+SHARE_MAGIC = b"hipporag_b200 share\n"
+SHARE_VERSION = 1
+
+
+def wrap_share_blob(fingerprint: dict, engine_blob: bytes) -> bytes:
+    """The blob ``share`` returns: magic, a uint32 header length, a JSON header (``SHARE_VERSION`` and the index
+    fingerprint of ``cache.fingerprint``), then the engine's ``export_index`` blob."""
+    head = json.dumps({"version": SHARE_VERSION, "fingerprint": fingerprint}, sort_keys=True).encode()
+    return SHARE_MAGIC + struct.pack("<I", len(head)) + head + bytes(engine_blob)
+
+
+def unwrap_share_blob(blob: bytes) -> Tuple[dict, bytes]:
+    """(fingerprint, engine blob) of a ``share`` blob; ValueError for anything else, another version or a
+    truncated header."""
+    blob = bytes(blob)
+    n0 = len(SHARE_MAGIC)
+    if blob[:n0] != SHARE_MAGIC or len(blob) < n0 + 4:
+        raise ValueError("not a blob written by hipporag_b200.share()")
+    (n,) = struct.unpack_from("<I", blob, n0)
+    if len(blob) < n0 + 4 + n:
+        raise ValueError("the share blob is truncated")
+    head = json.loads(blob[n0 + 4:n0 + 4 + n])
+    if head.get("version") != SHARE_VERSION:
+        raise ValueError(f"share blob version {head.get('version')}, this package reads version {SHARE_VERSION}: "
+                         "share and attach with the same build")
+    return head["fingerprint"], blob[n0 + 4 + n:]
+
+
+def share(rag) -> bytes:
+    """Owner side of one index served to several worker processes on the same GPU: after ``accelerate(rag)`` and
+    ``rag.prepare_retrieval_objects()``, export the engine's index (``Engine.export_index``) wrapped with the index
+    fingerprint.  A worker passes the blob to ``accelerate(its_rag, attach=blob)``.  This process must outlive the
+    workers.  From now on ``rag``'s engine rejects reloads: to change the index, have every worker detach
+    (``rag._b200_state["engine"].detach()`` there), call ``unexport()`` on this engine, update, and share again."""
+    state = getattr(rag, "_b200_state", None)
+    if state is None or not state.get("uploaded") or state.get("engine") is None:
+        raise HragError("share(): call accelerate(rag) and rag.prepare_retrieval_objects() first")
+    from . import cache as _cache
+    return wrap_share_blob(_cache.fingerprint(rag), state["engine"].export_index())
 
 
 def extract_tables(rag) -> dict:
@@ -173,7 +216,8 @@ def _resident_knn_applies(query_ids, key_ids, query_vecs, key_vecs, thr: float) 
 
 def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_workers: int = 1,
                filter_chunk: int = 256, ppr_tol: float = 0.0, cache: bool = True, run_ppr_fp64: bool = False,
-               incremental: bool = False, fact_device_bytes: Optional[int] = None, **engine_opts):
+               incremental: bool = False, fact_device_bytes: Optional[int] = None, attach: Optional[bytes] = None,
+               **engine_opts):
     """Rebinds the hot-path methods of ``rag`` (a reference ``HippoRAG`` instance) in place.
 
     ``filter_workers > 1`` (SURVEY.md 8(f)-1) runs the per-query recognition-memory filter calls (LLM HTTP
@@ -207,9 +251,20 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     Stage A then streams the planes once per call, so ``filter_workers > 1`` streams them once per ``filter_chunk``
     queries: give it a large ``filter_chunk``.  Host planes cannot be updated in place: with ``incremental=True``
     every ``index()`` / ``delete()`` takes the full reload.
+    ``attach`` (a blob from ``share(owner_rag)`` in a process on the same GPU): after the reference's own
+    ``prepare_retrieval_objects`` has run, the index fingerprint is checked against the owner's (a mismatch raises)
+    and the engine maps the owner's index read-only (``Engine.attach``) instead of uploading one; only the fact
+    triples the filter needs are read on the host (from the cache, else ``extract_tables``).  ``index()`` /
+    ``delete()`` then raise: the owner updates the index (see ``share``).  ``attach`` excludes ``incremental`` and
+    ``fact_device_bytes`` (ValueError).
     ``engine_opts`` go to ``Engine.set_options``.
     """
     from hipporag.utils.misc_utils import QuerySolution
+
+    if attach is not None and (incremental or fact_device_bytes is not None):
+        raise ValueError("accelerate(attach=...) serves another process's index read-only: it excludes "
+                         "incremental=True and fact_device_bytes")
+    shared = unwrap_share_blob(attach) if attach is not None else None     # (fingerprint, engine blob)
 
     state: Dict[str, object] = {"engine": engine, "facts": [], "uploaded": False}
     # calling accelerate() again on the same object re-wraps the REFERENCE's methods, not the previous wrappers
@@ -301,8 +356,27 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         state["last_update"] = kind
         state["uploaded"] = True
 
+    def prepare_attached(self):
+        from . import cache as _cache
+        fp = _cache.fingerprint(self)
+        if fp != shared[0]:
+            raise HragError("accelerate(attach=...): this HippoRAG object's index differs from the one the owner "
+                            "shared (index fingerprints differ); load the same index, or share it again")
+        eng = _engine()
+        if eng.share_info()["role"] != "attached":
+            eng.attach(shared[1])
+        wd = getattr(self, "working_dir", None) if cache else None
+        tb = _cache.load(wd, fp) if wd else None
+        state["cache_hit"] = tb is not None
+        state["facts"] = (tb if tb is not None else extract_tables(self))["facts"]
+        if engine_opts:
+            eng.set_options(**engine_opts)
+        state["uploaded"] = True
+
     def prepare_retrieval_objects(self):
         orig_prepare()
+        if shared is not None:
+            return prepare_attached(self)
         if incremental:
             return prepare_incremental(self)
         eng = _engine()
@@ -556,12 +630,20 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         order = np.lexsort((np.arange(s.shape[0]), -s))
         return order, s[order]
 
+    def _reject_update(what):
+        if shared is not None:
+            raise HragError(f"{what}: this HippoRAG object serves an index attached from another process "
+                            "(accelerate(attach=...)), which it only reads; update the index in the owner process "
+                            "(see hipporag_b200.share)")
+
     def index(self, docs):
+        _reject_update("index()")
         state["uploaded"] = False
         self.ready_to_retrieve = False
         return orig_index(docs)
 
     def delete(self, docs_to_delete):
+        _reject_update("delete()")
         state["uploaded"] = False
         return orig_delete(docs_to_delete)
 

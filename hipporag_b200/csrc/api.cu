@@ -363,6 +363,7 @@ void hrag_destroy(hrag_t* h) {
     if (h->stream_sim) cudaStreamSynchronize(h->stream_sim);
     if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
     drop_captured_solves(h);
+    index_share_destroy(h);
     for (auto e : h->pool) cudaEventDestroy(e);
     for (void* p : h->peer_slab) if (p) cudaIpcCloseMemHandle(p);
     for (cudaEvent_t e : {h->ev_ready[0], h->ev_ready[1], h->ev_released[0], h->ev_released[1], h->ev_inputs,

@@ -1,6 +1,6 @@
 // The handle behind the C ABI of libhrag_b200.so and what the host sources share: api.cu (lifecycle, options, stages
 // A/B, similarity, stats), ingest.cu (graph, tables, embeddings), graph_build.cu (the graph planes, built on the
-// device), solve.cu (the PPR solvers) and comm.cu (NCCL, peers).
+// device), solve.cu (the PPR solvers), comm.cu (NCCL, peers) and index_share.cu (one index mapped into other processes).
 //
 // HBM layout per handle (N nodes, P passages, F facts, d dims; DESIGN.md section 3):
 //   graph     row_ptr int32[n_rows+1], cv int2[nnz] {col, fp32 bits of P[i,j]}, row_order int32[n_rows]   (resident)
@@ -10,6 +10,8 @@
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
 //             facts over the hrag_set_fact_memory budget: the planes in pinned host memory, and on the device a
 //             ring of two slices (fact_stream.cu) of at most the budget
+//   shared    with hrag_index_export / hrag_index_attach the graph planes (but seg_partial), the tables and the embedding
+//             planes of an attached handle are the owner's allocations, mapped through CUDA IPC (index_share.cu)
 //   knn       self-KNN index (knn_index.cu): bf16 hi/lo [entities, d] x 2, ids / scores [entities, pad4(kmax + 1)]
 //             (only after hrag_knn_index_update; independent of the retrieval index)
 //   state     mixed solver: x0[2], A, C, R [N, 32] fp16 in one IPC-exportable slab, and for paired solves the same
@@ -61,13 +63,19 @@ inline NcclApi g_nccl;   // filled in by load_nccl (comm.cu): only sharded runs 
 // graphs of the mixed solve hold raw pointers, so they are replayed only under the generation they were captured in.
 inline std::atomic<int64_t> g_buf_generation{0};
 
-// One device allocation, owned: move-only, freed by its destructor.
+// One device allocation, owned: move-only, freed by its destructor.  An imported Buf (ipc: mapped from another
+// process by hrag_index_attach, index_share.cu) is unmapped instead of freed.
 struct Buf {
     void* p = nullptr;
     size_t cap = 0;
+    bool ipc = false;
     Buf() = default;
-    Buf(Buf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
-    Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }   // o frees ours
+    Buf(Buf&& o) noexcept
+        : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)), ipc(std::exchange(o.ipc, false)) {}
+    Buf& operator=(Buf&& o) noexcept {   // o frees ours
+        std::swap(p, o.p); std::swap(cap, o.cap); std::swap(ipc, o.ipc);
+        return *this;
+    }
     ~Buf() { reset(); }
     int ensure(size_t bytes) {    // grow-only; the contents are not kept
         if (bytes <= cap) return 0;
@@ -88,8 +96,12 @@ struct Buf {
         return 0;
     }
     void reset() {
-        if (p) { g_buf_generation += 1; cudaFree(p); }
-        p = nullptr; cap = 0;
+        if (p) {
+            g_buf_generation += 1;
+            if (ipc) cudaIpcCloseMemHandle(p);
+            else cudaFree(p);
+        }
+        p = nullptr; cap = 0; ipc = false;
     }
     template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
@@ -142,6 +154,17 @@ struct FactPlanes {
     ~FactPlanes() { release(); }
     void release();
     bool held() const { return hi != nullptr; }
+};
+
+// The read-only index shared between processes on one GPU through CUDA IPC (index_share.cu).  role 1 (owner,
+// hrag_index_export): the index stays the handle's own, `counter` is the exported attach counter.  role 2 (attached,
+// hrag_index_attach): the index Bufs are mapped from the owner (Buf::ipc), `counter` is the owner's counter, mapped.
+// shared_bytes: of the shared index allocations, the counter not included.
+enum ShareRole { SHARE_NONE = 0, SHARE_OWNER = 1, SHARE_ATTACHED = 2 };
+struct IndexShare {
+    int role = SHARE_NONE;
+    Buf counter;   // int64: attached handles
+    int64_t shared_bytes = 0;
 };
 
 }  // namespace hrag
@@ -208,6 +231,7 @@ struct hrag_handle {
     int64_t fact_budget = 0;           // hrag_set_fact_memory: device bytes the fact planes may take (0 = no limit)
     hrag::FactPlanes fplanes;          // the fact planes in pinned host memory when they exceed fact_budget
     hrag::KnnIndex knn;                // hrag_knn_index_update: the synonymy KNN of the entities, kept between calls
+    hrag::IndexShare share;            // hrag_index_export / hrag_index_attach: the index shared with other processes
     int num_sms = 132;
     int64_t fact_row_lo = 0;        // first global fact row of the local slice
     int64_t n_facts_global = 0;
@@ -401,6 +425,12 @@ int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int 
 // Raw fact scores of nb (<= 1024) device queries into S [nb, ldS], the planes streamed once.
 int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ldS);
 int64_t fact_stream_pass_cap(const hrag_t* h);
+
+// index_share.cu: status 1 with a message naming `who` when the handle's index is exported or attached (loads and
+// in-place updates would change, or free, memory other processes map); index_share_destroy is hrag_destroy's part:
+// an attached handle detaches, an owner with live attachments leaves the exported allocations mapped.
+int check_index_private(const hrag_t* h, const std::string& who);
+void index_share_destroy(hrag_t* h);
 
 int exchange_rows(hrag_t* h, float* y, int B);
 int p2p_wait(hrag_t* h);

@@ -209,6 +209,7 @@ bool has_split(const hrag_t* h) { return h->dim % 8 == 0; }
 // The preconditions every update entry shares.
 int check_updatable(hrag_t* h, const std::string& who) {
     HRAG_CHECK(h, who + ": null handle");
+    HRAG_TRY(check_index_private(h, who));
     HRAG_CHECK(h->world == 1, who + ": a node-range-sharded handle (world > 1) cannot be updated in place; reload it");
     HRAG_CHECK(!h->fplanes.held(), who + ": the fact planes are held in host memory (hrag_set_fact_memory) and cannot "
                                          "be updated in place; reload the index");

@@ -38,6 +38,7 @@ int load_graph_csr_impl(hrag_t* h, const std::string& who, int64_t n_nodes, int6
                         int64_t nnz, const int64_t* row_ptr, const int32_t* col, const float* val,
                         const double* val64) {
     HRAG_CHECK(h && row_ptr && (nnz == 0 || (col && (val || val64))), who + ": null argument");
+    HRAG_TRY(check_index_private(h, who));
     HRAG_CHECK(n_nodes > 0 && n_nodes < (int64_t)1 << 30, who + ": n_nodes out of range");
     HRAG_CHECK(nnz >= 0 && nnz < ((int64_t)1 << 31) - 8, who + ": nnz must fit int32");
     HRAG_CHECK(0 <= row_lo && row_lo <= row_hi && row_hi <= n_nodes, who + ": bad row range");
@@ -133,6 +134,7 @@ int hrag_load_graph_csr_f64(hrag_t* h, int64_t n_nodes, int64_t row_lo, int64_t 
 int hrag_load_graph_coo(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32_t* src, const int32_t* dst,
                         const double* w) {
     HRAG_CHECK(h && (n_edges == 0 || (src && dst && w)), "hrag_load_graph_coo: null argument");
+    HRAG_TRY(check_index_private(h, "hrag_load_graph_coo"));
     HRAG_CHECK(n_nodes > 0 && n_nodes < (int64_t)1 << 30 && n_edges >= 0 && n_edges < (int64_t)1 << 30,
                "hrag_load_graph_coo: sizes out of range");
     for (int64_t i = 0; i < n_edges; ++i)
@@ -150,6 +152,7 @@ int hrag_load_graph_coo(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32
 int hrag_load_graph_coo_device(hrag_t* h, int64_t n_nodes, int64_t n_edges, const int32_t* d_src,
                                const int32_t* d_dst, const double* d_w) {
     HRAG_CHECK(h && (n_edges == 0 || (d_src && d_dst && d_w)), "hrag_load_graph_coo_device: null argument");
+    HRAG_TRY(check_index_private(h, "hrag_load_graph_coo_device"));
     HRAG_CHECK(n_nodes > 0 && n_nodes < (int64_t)1 << 30 && n_edges >= 0 && n_edges < (int64_t)1 << 30,
                "hrag_load_graph_coo_device: sizes out of range");
     HRAG_CUDA(cudaSetDevice(h->device));
@@ -159,6 +162,7 @@ int hrag_load_graph_coo_device(hrag_t* h, int64_t n_nodes, int64_t n_edges, cons
 int hrag_load_tables(hrag_t* h, int64_t n_passages, const int32_t* passage_vid, int64_t n_facts,
                      const int32_t* fact_subj_vid, const int32_t* fact_obj_vid, const int32_t* ent_chunk_count) {
     HRAG_CHECK(h, "hrag_load_tables: null handle");
+    HRAG_TRY(check_index_private(h, "hrag_load_tables"));
     HRAG_CHECK(h->g.n_global > 0, "hrag_load_tables: load the graph first");
     HRAG_CHECK(n_passages >= 0 && n_passages < (int64_t)1 << 31 && n_facts >= 0, "hrag_load_tables: bad sizes");
     HRAG_CUDA(cudaSetDevice(h->device));
@@ -183,6 +187,7 @@ int hrag_load_tables(hrag_t* h, int64_t n_passages, const int32_t* passage_vid, 
 
 int hrag_load_embeddings(hrag_t* h, int which, int64_t rows, int32_t dim, const float* emb, int on_device) {
     HRAG_CHECK(h && (which == 0 || which == 1), "hrag_load_embeddings: which must be 0 (fact) or 1 (passage)");
+    HRAG_TRY(check_index_private(h, "hrag_load_embeddings"));
     HRAG_CHECK(rows >= 0 && dim > 0 && dim % 4 == 0, "hrag_load_embeddings: dim must be a positive multiple of 4");
     HRAG_CHECK(rows == 0 || emb != nullptr, "hrag_load_embeddings: null embeddings");
     HRAG_CHECK(h->dim == 0 || h->dim == dim || h->emb[1 - which].rows == 0,
@@ -215,6 +220,7 @@ int hrag_load_embeddings(hrag_t* h, int which, int64_t rows, int32_t dim, const 
 
 int hrag_load_embeddings_begin(hrag_t* h, int which, int64_t rows, int32_t dim) {
     HRAG_CHECK(h && (which == 0 || which == 1), "hrag_load_embeddings_begin: which must be 0 (fact) or 1 (passage)");
+    HRAG_TRY(check_index_private(h, "hrag_load_embeddings_begin"));
     HRAG_CHECK(rows > 0 && dim > 0 && dim % 8 == 0, "hrag_load_embeddings_begin: rows > 0 and dim a multiple of 8");
     HRAG_CHECK(h->dim == 0 || h->dim == dim || h->emb[1 - which].rows == 0,
                "hrag_load_embeddings_begin: fact and passage embeddings must share dim");
@@ -231,6 +237,7 @@ int hrag_load_embeddings_begin(hrag_t* h, int which, int64_t rows, int32_t dim) 
 
 int hrag_load_embeddings_chunk(hrag_t* h, int which, int64_t row0, int64_t n_rows, const float* emb, int on_device) {
     HRAG_CHECK(h && (which == 0 || which == 1) && emb, "hrag_load_embeddings_chunk: bad arguments");
+    HRAG_TRY(check_index_private(h, "hrag_load_embeddings_chunk"));
     const EmbMem& e = h->emb[which];
     const bool host_planes = which == 0 && h->fplanes.held();
     HRAG_CHECK((e.hi.p != nullptr || host_planes) && e.f32 == nullptr,

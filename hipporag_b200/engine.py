@@ -143,7 +143,13 @@ class Engine:
 
     # ---------------------------------------------------------------- lifecycle
     def close(self):
+        """Free the handle.  Raises ``HragError`` on an owner whose exported index is still attached by other
+        processes (their mappings would be left dangling); the handle then stays open."""
         if self._h:
+            info = self.share_info()
+            if info["role"] == "owner" and info["n_attached"] > 0:
+                raise HragError(f"close: {info['n_attached']} handle(s) in other processes are still attached to the "
+                                "exported index; they must detach first (the owner must outlive its workers)")
             self._lib.hrag_destroy(self._h)
             self._h = C.c_void_p()
 
@@ -175,6 +181,55 @@ class Engine:
         """Handles of all ranks in rank order -> fused sweep + exchange (peer stores over NVLink)."""
         blob = C.create_string_buffer(b"".join(handles), 64 * len(handles))
         _lib.check(self._lib.hrag_p2p_import(self._h, blob, len(handles)))
+
+    # ---------------------------------------------------------------- one index shared between processes
+    SHARE_ROLES = ("none", "owner", "attached")
+
+    def export_index(self) -> bytes:
+        """Export the loaded index to other processes on this GPU (``hrag_index_export``): a blob that
+        ``attach`` takes in another process, which then reads this handle's graph, tables and embeddings in place.
+        While exported, this handle serves every call as before, but its loads and updates are rejected until
+        ``unexport``."""
+        n = C.c_int64()
+        _lib.check(self._lib.hrag_index_export(self._h, None, 0, C.byref(n)))
+        buf = C.create_string_buffer(n.value)
+        _lib.check(self._lib.hrag_index_export(self._h, buf, n.value, C.byref(n)))
+        return buf.raw[:n.value]
+
+    def unexport(self):
+        """End the export (``hrag_index_unexport``); rejected while a handle is attached."""
+        _lib.check(self._lib.hrag_index_unexport(self._h))
+
+    def attach(self, blob: bytes):
+        """Serve the index another process exported (``export_index``) from this fresh handle, without a copy
+        (``hrag_index_attach``).  Loads and updates are rejected until ``detach``."""
+        blob = bytes(blob)
+        _lib.check(self._lib.hrag_index_attach(self._h, blob, len(blob)))
+        self.n_nodes = self.debug_index("ent_chunk_count", size_only=True) // 4
+        self.n_passages = self.debug_index("passage_vid", size_only=True) // 4
+        self.n_facts = self.debug_index("fact_subj_vid", size_only=True) // 4
+        self.dim = 0
+        for plane, width, rows in (("passage_hi", 2, self.n_passages), ("passage_f32", 4, self.n_passages),
+                                   ("fact_hi", 2, self.n_facts), ("fact_f32", 4, self.n_facts)):
+            size = self.debug_index(plane, size_only=True)
+            if rows and size:
+                self.dim = size // (width * rows)
+                break
+
+    def detach(self):
+        """Close the mappings of an attached handle (``hrag_index_detach``); it is then an empty handle."""
+        _lib.check(self._lib.hrag_index_detach(self._h))
+        self.n_nodes = self.n_passages = self.n_facts = self.dim = 0
+
+    def share_info(self) -> dict:
+        """``role`` ("none", "owner" or "attached"), ``n_attached`` (live attached handles), ``imported_bytes`` (the
+        shared allocations: exported by an owner, mapped by an attached handle) and ``owned_bytes`` (device memory
+        this handle allocated itself) (``hrag_index_share_info``)."""
+        role, n, imported, owned = C.c_int(), C.c_int64(), C.c_int64(), C.c_int64()
+        _lib.check(self._lib.hrag_index_share_info(self._h, C.byref(role), C.byref(n), C.byref(imported),
+                                                   C.byref(owned)))
+        return {"role": self.SHARE_ROLES[role.value], "n_attached": int(n.value), "imported_bytes": int(imported.value),
+                "owned_bytes": int(owned.value)}
 
     # ---------------------------------------------------------------- uploads
     def set_mutable(self, on: bool = True):

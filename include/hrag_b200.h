@@ -206,6 +206,45 @@ int hrag_index_append(hrag_t* h, int64_t n_new_nodes, int64_t n_new_edges, const
 int hrag_index_delete(hrag_t* h, int64_t n_del_nodes, const int32_t* del_nodes, int64_t n_del_facts,
                       const int32_t* del_facts, const int32_t* ent_chunk_count);
 
+/* One loaded index served to several processes on the same GPU through CUDA IPC (a rag_qa service runs one
+ * worker process per HippoRAG object; each would otherwise load and hold its own copy of the index).
+ *
+ * hrag_index_export (the owner: a handle with graph, tables and embeddings loaded) writes a self-describing blob of
+ * *size bytes; blob == NULL only reports *size, cap is the room at blob.  The blob begins with an 8-byte magic and a
+ * uint32 layout version, and carries the owner's device UUID and pid, the index's sizes, and one CUDA IPC handle per
+ * allocation that query code only reads: the graph planes (row_ptr, cv, row_order, the long-row segment tables,
+ * val_lo), the four seed tables, and the bf16 planes and owned fp32 rows of both embedding matrices; plus an 8-byte
+ * attach counter.  Rejected: no index loaded, fact planes in pinned host memory (hrag_set_fact_memory; that memory
+ * is this process's), world > 1, fp32 rows borrowed from the caller (device load), an attached handle.  Exporting
+ * again returns the same allocations.  While exported the owner serves every call as before, but its loads (graph,
+ * tables, embeddings, streamed embeddings) and hrag_index_append / _delete / _reserve are rejected, leaving the
+ * handle and its results unchanged.  hrag_index_unexport is rejected while a handle is attached; after it the
+ * handle is an ordinary one again (blobs exported before it no longer attach).  To update a shared index: have the
+ * workers detach, unexport, update, export again.
+ *
+ * The owner process must outlive every attached handle: freeing an allocation another process maps is undefined
+ * in CUDA, so hrag_destroy of an owner with live attachments frees everything except the exported allocations, which
+ * the process exit releases.
+ *
+ * hrag_index_attach maps the blob's allocations into a fresh handle (no index loaded, world == 1) in another process
+ * on the same physical GPU, without a copy.  Rejected: a blob of another version or size (truncated), another GPU
+ * (UUID), a handle that already holds an index, and a blob exported by the calling process (cudaIpcOpenMemHandle
+ * cannot open a handle its own process exported).  The attached handle serves every call an owner serves
+ * (stages A / B, hrag_stage_b_f64, hrag_ppr, hrag_ppr_f64, hrag_similarity, hrag_topk_similarity,
+ * hrag_knn_threshold, hrag_retrieve_resident, the debug reads, its own synonymy KNN index) with the same results;
+ * its streams, solver state, scratch, captured solves and stats are its own.  Loads and updates are rejected until
+ * hrag_index_detach, which closes the mappings and leaves an ordinary empty handle; hrag_destroy detaches too.
+ * Attached handles time-slice the GPU with the owner; they do not run concurrently.
+ *
+ * hrag_index_share_info: role (0 none, 1 owner, 2 attached), the live attach count (0 for role 0), imported_bytes
+ * = the bytes of the shared allocations (exported by an owner, mapped by an attached handle; 0 for role 0) and
+ * owned_bytes = the device bytes this handle allocated itself (an owner's include its shared allocations). */
+int hrag_index_export(hrag_t* h, void* blob, int64_t cap, int64_t* size);
+int hrag_index_unexport(hrag_t* h);
+int hrag_index_attach(hrag_t* h, const void* blob, int64_t size);
+int hrag_index_detach(hrag_t* h);
+int hrag_index_share_info(hrag_t* h, int* role, int64_t* n_attached, int64_t* imported_bytes, int64_t* owned_bytes);
+
 /* Engine knobs that are not BaseConfig fields (SURVEY.md 5).  ppr_iters > 0 pins the sweep count of the
  * fp32 solver; by default it is derived from the damping factor (see hrag_stage_b). */
 int hrag_set_options(hrag_t* h, int ppr_method, int ppr_iters, int ppr_batch, int sim_mode);
