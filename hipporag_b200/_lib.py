@@ -83,6 +83,8 @@ SIGNATURES = {
     "hrag_knn_index_read": (C.c_int, [_p, _i64, _i64, _p, _p, _p]),
     "hrag_knn_index_info": (C.c_int, [_p, C.POINTER(_i64), C.POINTER(_i32), C.POINTER(_i32)]),
     "hrag_knn_index_clear": (C.c_int, [_p]),
+    "hrag_knn_set_memory": (C.c_int, [_p, _i64]),
+    "hrag_knn_planes_info": (C.c_int, [_p, C.POINTER(C.c_int), C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
     "hrag_bench_sweep":(C.c_int, [_p, _i32, _i32, _i32, C.POINTER(_f32)]),
     "hrag_stream": (_p, [_p]),
     "hrag_get_stats": (C.c_int, [_p, C.POINTER(Stats)]),

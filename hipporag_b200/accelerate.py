@@ -217,7 +217,7 @@ def _resident_knn_applies(query_ids, key_ids, query_vecs, key_vecs, thr: float) 
 def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_workers: int = 1,
                filter_chunk: int = 256, ppr_tol: float = 0.0, cache: bool = True, run_ppr_fp64: bool = False,
                incremental: bool = False, fact_device_bytes: Optional[int] = None, attach: Optional[bytes] = None,
-               **engine_opts):
+               knn_device_bytes: Optional[int] = None, **engine_opts):
     """Rebinds the hot-path methods of ``rag`` (a reference ``HippoRAG`` instance) in place.
 
     ``filter_workers > 1`` (SURVEY.md 8(f)-1) runs the per-query recognition-memory filter calls (LLM HTTP
@@ -251,6 +251,9 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     Stage A then streams the planes once per call, so ``filter_workers > 1`` streams them once per ``filter_chunk``
     queries: give it a large ``filter_chunk``.  Host planes cannot be updated in place: with ``incremental=True``
     every ``index()`` / ``delete()`` takes the full reload.
+    ``knn_device_bytes`` (``Engine.knn_set_memory``, needs ``incremental=True``: only the resident self-KNN index uses
+    it): device memory the synonymy KNN index's planes may take; larger planes are kept in pinned host memory and
+    streamed through the GPU by every update, with the same synonymy edges and ``last_knn`` values.
     ``attach`` (a blob from ``share(owner_rag)`` in a process on the same GPU): after the reference's own
     ``prepare_retrieval_objects`` has run, the index fingerprint is checked against the owner's (a mismatch raises)
     and the engine maps the owner's index read-only (``Engine.attach``) instead of uploading one; only the fact
@@ -264,6 +267,11 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     if attach is not None and (incremental or fact_device_bytes is not None):
         raise ValueError("accelerate(attach=...) serves another process's index read-only: it excludes "
                          "incremental=True and fact_device_bytes")
+    if knn_device_bytes is not None and not incremental:
+        raise ValueError("accelerate(knn_device_bytes=...) bounds the resident synonymy KNN index, which only "
+                         "incremental=True keeps")
+    if knn_device_bytes is not None and int(knn_device_bytes) < 0:
+        raise ValueError("accelerate(knn_device_bytes=...) must be >= 0 (0 = no limit)")
     shared = unwrap_share_blob(attach) if attach is not None else None     # (fingerprint, engine blob)
 
     state: Dict[str, object] = {"engine": engine, "facts": [], "uploaded": False}
@@ -284,6 +292,8 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         state["mutable_set"] = incremental
         if fact_device_bytes is not None:     # before every load, which is what applies it
             state["engine"].set_fact_memory(fact_device_bytes)
+        if knn_device_bytes is not None:      # before every KNN index update, which is what applies it
+            state["engine"].knn_set_memory(knn_device_bytes)
         return state["engine"]
 
     def _embeddings(self):

@@ -8,6 +8,9 @@
 // per-tile lists with the slice's first row as index offset and folds the per-slice lists into a running one with the
 // same kernel the fact-sharded stage A uses across ranks (merge_minmax_topk_ex); the materialised path (k > 8, or
 // hrag_debug_keep_scores) takes each slice's exact top-k and (min, max) and folds them with fold_topk (select.cu).
+//
+// The ring walker (stream_slices, handle.h) and the fill (planes_fill) take any plane set (HostPlanes): the synonymy
+// KNN index streams its planes through them too when they exceed the hrag_knn_set_memory budget (knn_index.cu).
 #include <algorithm>
 
 #include "handle.h"
@@ -27,46 +30,24 @@ constexpr int kFusedK = 8;                           // the fused epilogue's lis
 const char* kNoFp32 = "similarity: the fact planes are held in host memory (hrag_set_fact_memory) and no fp32 copy "
                       "of the fact rows is kept; only the tensor-core modes are available";
 
-// Walks the slices of the host planes on `stream`: body(s, first row, rows, hi, lo) reads slice s from its ring half
-// while the copy stream fills the other half with slice s + 1.  `both`: stream the lo plane too (HRAG_SIM_BF16 reads
-// only hi).  Every copy is joined into `stream` before its slice is read, so the caller's later work on `stream` sees
-// the whole walk.
-template <class Body> int stream_slices(hrag_t* h, bool both, Body body) {
-    FactPlanes& fp = h->fplanes;
-    const int64_t d = h->dim, S = fp.slice_rows, F = h->emb[0].rows;
-    const int64_t n_slices = ceil_div(F, S);
-    const size_t half_bytes = (size_t)S * d * 4;
-    char* ring = fp.ring.as<char>();
-    auto copy = [&](int64_t s) -> int {
-        const int64_t r0 = s * S, n = std::min(S, F - r0);
-        const int half = (int)(s & 1);
-        char* dst = ring + half * half_bytes;
-        HRAG_CUDA(cudaStreamWaitEvent(fp.copy, fp.freed[half], 0));   // the last read of this half is done
-        HRAG_CUDA(cudaMemcpyAsync(dst, static_cast<char*>(fp.hi) + (size_t)r0 * d * 2, (size_t)n * d * 2,
-                                  cudaMemcpyHostToDevice, fp.copy));
-        if (both)
-            HRAG_CUDA(cudaMemcpyAsync(dst + (size_t)S * d * 2, static_cast<char*>(fp.lo) + (size_t)r0 * d * 2,
-                                      (size_t)n * d * 2, cudaMemcpyHostToDevice, fp.copy));
-        h->stats.h2d_bytes += (int64_t)n * d * 2 * (both ? 2 : 1);
-        HRAG_CUDA(cudaEventRecord(fp.loaded[half], fp.copy));
-        return 0;
-    };
-    for (int i = 0; i < 2; ++i) HRAG_CUDA(cudaEventRecord(fp.freed[i], h->stream));   // after the earlier reads
-    HRAG_TRY(copy(0));
-    for (int64_t s = 0; s < n_slices; ++s) {
-        if (s + 1 < n_slices) HRAG_TRY(copy(s + 1));
-        const int half = (int)(s & 1);
-        HRAG_CUDA(cudaStreamWaitEvent(h->stream, fp.loaded[half], 0));
-        const char* e_hi = ring + half * half_bytes;
-        HRAG_TRY(body(s, s * S, std::min(S, F - s * S), e_hi, e_hi + (size_t)S * d * 2));
-        HRAG_CUDA(cudaEventRecord(fp.freed[half], h->stream));
+}  // namespace
+
+int HostPlanes::alloc(size_t bytes, int64_t slice, int dim) {
+    release();
+    HRAG_CUDA(cudaHostAlloc(&hi, bytes, cudaHostAllocDefault));
+    HRAG_CUDA(cudaHostAlloc(&lo, bytes, cudaHostAllocDefault));
+    plane_bytes = bytes;
+    slice_rows = slice;
+    HRAG_TRY(ring.ensure((size_t)2 * slice * dim * 4));
+    HRAG_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
+    for (int i = 0; i < 2; ++i) {
+        HRAG_CUDA(cudaEventCreateWithFlags(&loaded[i], cudaEventDisableTiming));
+        HRAG_CUDA(cudaEventCreateWithFlags(&freed[i], cudaEventDisableTiming));
     }
     return 0;
 }
 
-}  // namespace
-
-void FactPlanes::release() {
+void HostPlanes::release() {
     if (copy) cudaStreamSynchronize(copy);
     if (hi) cudaFreeHost(hi);
     if (lo) cudaFreeHost(lo);
@@ -74,12 +55,6 @@ void FactPlanes::release() {
     plane_bytes = 0;
     slice_rows = 0;
     ring.reset();
-    run_mm.reset();
-    run_keys.reset();
-    sl_ids.reset();
-    sl_scores.reset();
-    sl_mm.reset();
-    tail.reset();
     for (int i = 0; i < 2; ++i) {
         if (loaded[i]) cudaEventDestroy(loaded[i]);
         if (freed[i]) cudaEventDestroy(freed[i]);
@@ -89,6 +64,30 @@ void FactPlanes::release() {
     copy = nullptr;
 }
 
+void FactPlanes::release() {
+    HostPlanes::release();
+    run_mm.reset();
+    run_keys.reset();
+    sl_ids.reset();
+    sl_scores.reset();
+    sl_mm.reset();
+    tail.reset();
+}
+
+int host_planes_plan(int64_t budget, const std::string& who, const char* setter, int64_t rows, int dim,
+                     int64_t* slice_rows) {
+    *slice_rows = 0;
+    const int64_t plane_bytes = rows * (int64_t)dim * 4;   // hi + lo
+    if (budget <= 0 || plane_bytes <= budget) return 0;
+    const int64_t slice = budget / (2 * (int64_t)dim * 4) / kSliceAlign * kSliceAlign;
+    HRAG_CHECK(slice >= kSliceAlign,
+               who + ": " + setter + " budget of " + std::to_string(budget) + " bytes is below the " +
+                   std::to_string(2 * kSliceAlign * dim * 4) + " bytes of a ring of two 256-row slices at dim " +
+                   std::to_string(dim));
+    *slice_rows = slice;
+    return 0;
+}
+
 int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows) {
     *slice_rows = 0;
     const int64_t plane_bytes = rows * (int64_t)dim * 4;   // hi + lo
@@ -96,39 +95,18 @@ int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int 
     HRAG_CHECK(h->world == 1, who + ": fact planes in host memory (hrag_set_fact_memory) serve one GPU only; a "
                                     "node-range-sharded handle (world > 1) keeps its fact slice resident");
     HRAG_CHECK(dim % 8 == 0, who + ": fact planes in host memory need dim % 8 == 0 (the tensor-core layout)");
-    const int64_t slice = h->fact_budget / (2 * (int64_t)dim * 4) / kSliceAlign * kSliceAlign;
-    HRAG_CHECK(slice >= kSliceAlign,
-               who + ": hrag_set_fact_memory budget of " + std::to_string(h->fact_budget) + " bytes is below the " +
-                   std::to_string(2 * kSliceAlign * dim * 4) + " bytes of a ring of two 256-row slices at dim " +
-                   std::to_string(dim));
-    *slice_rows = slice;
-    return 0;
+    return host_planes_plan(h->fact_budget, who, "hrag_set_fact_memory", rows, dim, slice_rows);
 }
 
 int fact_planes_alloc(hrag_t* h, int64_t slice_rows) {
-    FactPlanes& fp = h->fplanes;
-    fp.release();
-    const int64_t d = h->dim, F = h->emb[0].rows;
-    fp.plane_bytes = (size_t)F * d * 2;
-    HRAG_CUDA(cudaHostAlloc(&fp.hi, fp.plane_bytes, cudaHostAllocDefault));
-    HRAG_CUDA(cudaHostAlloc(&fp.lo, fp.plane_bytes, cudaHostAllocDefault));
-    fp.slice_rows = slice_rows;
-    HRAG_TRY(fp.ring.ensure((size_t)2 * slice_rows * d * 4));
-    HRAG_CUDA(cudaStreamCreateWithFlags(&fp.copy, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i) {
-        HRAG_CUDA(cudaEventCreateWithFlags(&fp.loaded[i], cudaEventDisableTiming));
-        HRAG_CUDA(cudaEventCreateWithFlags(&fp.freed[i], cudaEventDisableTiming));
-    }
-    return 0;
+    h->fplanes.release();
+    return h->fplanes.alloc((size_t)h->emb[0].rows * h->dim * 2, slice_rows, h->dim);
 }
 
-// Ring half 0 stages up to slice_rows fp32 rows (slice_rows x dim x 4 bytes: exactly one half), half 1 takes their
-// split (hi rows, then lo rows), which goes back to the pinned planes.  split_bf16 is element-wise, so the planes are
-// byte for byte those of a resident load.
-int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool src_on_device) {
-    FactPlanes& fp = h->fplanes;
-    const int64_t d = h->dim, S = fp.slice_rows;
-    char* stage = fp.ring.as<char>();
+int planes_fill(hrag_t* h, HostPlanes& ps, int dim, int64_t row0, int64_t n, const float* src, bool src_on_device,
+                const BeforeWrite& before_write) {
+    const int64_t d = dim, S = ps.slice_rows;
+    char* stage = ps.ring.as<char>();
     char* split = stage + (size_t)S * d * 4;
     for (int64_t r = 0; r < n; r += S) {
         const int64_t m = std::min(S, n - r);
@@ -139,13 +117,21 @@ int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool 
             x = reinterpret_cast<const float*>(stage);
         }
         HRAG_TRY(split_bf16(x, (int64_t)ne, split, split + (size_t)S * d * 2, h->stream));
+        if (before_write) HRAG_TRY(before_write(r, m, split, split + (size_t)S * d * 2));
         const size_t at = (size_t)(row0 + r) * d * 2;
-        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(fp.hi) + at, split, ne * 2, cudaMemcpyDeviceToHost, h->stream));
-        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(fp.lo) + at, split + (size_t)S * d * 2, ne * 2,
+        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(ps.hi) + at, split, ne * 2, cudaMemcpyDeviceToHost, h->stream));
+        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(ps.lo) + at, split + (size_t)S * d * 2, ne * 2,
                                   cudaMemcpyDeviceToHost, h->stream));
     }
     HRAG_CUDA(cudaStreamSynchronize(h->stream));
     return 0;
+}
+
+// Ring half 0 stages up to slice_rows fp32 rows (slice_rows x dim x 4 bytes: exactly one half), half 1 takes their
+// split (hi rows, then lo rows), which goes back to the pinned planes.  split_bf16 is element-wise, so the planes are
+// byte for byte those of a resident load.
+int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool src_on_device) {
+    return planes_fill(h, h->fplanes, h->dim, row0, n, src, src_on_device);
 }
 
 // Queries per pass: their bf16 hi / lo splits (dim x 4 bytes each) stay on the device for the whole pass and are
@@ -275,7 +261,7 @@ int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int 
             if (fused && s > 0) cur = 1 - cur;
             return 0;
         };
-        HRAG_TRY(stream_slices(h, n_seg == 4, body));
+        HRAG_TRY(stream_slices(h, fp, d, 0, F, n_seg == 4, body));
         if (!fused) {
             StageTimer tm(h, ST_SEL_FACT);
             HRAG_TRY(topk_normalize((int)Bp, k, F, run_mm, d_top_idx + p0 * k, d_top_score + p0 * k, d_nvalid + p0,
@@ -295,7 +281,7 @@ int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ld
     const int64_t F = h->emb[0].rows, last_rows = F - (ceil_div(F, fp.slice_rows) - 1) * fp.slice_rows;
     HRAG_TRY(split_queries(h, d_q, nb, h->stream));
     if (last_rows % kSliceAlign) HRAG_TRY(fp.tail.ensure((size_t)nb * pad4(last_rows) * sizeof(float)));
-    return stream_slices(h, n_seg == 4, [&](int64_t, int64_t r0, int64_t ns, const void* e_hi, const void* e_lo) {
+    auto body = [&](int64_t, int64_t r0, int64_t ns, const void* e_hi, const void* e_lo) -> int {
         const bool ragged = ns % kSliceAlign != 0;
         float* out = ragged ? fp.tail.as<float>() : S + r0;
         const int64_t ld = ragged ? pad4(ns) : ldS;
@@ -305,7 +291,8 @@ int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ld
             HRAG_CUDA(cudaMemcpy2DAsync(S + r0, (size_t)ldS * sizeof(float), out, (size_t)ld * sizeof(float),
                                         (size_t)ns * sizeof(float), (size_t)nb, cudaMemcpyDeviceToDevice, h->stream));
         return 0;
-    });
+    };
+    return stream_slices(h, fp, h->dim, 0, F, n_seg == 4, body);
 }
 
 }  // namespace hrag

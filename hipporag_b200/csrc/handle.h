@@ -13,7 +13,8 @@
 //   shared    with hrag_index_export / hrag_index_attach the graph planes (but seg_partial), the tables and the embedding
 //             planes of an attached handle are the owner's allocations, mapped through CUDA IPC (index_share.cu)
 //   knn       self-KNN index (knn_index.cu): bf16 hi/lo [entities, d] x 2, ids / scores [entities, pad4(kmax + 1)]
-//             (only after hrag_knn_index_update; independent of the retrieval index)
+//             (only after hrag_knn_index_update; independent of the retrieval index); planes over the
+//             hrag_knn_set_memory budget in pinned host memory, streamed through a ring of two slices as the facts'
 //   state     mixed solver: x0[2], A, C, R [N, 32] fp16 in one IPC-exportable slab, and for paired solves the same
 //             [N, 2, 32] fp16 (two sub-batches interleaved row by row); fp32 solver: V, XA, XC [N, B] fp32
 //   rhs       compact: slot_map [N] (node -> rhs slot), Vc [P + 2048, 32] fp32 (exact v) + R16 [P + 2048, 32] fp16
@@ -26,7 +27,10 @@
 #pragma once
 #include <nccl.h>
 
+#include <algorithm>
 #include <atomic>
+#include <functional>
+#include <string>
 #include <utility>
 #include <vector>
 
@@ -120,12 +124,43 @@ struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passag
     Buf own, hi, lo;              // hi / lo: bf16 split for the tensor-core path (dim % 8 == 0)
     int64_t rows = 0;             // rows held by THIS handle (node-range sharding: the rank's slice of the facts)
 };
+// bf16 hi / lo planes [rows, dim] held in pinned host memory and streamed through a device ring of two halves, each
+// slice_rows rows of hi then lo (fact_stream.cu): the fact planes over the hrag_set_fact_memory budget (FactPlanes) and
+// the synonymy KNN planes over the hrag_knn_set_memory budget (KnnIndex::host).  `copy` carries the ring uploads;
+// loaded[i] marks half i filled, freed[i] the last read of half i on `stream`.  Owned and move-only: freed by release().
+struct HostPlanes {
+    void *hi = nullptr, *lo = nullptr;   // pinned (cudaHostAlloc)
+    size_t plane_bytes = 0;              // of one of them (the capacity)
+    int64_t slice_rows = 0;              // a multiple of 256, the K2 tile width
+    Buf ring;                            // 2 halves, each hi [slice_rows, dim] then lo [slice_rows, dim] bf16
+    cudaStream_t copy = nullptr;
+    cudaEvent_t loaded[2] = {nullptr, nullptr}, freed[2] = {nullptr, nullptr};
+    HostPlanes() = default;
+    HostPlanes(HostPlanes&& o) noexcept { swap(o); }
+    HostPlanes& operator=(HostPlanes&& o) noexcept {   // o frees ours
+        swap(o);
+        return *this;
+    }
+    ~HostPlanes() { release(); }
+    void swap(HostPlanes& o) noexcept {
+        std::swap(hi, o.hi); std::swap(lo, o.lo); std::swap(plane_bytes, o.plane_bytes);
+        std::swap(slice_rows, o.slice_rows); std::swap(ring, o.ring); std::swap(copy, o.copy);
+        std::swap(loaded, o.loaded); std::swap(freed, o.freed);
+    }
+    // pinned planes of `bytes` each (contents lost), a ring of two `slice`-row halves at `dim`, the copy stream
+    int alloc(size_t bytes, int64_t slice, int dim);
+    void release();
+    bool held() const { return hi != nullptr; }
+};
+
 // The resident self-KNN index (knn_index.cu), independent of the retrieval index: the bf16 hi / lo planes of its unit
 // rows, and per row the first kmax keys with score >= thr, best first.  A list row is `width` = pad4(kmax + 1) int32
 // ids (-1 padded) / fp32 scores; ids[row * width + kmax] holds the row's flags (kKnnComplete: the list holds every key
-// >= thr).  held == false: no index (rows == 0 then too).
+// >= thr).  held == false: no index (rows == 0 then too).  Planes over the hrag_knn_set_memory budget live in `host`
+// (hi / lo then empty); the lists are always on the device.
 struct KnnIndex {
     Buf hi, lo, ids, scores;
+    HostPlanes host;
     int64_t rows = 0;
     int dim = 0, kmax = 0, width = 0;
     float thr = 0.f;
@@ -134,26 +169,17 @@ struct KnnIndex {
 constexpr int kKnnComplete = 1, kKnnRefill = 2;
 
 // Fact planes held in pinned host memory (hrag_set_fact_memory with a budget below rows x dim x 4 bytes;
-// fact_stream.cu): hi / lo [rows, dim] bf16 each, byte for byte what a resident load builds, streamed through a
-// device ring of two halves, each slice_rows rows of hi then lo.  `copy` carries the ring uploads; loaded[i] marks
-// half i filled, freed[i] the last read of half i on `stream`.  Owned: freed by release().
-struct FactPlanes {
-    void *hi = nullptr, *lo = nullptr;   // pinned (cudaHostAlloc)
-    size_t plane_bytes = 0;              // of one of them
-    int64_t slice_rows = 0;              // a multiple of 256, the K2 tile width
-    Buf ring;                            // 2 halves, each hi [slice_rows, dim] then lo [slice_rows, dim] bf16
+// fact_stream.cu): byte for byte what a resident load builds, plus the per-pass state of a streamed stage A.
+struct FactPlanes : HostPlanes {
     // a pass's per-query state: fused, (min, max) [3, B] and 8 keys [3, B, 8] (two running slots and this slice's);
     // materialised, the running (min, max) [B] and one chunk's slice top-k sl_ids / sl_scores [chunk, k], sl_mm
     Buf run_mm, run_keys, sl_ids, sl_scores, sl_mm;
     Buf tail;                            // hrag_similarity's scores of a ragged last slice (fact_stream_scores)
-    cudaStream_t copy = nullptr;
-    cudaEvent_t loaded[2] = {nullptr, nullptr}, freed[2] = {nullptr, nullptr};
     FactPlanes() = default;
     FactPlanes(const FactPlanes&) = delete;
     FactPlanes& operator=(const FactPlanes&) = delete;
     ~FactPlanes() { release(); }
     void release();
-    bool held() const { return hi != nullptr; }
 };
 
 // The read-only index shared between processes on one GPU through CUDA IPC (index_share.cu).  role 1 (owner,
@@ -231,6 +257,7 @@ struct hrag_handle {
     int64_t fact_budget = 0;           // hrag_set_fact_memory: device bytes the fact planes may take (0 = no limit)
     hrag::FactPlanes fplanes;          // the fact planes in pinned host memory when they exceed fact_budget
     hrag::KnnIndex knn;                // hrag_knn_index_update: the synonymy KNN of the entities, kept between calls
+    int64_t knn_budget = 0;            // hrag_knn_set_memory: device bytes the KNN planes may take (0 = no limit)
     hrag::IndexShare share;            // hrag_index_export / hrag_index_attach: the index shared with other processes
     int num_sms = 132;
     int64_t fact_row_lo = 0;        // first global fact row of the local slice
@@ -410,14 +437,62 @@ int compact_rows(hrag_t* h, void* base, size_t row_bytes, int64_t n_new, int64_t
 // out row r = base row row_src[r] (device), r < n_rows, on h->stream; row_bytes % 16 == 0.
 int gather_rows(hrag_t* h, const void* base, size_t row_bytes, const int* row_src, int64_t n_rows, void* out);
 
-// fact_stream.cu: the fact planes in pinned host memory, streamed through a device ring.
-// fact_planes_plan, before a fact load touches the handle: *slice_rows = 0 when the planes of `rows` x `dim` stay
-// resident, else the rows of one ring slice; rejects a budget below two 256-row slices, sharded handles and
-// dim % 8 != 0.  fact_planes_alloc, after reset_embeddings: the pinned planes and the ring for the handle's fact rows.
+// fact_stream.cu: planes in pinned host memory, streamed through a device ring.
+// host_planes_plan: *slice_rows = 0 when the planes of `rows` x `dim` fit `budget` (0 = no limit), else the rows of
+// one ring slice, the largest multiple of 256 of which two fit the budget; a budget below two 256-row slices is
+// rejected with a message naming `who` and the entry that set the budget, `setter`.
+int host_planes_plan(int64_t budget, const std::string& who, const char* setter, int64_t rows, int dim,
+                     int64_t* slice_rows);
+// fact_planes_plan, before a fact load touches the handle: host_planes_plan of the fact budget; rejects sharded
+// handles and dim % 8 != 0.  fact_planes_alloc, after reset_embeddings: the pinned planes and the ring for the
+// handle's fact rows.
 int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows);
 int fact_planes_alloc(hrag_t* h, int64_t slice_rows);
-// Fills host plane rows [row0, row0 + n) from fp32 rows (host or device), split through the ring.
+// Fills host plane rows [row0, row0 + n) of `ps` (dim wide) from fp32 rows (host or device): ring half 0 stages up to
+// slice_rows fp32 rows, half 1 takes their split, which goes back to the pinned planes.  before_write(r, m, hi, lo),
+// when given, runs on `stream` after rows [row0 + r, row0 + r + m) are split into hi / lo (ring half 1) and before they
+// are written back; half 0 is free then.  Returns once the rows are written.
+using BeforeWrite = std::function<int(int64_t r, int64_t m, const char* hi, const char* lo)>;
+int planes_fill(hrag_t* h, HostPlanes& ps, int dim, int64_t row0, int64_t n, const float* src, bool src_on_device,
+                const BeforeWrite& before_write = nullptr);
 int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool src_on_device);
+// Walks rows [row0, row1) of the host planes `ps` (dim wide) on `stream`, in slices of slice_rows from row0:
+// body(s, first row, rows, hi, lo) reads slice s from its ring half while the copy stream fills the other half with
+// slice s + 1.  `both`: stream the lo plane too (HRAG_SIM_BF16 reads only hi).  Every copy is joined into `stream`
+// before its slice is read, so the caller's later work on `stream` sees the whole walk.
+template <class Body>
+int stream_slices(hrag_t* h, HostPlanes& ps, int64_t dim, int64_t row0, int64_t row1, bool both, Body body) {
+    const int64_t S = ps.slice_rows, n_slices = ceil_div(row1 - row0, S);
+    const size_t half_bytes = (size_t)S * dim * 4;
+    char* ring = ps.ring.as<char>();
+    auto copy = [&](int64_t s) -> int {
+        const int64_t r0 = row0 + s * S, n = std::min(S, row1 - r0);
+        const int half = (int)(s & 1);
+        char* dst = ring + half * half_bytes;
+        HRAG_CUDA(cudaStreamWaitEvent(ps.copy, ps.freed[half], 0));   // the last read of this half is done
+        HRAG_CUDA(cudaMemcpyAsync(dst, static_cast<char*>(ps.hi) + (size_t)r0 * dim * 2, (size_t)n * dim * 2,
+                                  cudaMemcpyHostToDevice, ps.copy));
+        if (both)
+            HRAG_CUDA(cudaMemcpyAsync(dst + (size_t)S * dim * 2, static_cast<char*>(ps.lo) + (size_t)r0 * dim * 2,
+                                      (size_t)n * dim * 2, cudaMemcpyHostToDevice, ps.copy));
+        h->stats.h2d_bytes += (int64_t)n * dim * 2 * (both ? 2 : 1);
+        HRAG_CUDA(cudaEventRecord(ps.loaded[half], ps.copy));
+        return 0;
+    };
+    if (n_slices <= 0) return 0;
+    for (int i = 0; i < 2; ++i) HRAG_CUDA(cudaEventRecord(ps.freed[i], h->stream));   // after the earlier reads
+    HRAG_TRY(copy(0));
+    for (int64_t s = 0; s < n_slices; ++s) {
+        if (s + 1 < n_slices) HRAG_TRY(copy(s + 1));
+        const int half = (int)(s & 1);
+        HRAG_CUDA(cudaStreamWaitEvent(h->stream, ps.loaded[half], 0));
+        const char* e_hi = ring + half * half_bytes;
+        const int64_t r0 = row0 + s * S;
+        HRAG_TRY(body(s, r0, std::min(S, row1 - r0), e_hi, e_hi + (size_t)S * dim * 2));
+        HRAG_CUDA(cudaEventRecord(ps.freed[half], h->stream));
+    }
+    return 0;
+}
 // Stage A of B queries (host or device fp32 [B, dim]) in passes of at most fact_stream_pass_cap queries, each
 // streaming the planes once: the outputs of dev_stage_a, bit for bit, for all B queries (device [B, k], [B]).
 int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* d_top_idx,

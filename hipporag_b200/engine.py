@@ -602,6 +602,23 @@ class Engine:
         """Drop the resident self-KNN index and free its memory."""
         _lib.check(self._lib.hrag_knn_index_clear(self._h))
 
+    def knn_set_memory(self, max_device_bytes: int):
+        """The device bytes the self-KNN index's bf16 hi / lo planes (rows x dim x 4 bytes) may take
+        (``hrag_knn_set_memory``; 0 = no limit), applied by the next ``knn_index_update``.  Larger planes are kept in
+        pinned host memory and streamed through a device ring of at most this many bytes (two slices of a multiple of
+        256 rows); the lists stay on the device and are bit for bit those of device planes.  When an update's rows
+        cross the budget, or the budget changed, the planes move with one copy."""
+        _lib.check(self._lib.hrag_knn_set_memory(self._h, int(max_device_bytes)))
+
+    def knn_planes_info(self) -> dict:
+        """Where the self-KNN index's planes are: ``on_host``, the ring's ``slice_rows`` (0 on the device), the planes'
+        ``device_bytes`` (the ring when on the host) and the pinned ``host_bytes``."""
+        on_host, slice_rows, dev, host = C.c_int(), C.c_int64(), C.c_int64(), C.c_int64()
+        _lib.check(self._lib.hrag_knn_planes_info(self._h, C.byref(on_host), C.byref(slice_rows), C.byref(dev),
+                                                  C.byref(host)))
+        return {"on_host": int(on_host.value), "slice_rows": int(slice_rows.value), "device_bytes": int(dev.value),
+                "host_bytes": int(host.value)}
+
     def bench_sweep(self, batch: int, sweeps: int = 20, method: int = PPR_POWER) -> float:
         ms = C.c_float()
         _lib.check(self._lib.hrag_bench_sweep(self._h, batch, sweeps, method, C.byref(ms)))

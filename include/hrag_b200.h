@@ -359,9 +359,25 @@ int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float mi
  * index held, or a changed min_score, kmax (in [1, 512]) or dim builds from scratch.  *mode: 0 built, 1 updated, 2
  * unchanged (no GEMM ran).  Every argument is checked before the index is touched (a rejected call leaves it as it
  * was); a failure after that (out of memory) clears it.  Rejected on a node-range-sharded handle (world > 1).  Device
- * memory: 4 dim + 8 pad4(kmax + 1) bytes per row, capacity grown by half at a time. */
+ * memory: 4 dim + 8 pad4(kmax + 1) bytes per row, capacity grown by half at a time (the planes' share bounded by
+ * hrag_knn_set_memory). */
 int hrag_knn_index_update(hrag_t* h, int64_t rows, int32_t dim, const float* emb, int on_device, int64_t n_kept,
                           const int64_t* kept_from, float min_score, int32_t kmax, int32_t* mode);
+/* Device memory of the index's bf16 hi / lo planes (rows x dim x 4 bytes), applied by every later
+ * hrag_knn_index_update.  0 (the default) or a budget of at least the planes keeps them on the device as above.  A
+ * smaller budget keeps them in library-owned pinned host memory and streams them through a device ring of two halves,
+ * each a multiple of 256 rows, within the budget; an update then stages its query rows on the device in passes of up
+ * to 65,536 rows and streams the keys once per pass.  The lists (8 pad4(kmax + 1) bytes per row) stay on the device and
+ * every list is bit for bit what resident planes give.  Placement follows the rows of each update: when they cross the
+ * budget, in either direction, or the budget changed, the planes move with one copy and the lists are kept.  An update
+ * whose planes would need a ring below two 256-row slices (2 x 256 x dim x 4 bytes) is rejected, leaving the index as
+ * it was.  There is no automatic mode: free device memory on a shared GPU would pick another placement from run to
+ * run.  A non-zero budget is rejected on a node-range-sharded handle (world > 1). */
+int hrag_knn_set_memory(hrag_t* h, int64_t max_device_bytes);
+/* Where the index's planes are: on_host (1 = pinned host planes), the ring's slice_rows (0 when on the device), the
+ * device bytes of the planes (the ring, or the planes' capacity) and the pinned host bytes (capacity; 0 on the
+ * device). */
+int hrag_knn_planes_info(hrag_t* h, int* on_host, int64_t* slice_rows, int64_t* device_bytes, int64_t* host_bytes);
 /* Rows [row0, row0 + n) of the index: ids / scores [n, kmax] (host, -1 / 0 padded), n_valid[n] (may be NULL). */
 int hrag_knn_index_read(hrag_t* h, int64_t row0, int64_t n, int32_t* ids, float* scores, int32_t* n_valid);
 /* What the index holds: *rows, *dim and *kmax (all 0 when no index is held). */
