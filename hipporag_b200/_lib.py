@@ -27,7 +27,7 @@ class Stats(C.Structure):
         ("ms_seed", C.c_double), ("ms_ppr", C.c_double), ("ms_topk", C.c_double), ("ms_comm", C.c_double),
         ("ppr_sweeps", C.c_int64), ("ppr_columns", C.c_int64), ("kernel_launches", C.c_int64),
         ("h2d_bytes", C.c_int64), ("d2h_bytes", C.c_int64),
-        ("ppr_residual", C.c_double), ("ppr_error_bound", C.c_double),
+        ("ppr_residual", C.c_double), ("ppr_error_bound", C.c_double), ("stage_a_fallbacks", C.c_int64),
     ]
 
     def as_dict(self):
@@ -92,6 +92,8 @@ SIGNATURES = {
     "hrag_debug_keep_scores": (C.c_int, [_p, C.c_int]),
     "hrag_debug_sim_ctas": (C.c_int, [_p, C.c_int]),
     "hrag_debug_dense_first_sweep": (C.c_int, [_p, C.c_int]),
+    "hrag_debug_exact_stage_a": (C.c_int, [_p, C.c_int]),
+    "hrag_debug_fact_minmax": (C.c_int, [_p, _p, _i64, C.POINTER(_i64)]),
     "hrag_debug_copy": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
     "hrag_debug_graph": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),
     "hrag_debug_index": (C.c_int, [_p, C.c_int, _p, _i64, C.POINTER(_i64)]),

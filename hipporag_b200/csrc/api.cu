@@ -52,6 +52,106 @@ int64_t chunk_b(hrag_t* h) {
     return std::max<int64_t>(1, std::min<int64_t>(c, 1024));
 }
 
+int fact_norms_update(hrag_t* h, int64_t row0, int64_t n, bool reset) {
+    EmbMem& e = h->emb[0];
+    if (e.hi.p == nullptr) return 0;
+    const bool fresh = e.nmax.p == nullptr;
+    HRAG_TRY(e.nmax.ensure(2 * sizeof(float)));
+    if (reset || fresh) HRAG_CUDA(cudaMemsetAsync(e.nmax.p, 0, 2 * sizeof(float), h->stream));
+    return plane_norm_max(static_cast<const char*>(e.hi.p) + (size_t)row0 * h->dim * 2,
+                          static_cast<const char*>(e.lo.p) + (size_t)row0 * h->dim * 2, n, h->dim,
+                          e.nmax.as<unsigned int>(), h->stream);
+}
+
+// The stage-A screen replaces the split K2 over all facts on one GPU with resident planes (DESIGN.md section 4, K2).
+// Below 65,536 facts the split K2 takes a fraction of a millisecond per chunk and the screen's dozen extra launches
+// cost more than they save (MuSiQue-1k, 10,734 facts: 0.9 against 0.7 ms per 64-query step).
+constexpr int64_t kScreenMinFacts = 65536;
+static bool screened(const hrag_t* h) {
+    return h->world == 1 && h->sim_mode == HRAG_SIM_BF16X3 && !h->debug_exact_stage_a && h->emb[0].hi.p != nullptr &&
+           h->emb[0].nmax.p != nullptr && h->emb[0].rows >= kScreenMinFacts;
+}
+
+// Stage A of Bq <= 1024 queries (split into q_hi / q_lo) by the screen: hi.hi over all facts with the screen epilogue,
+// the candidates of each query (screen_select), their rows staged per 128-query m-tile at column f mod 256, the split
+// K2 over the staged tiles and the exact selection over them.  Every score the selection reads is the one the split K2
+// gives over all facts, bit for bit (same query row, same column, same k sequence), and the candidates hold the k best
+// and the minimum, so the outputs are those of the exact path.  When the screen cannot prove that (a non-finite bound,
+// a cap overflowed, or a rescored score outside the bound) it raises scr.flag, and the gated exact path below reruns
+// the chunk and counts it.
+static int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, float* d_top_score,
+                            int* d_nvalid, cudaStream_t s, int n_ctas) {
+    const int64_t F = h->emb[0].rows;
+    const int nt = sim_tc_n_tiles(F), mtiles = (int)ceil_div(Bq, 128), ST = kScreenStageTiles;
+    auto& c = h->scr;
+    HRAG_TRY(h->part_mm.ensure((size_t)Bq * nt * sizeof(float2)));
+    HRAG_TRY(h->part_keys.ensure((size_t)Bq * nt * 8 * sizeof(uint64_t)));
+    HRAG_TRY(h->part_bound.ensure((size_t)Bq * sizeof(uint64_t)));
+    HRAG_TRY(c.err.ensure((size_t)Bq * sizeof(float)));
+    HRAG_TRY(c.part_low.ensure((size_t)Bq * nt * sizeof(uint4)));
+    HRAG_TRY(c.cand_ids.ensure((size_t)Bq * kScreenCandidates * sizeof(int)));
+    HRAG_TRY(c.cand_s1.ensure((size_t)Bq * kScreenCandidates * sizeof(float)));
+    HRAG_TRY(c.cand_n.ensure((size_t)Bq * sizeof(int)));
+    HRAG_TRY(c.sat.ensure((size_t)Bq * kScreenSatTiles * sizeof(int)));
+    HRAG_TRY(c.sat_n.ensure((size_t)Bq * sizeof(int)));
+    HRAG_TRY(c.pos_of.ensure((size_t)mtiles * F * sizeof(int)));
+    HRAG_TRY(c.slot_ids.ensure((size_t)mtiles * ST * 256 * sizeof(int)));
+    HRAG_TRY(c.res_count.ensure((size_t)mtiles * 256 * sizeof(int)));
+    HRAG_TRY(c.stage_count.ensure((size_t)mtiles * sizeof(int)));
+    HRAG_TRY(c.st_hi.ensure((size_t)mtiles * ST * 256 * h->dim * 2));
+    HRAG_TRY(c.st_lo.ensure((size_t)mtiles * ST * 256 * h->dim * 2));
+    HRAG_TRY(c.st_S.ensure((size_t)Bq * ST * 256 * sizeof(float)));
+    HRAG_TRY(c.flag.ensure(sizeof(int)));
+    if (c.fallbacks.p == nullptr) HRAG_TRY(c.fallbacks.zeros(sizeof(unsigned long long)));
+    int* flag = c.flag.as<int>();
+    const EmbMem& e = h->emb[0];
+    const int dim = h->dim;
+    {
+        StageTimer tm(h, ST_SIM_FACT, s);
+        HRAG_TRY(split_queries(h, d_qf, Bq, s));
+        HRAG_TRY(query_err(h->q_hi.p, h->q_lo.p, Bq, dim, e.nmax.as<unsigned int>(), c.err.as<float>(), s));
+        HRAG_TRY(sim_tc_screen(h->q_hi.p, Bq, e.hi.p, F, dim, c.err.as<float>(), h->part_keys.as<uint64_t>(),
+                               c.part_low.as<uint4>(), h->part_bound.as<uint64_t>(), n_ctas, s));
+    }
+    {
+        StageTimer tm(h, ST_SEL_FACT, s);
+        HRAG_CUDA(cudaMemsetAsync(flag, 0, sizeof(int), s));
+        HRAG_CUDA(cudaMemsetAsync(c.pos_of.p, 0xff, (size_t)mtiles * F * sizeof(int), s));
+        HRAG_CUDA(cudaMemsetAsync(c.slot_ids.p, 0xff, (size_t)mtiles * ST * 256 * sizeof(int), s));
+        HRAG_CUDA(cudaMemsetAsync(c.res_count.p, 0, (size_t)mtiles * 256 * sizeof(int), s));
+        HRAG_CUDA(cudaMemsetAsync(c.stage_count.p, 0, (size_t)mtiles * sizeof(int), s));
+        HRAG_TRY(screen_select(h->part_keys.as<uint64_t>(), c.part_low.as<uint4>(), Bq, nt, c.err.as<float>(),
+                               c.cand_ids.as<int>(), c.cand_s1.as<float>(), c.cand_n.as<int>(), c.sat.as<int>(),
+                               c.sat_n.as<int>(), flag, s));
+        HRAG_TRY(screen_stage(c.cand_ids.as<int>(), c.cand_n.as<int>(), c.sat.as<int>(), c.sat_n.as<int>(), Bq, F, ST,
+                              c.pos_of.as<int>(), c.slot_ids.as<int>(), c.res_count.as<int>(), c.stage_count.as<int>(),
+                              flag, s));
+        HRAG_TRY(screen_gather(c.slot_ids.as<int>(), c.stage_count.as<int>(), mtiles, ST, e.hi.p, e.lo.p, dim,
+                               c.st_hi.p, c.st_lo.p, s));
+    }
+    {
+        StageTimer tm(h, ST_SIM_FACT, s);
+        HRAG_TRY(sim_tc_staged(h->q_hi.p, h->q_lo.p, Bq, c.st_hi.p, c.st_lo.p, ST, c.stage_count.as<int>(), dim,
+                               c.st_S.as<float>(), n_ctas, s));
+    }
+    {
+        StageTimer tm(h, ST_SEL_FACT, s);
+        HRAG_TRY(screen_finish(c.st_S.as<float>(), Bq, ST, c.slot_ids.as<int>(), c.stage_count.as<int>(),
+                               c.pos_of.as<int>(), F, c.cand_ids.as<int>(), c.cand_s1.as<float>(), c.cand_n.as<int>(),
+                               c.err.as<float>(), k, h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, flag, s));
+    }
+    // the exact path, run only when the flag is up (kernels that find it down return at once)
+    {
+        StageTimer tm(h, ST_SIM_FACT, s);
+        HRAG_TRY(sim_tc(h->q_hi.p, h->q_lo.p, Bq, e.hi.p, e.lo.p, F, dim, 4, nullptr, 0, h->part_mm.as<float2>(),
+                        h->part_keys.as<uint64_t>(), h->part_bound.as<uint64_t>(), n_ctas, s, flag));
+    }
+    StageTimer tm(h, ST_SEL_FACT, s);
+    return merge_minmax_topk_gated(h->part_mm.as<float2>(), h->part_keys.as<uint64_t>(), Bq, nt, F, k,
+                                   h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, flag,
+                                   c.fallbacks.as<unsigned long long>(), s);
+}
+
 // Stage A on device pointers, Bq <= chunk_a, on stream s (h->stream when world > 1: the all-gathers run there).
 int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, float* d_top_score, int* d_nvalid,
                 cudaStream_t s, int n_ctas) {
@@ -64,6 +164,12 @@ int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, flo
     }
     const int64_t ld = pad4(F);
     HRAG_TRY(h->mm_fact.ensure((size_t)Bq * sizeof(float2)));
+    h->last_mm_rows = Bq;
+    if (fused_stage_a(h, k) && screened(h)) {
+        HRAG_TRY(screened_stage_a(h, Bq, d_qf, k, d_top_idx, d_top_score, d_nvalid, s, n_ctas));
+        h->last_fact_rows = 0;
+        return 0;
+    }
     if (fused_stage_a(h, k)) {
         const int nt = sim_tc_n_tiles(F);
         HRAG_TRY(h->part_mm.ensure((size_t)Bq * nt * sizeof(float2)));
@@ -247,16 +353,24 @@ int dev_stage_b_solve_f64(hrag_t* h, int Bq, const float* S, const float2* mm_pa
 // (non-zeros x 32-column sweeps per sub-batch x sub-batches).  Rates measured at C3 inside the overlapped step, with
 // paired sweeps and the bound-gated K2 epilogue, on an H100 SXM (132 SMs, 700 W) at G = 40: a paired sweep 0.381 ms
 // per 32 columns (38.0 G non-zeros/s); K2 2.49 TFLOP/s per SM, 0.73 of its rate alone (3.43), as its TMA operand
-// loads queue behind the sweeps' gathers.  DESIGN.md section 4 K2 has the scan of G.
+// loads queue behind the sweeps' gathers.  The stage-A screen (one hi.hi product over the facts; its rescore counted
+// as the split product over at most kScreenStageTiles staged tiles) reads twice the operand bytes per FLOP and
+// suffers more next to the sweeps: 0.76 TFLOP/s per SM in the C3 step at G = 37, where the sweeps took 0.345 ms per 32
+// columns (42 G non-zeros/s).  Its rate here is 0.66, 13 % below that: a G below the optimum costs far more than one
+// above it (C3 scan: G = 28 +121 ms per step, G = 44 +5 ms).  DESIGN.md section 4 K2 has the scans of G.
 int overlap_ctas(const hrag_t* h, int Bq, const SweepPlan& plan) {
-    constexpr double kGemmFlopPerSmMs = 2.49e9, kSweepNnzPerMs = 3.80e7;
+    constexpr double kGemmFlopPerSmMs = 2.49e9, kScreenFlopPerSmMs = 0.66e9;
+    const bool screen = screened(h);
+    const double kSweepNnzPerMs = screen ? 4.20e7 : 3.80e7;
     const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
     const int64_t fact_rows = h->fplanes.held() ? 0 : h->emb[0].rows;   // streamed planes: stage A ran up front
-    const double gemm_flop = 2.0 * n_seg * Bq * (double)(fact_rows + h->emb[1].rows) * h->dim;
+    const double split_cols = (screen ? (double)kScreenStageTiles * 256 : (double)fact_rows) + (double)h->emb[1].rows;
+    const double t_gemm = 2.0 * n_seg * Bq * split_cols * h->dim / kGemmFlopPerSmMs +
+                          (screen ? 2.0 * Bq * (double)fact_rows * h->dim / kScreenFlopPerSmMs : 0.0);
     const int64_t sweeps = plan.mixed ? (int64_t)(plan.m1 + 1 + plan.m2) * ceil_div(Bq, 32)
                                       : (int64_t)plan.iters * ceil_div(Bq, round_batch(std::min(h->ppr_batch, Bq)));
     const double t_sweep = (double)sweeps * (double)h->g.nnz / kSweepNnzPerMs;
-    const int g = (int)std::ceil(gemm_flop / (kGemmFlopPerSmMs * std::max(t_sweep, 1e-9)));
+    const int g = (int)std::ceil(t_gemm / std::max(t_sweep, 1e-9));
     return std::min(std::max(g, 1), h->num_sms / 2);
 }
 
@@ -704,6 +818,23 @@ int hrag_debug_sim_ctas(hrag_t* h, int n) {
 int hrag_debug_dense_first_sweep(hrag_t* h, int on) {
     HRAG_CHECK(h, "hrag_debug_dense_first_sweep: null handle");
     h->debug_dense_first_sweep = on != 0;
+    return 0;
+}
+
+int hrag_debug_exact_stage_a(hrag_t* h, int on) {
+    HRAG_CHECK(h, "hrag_debug_exact_stage_a: null handle");
+    h->debug_exact_stage_a = on != 0;
+    return 0;
+}
+
+int hrag_debug_fact_minmax(hrag_t* h, float* host_out, int64_t max_rows, int64_t* n_rows) {
+    HRAG_CHECK(h && host_out && n_rows, "hrag_debug_fact_minmax: null argument");
+    HRAG_CHECK(h->last_mm_rows <= max_rows, "hrag_debug_fact_minmax: host buffer too small");
+    HRAG_CUDA(cudaSetDevice(h->device));
+    HRAG_CUDA(cudaStreamSynchronize(h->stream));
+    if (h->last_mm_rows)
+        HRAG_CUDA(cudaMemcpy(host_out, h->mm_fact.p, (size_t)h->last_mm_rows * sizeof(float2), cudaMemcpyDeviceToHost));
+    *n_rows = h->last_mm_rows;
     return 0;
 }
 

@@ -147,6 +147,7 @@ int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int 
     FactPlanes& fp = h->fplanes;
     HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, std::string("stage A ") + kNoFp32);
     h->last_fact_rows = 0;
+    h->last_mm_rows = 0;
     if (B == 0) return 0;
     const int64_t F = h->emb[0].rows, d = h->dim, S = fp.slice_rows;
     const int64_t n_slices = ceil_div(F, S);

@@ -122,6 +122,8 @@ struct TableMem { Buf passage_vid, fact_subj_vid, fact_obj_vid, ent_chunk_count;
 struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passages)
     const float* f32 = nullptr;   // fp32 rows: borrowed from the caller (device upload, caller keeps it alive) or own
     Buf own, hi, lo;              // hi / lo: bf16 split for the tensor-core path (dim % 8 == 0)
+    Buf nmax;                     // facts: float [2], upper bounds on the largest row norm of hi / lo (only grow;
+                                  // the stage-A screen's bound, fact_norms_update)
     int64_t rows = 0;             // rows held by THIS handle (node-range sharding: the rank's slice of the facts)
 };
 // bf16 hi / lo planes [rows, dim] held in pinned host memory and streamed through a device ring of two halves, each
@@ -271,6 +273,7 @@ struct hrag_handle {
     bool keep_fact_scores = false;   // debugging: materialise S_fact even in tensor-core modes
     int debug_sim_ctas = 0;          // hrag_debug_sim_ctas: > 0 GEMM CTAs, < 0 no chunk overlap, 0 defaults
     bool debug_dense_first_sweep = false;   // hrag_debug_dense_first_sweep: stage B builds the dense first iterate
+    bool debug_exact_stage_a = false;       // hrag_debug_exact_stage_a: stage A runs the split K2 over all facts
     int ppr_precision = HRAG_PPR_MIXED;   // applies to batches of > 16 queries; smaller ones run fp32
     int mixed_m1 = 0, mixed_m2 = 0;   // 0 = derived from damping (8 / 7 at damping 0.5)
     double check_tol = 0.0, check_kappa = 0.0;   // > 0: this call's mixed solves are verified in resolve_spans
@@ -300,6 +303,16 @@ struct hrag_handle {
     hrag::Buf S_fact, S_pass, mm_fact, mm_pass, mode, seed_vid, seed_w, q_hi, q_lo, part_mm, part_keys;
     hrag::Buf part_bound;                 // fused stage A: [Bq] per-query bound on the 8th best key (sim_tc's scratch)
     hrag::Buf xr_mm, xr_keys;             // fact-sharded stage A: [world, Bq] min/max and [world, Bq, 8] best keys
+    // the stage-A screen (api.cu screened_stage_a): per query err [Bq], the s1 tile lows part_low [Bq, n_tiles] (its
+    // keys in part_keys), candidates cand_ids / cand_s1 [Bq, 256], cand_n, saturated tiles sat [Bq, 8], sat_n; per
+    // m-tile pos_of [m, F], slot_ids [m, 48, 256], res_count [m, 256], stage_count [m], the staging planes st_hi / st_lo
+    // [m * 48 * 256, d] and the rescored scores st_S [Bq, 48 * 256]; flag: this chunk falls back; fallbacks: counted
+    // on the device, drained into stats by resolve_spans.  About 0.6 GB at C3 (F = 2.75 M, d = 768), on top of the
+    // fused buffers and outside the hrag_set_fact_memory budget
+    struct {
+        hrag::Buf err, part_low, cand_ids, cand_s1, cand_n, sat, sat_n, pos_of, slot_ids, res_count, stage_count,
+            st_hi, st_lo, st_S, flag, fallbacks;
+    } scr;
     hrag::Buf fs_top_idx, fs_top_score, fs_nvalid;   // hrag_retrieve_resident on host fact planes: stage A [B, k]
     hrag::Buf d_q, d_q2, d_top_idx, d_top_score, d_nvalid, d_kept_idx, d_kept_score, d_dpr, d_out_ids, d_out_scores;
     hrag::Buf d_reset, d_scores;
@@ -327,6 +340,7 @@ struct hrag_handle {
     // sim_ready[s]: slot s holds a chunk's stage A and passage scores; sim_consumed[s]: its solves and top-k are done
     cudaEvent_t ev_sim_ready[2] = {nullptr, nullptr}, ev_sim_consumed[2] = {nullptr, nullptr}, ev_sim_start = nullptr;
     int64_t last_fact_rows = 0, last_pass_rows = 0;
+    int64_t last_mm_rows = 0;   // rows of mm_fact the last device stage-A chunk wrote (hrag_debug_fact_minmax)
     const hrag::Buf* last_pass_S = &S_pass;   // the passage scores hrag_debug_copy reads (last_pass_rows rows)
 
     hrag_stats_t stats{};
@@ -500,6 +514,10 @@ int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int 
 // Raw fact scores of nb (<= 1024) device queries into S [nb, ldS], the planes streamed once.
 int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ldS);
 int64_t fact_stream_pass_cap(const hrag_t* h);
+
+// api.cu: emb[0].nmax (reset to 0 first when `reset`) raised to the row norms of fact plane rows [row0, row0 + n), on
+// `stream`.  Every writer of resident fact planes calls it, so nmax bounds every row the stage-A screen scores.
+int fact_norms_update(hrag_t* h, int64_t row0, int64_t n, bool reset);
 
 // index_share.cu: status 1 with a message naming `who` when the handle's index is exported or attached (loads and
 // in-place updates would change, or free, memory other processes map); index_share_destroy is hrag_destroy's part:

@@ -321,6 +321,8 @@ int hrag_index_attach(hrag_t* h, const void* blob, int64_t size) {
     h->dim = b.dim;
     h->n_facts_global = b.n_facts_global;
     h->fact_row_lo = 0;
+    HRAG_TRY(fact_norms_update(h, 0, h->emb[0].rows, true));   // this handle's own copy of the screen's bound
+    HRAG_CUDA(cudaStreamSynchronize(h->stream));
     h->row_bounds.assign(b.bounds, b.bounds + b.n_bounds);
     h->chunk_rows = b.n_global;
     h->share.role = SHARE_ATTACHED;

@@ -283,6 +283,8 @@ int append_rows(hrag_t* h, int which, int64_t n_new, const float* rows, bool on_
         HRAG_TRY(grow_keep(h, e.lo, old * d * 2, (old + add) * d * 2));
         HRAG_TRY(split_bf16(src, (int64_t)(add * d), static_cast<char*>(e.hi.p) + old * d * 2,
                             static_cast<char*>(e.lo.p) + old * d * 2, h->stream));
+        // the norm maxima only grow: still bounds after deletes (compact_matrix), raised here by the new rows
+        if (which == 0) HRAG_TRY(fact_norms_update(h, (int64_t)old, (int64_t)add, false));
     }
     HRAG_CUDA(cudaStreamSynchronize(h->stream));   // the staging buffer is freed on return
     e.rows = (int64_t)(old + add);

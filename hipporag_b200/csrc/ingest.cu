@@ -213,6 +213,7 @@ int hrag_load_embeddings(hrag_t* h, int which, int64_t rows, int32_t dim, const 
         HRAG_TRY(e.hi.ensure(n * 2));
         HRAG_TRY(e.lo.ensure(n * 2));
         HRAG_TRY(split_bf16(e.f32, (int64_t)n, e.hi.p, e.lo.p, h->stream));
+        if (which == 0) HRAG_TRY(fact_norms_update(h, 0, e.rows, true));
         HRAG_CUDA(cudaStreamSynchronize(h->stream));
     }
     return 0;
@@ -232,6 +233,10 @@ int hrag_load_embeddings_begin(hrag_t* h, int which, int64_t rows, int32_t dim) 
     const size_t n = (size_t)std::max<int64_t>(h->emb[which].rows, 1) * dim;
     HRAG_TRY(h->emb[which].hi.ensure(n * 2));
     HRAG_TRY(h->emb[which].lo.ensure(n * 2));
+    if (which == 0) {   // the chunks raise the norm maxima from zero
+        HRAG_TRY(fact_norms_update(h, 0, 0, true));
+        HRAG_CUDA(cudaStreamSynchronize(h->stream));
+    }
     return 0;
 }
 
@@ -258,6 +263,7 @@ int hrag_load_embeddings_chunk(hrag_t* h, int which, int64_t row0, int64_t n_row
     }
     HRAG_TRY(split_bf16(src, (int64_t)n, static_cast<char*>(e.hi.p) + (size_t)(a - lo) * h->dim * 2,
                         static_cast<char*>(e.lo.p) + (size_t)(a - lo) * h->dim * 2, h->stream));
+    if (which == 0) HRAG_TRY(fact_norms_update(h, a - lo, b - a, false));
     HRAG_CUDA(cudaStreamSynchronize(h->stream));
     return 0;
 }

@@ -157,10 +157,45 @@ int split_bf16(const float* x, int64_t n, void* hi, void* lo, cudaStream_t strea
 // which a tile list may drop keys (zero-padded; every tile key >= the bound that is in the tile's 8 best stays).  The
 // grid is persistent:
 // n_ctas CTAs (at most one per SM fits) walk the tiles; the merged outputs do not depend on n_ctas.
+// gate != null (fused only): the kernel does nothing unless *gate != 0 when it starts.
 int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const void* e_lo, int64_t M, int dim,
            int n_seg, float* S, int64_t ldS, float2* part_mm, uint64_t* part_keys, uint64_t* part_bound, int n_ctas,
-           cudaStream_t stream);
+           cudaStream_t stream, const int* gate = nullptr);
 int sim_tc_n_tiles(int64_t M);
+
+// ---- the stage-A screen (DESIGN.md section 4, K2): one hi.hi product over all facts, the split product over the
+// candidates only, the same outputs as sim_tc + merge_minmax_topk bit for bit or *flag raised.
+constexpr int kScreenCandidates = 256;   // listed candidates per query
+constexpr int kScreenSatTiles = 8;       // saturated tiles per query
+constexpr int kScreenStageTiles = 48;    // staged 256-column tiles per 128-query m-tile
+// nmax[0 / 1] = max(nmax[0 / 1], largest row norm of hi / lo) over `rows` rows (+inf when one is not finite)
+int plane_norm_max(const void* hi, const void* lo, int64_t rows, int dim, unsigned int* nmax, cudaStream_t stream);
+// err[q] >= |s4 - s1| for query row q and any row of planes whose norm maxima are nmax
+int query_err(const void* q_hi, const void* q_lo, int Bq, int dim, const unsigned int* nmax, float* err,
+              cudaStream_t stream);
+// hi.hi with the screen epilogue: per (query, tile) the 8 best keys (part_keys [Bq, n_tiles, 8]) and the two smallest
+// scores with their rows (part_low [Bq, n_tiles]); part_bound as in sim_tc, its cut lowered by 2 err[q]
+int sim_tc_screen(const void* q_hi, int Bq, const void* e_hi, int64_t M, int dim, const float* err,
+                  uint64_t* part_keys, uint4* part_low, uint64_t* part_bound, int n_ctas, cudaStream_t stream);
+// split scores of the staged tiles: m-tile mt's queries against its stage_count[mt] live tiles of the staging planes
+// (rows (mt * stage_tiles + j) * 256 ...) into S [Bq, stage_tiles * 256]
+int sim_tc_staged(const void* q_hi, const void* q_lo, int Bq, const void* st_hi, const void* st_lo, int stage_tiles,
+                  const int* stage_count, int dim, float* S, int n_ctas, cudaStream_t stream);
+// candidates of each query: cand_ids / cand_s1 [rows, kScreenCandidates], sat [rows, kScreenSatTiles] and counts
+int screen_select(const uint64_t* part_keys, const uint4* part_low, int rows, int n_tiles, const float* err,
+                  int* cand_ids, float* cand_s1, int* cand_n, int* sat, int* sat_n, int* flag, cudaStream_t stream);
+// slots of the candidates per m-tile: pos_of [m_tiles, F] (-1 on entry), slot_ids [m_tiles, stage_tiles, 256] (-1 on
+// entry), res_count [m_tiles, 256] and stage_count [m_tiles] (0 on entry)
+int screen_stage(const int* cand_ids, const int* cand_n, const int* sat, const int* sat_n, int rows, int64_t F,
+                 int stage_tiles, int* pos_of, int* slot_ids, int* res_count, int* stage_count, int* flag,
+                 cudaStream_t stream);
+int screen_gather(const int* slot_ids, const int* stage_count, int m_tiles, int stage_tiles, const void* e_hi,
+                  const void* e_lo, int dim, void* st_hi, void* st_lo, cudaStream_t stream);
+// the outputs of merge_minmax_topk over the rescored staged columns (F facts), after the |s4 - s1| check
+int screen_finish(const float* S, int rows, int stage_tiles, const int* slot_ids, const int* stage_count,
+                  const int* pos_of, int64_t F, const int* cand_ids, const float* cand_s1, const int* cand_n,
+                  const float* err, int k, float2* minmax, int* top_idx, float* top_score, int* n_valid, int* flag,
+                  cudaStream_t stream);
 // Threshold epilogue (index-time synonymy KNN, SURVEY.md 8(f)-2): no score matrix; every score >= thr is appended as
 // a rank key to cand_keys[query, :cand_cap] and counted in cand_count[query] (zeroed by the caller; it keeps counting
 // past cand_cap).  sort_candidates then orders each list and emits the first kmax (cap must be kCandidateCap).
@@ -172,6 +207,10 @@ int sort_candidates(const uint64_t* cand_keys, const int* cand_count, int rows, 
                     float* out_scores, int* n_found, cudaStream_t stream);
 int merge_minmax_topk(const float2* part_mm, const uint64_t* part_keys, int rows, int n_tiles, int64_t M, int k,
                       float2* minmax, int* top_idx, float* top_score, int* n_valid, cudaStream_t stream);
+// merge_minmax_topk that runs only when *gate != 0, and then adds 1 to *fallbacks
+int merge_minmax_topk_gated(const float2* part_mm, const uint64_t* part_keys, int rows, int n_tiles, int64_t M, int k,
+                            float2* minmax, int* top_idx, float* top_score, int* n_valid, const int* gate,
+                            unsigned long long* fallbacks, cudaStream_t stream);
 // Strided form (entry of (row, tile) at row * row_stride + tile * tile_stride) with an index offset; raw_keys != null
 // writes the k best keys of each row unnormalised ([rows, k], 0 = none) instead of idx / score -- the local half of a
 // fact-sharded stage A, whose per-rank results the same kernel merges after the all-gather.

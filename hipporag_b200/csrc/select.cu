@@ -14,6 +14,7 @@ namespace {
 
 constexpr int kSelThreads = 256;
 constexpr int kMaxSmallK = 8;
+constexpr int kScreenCand = kScreenCandidates, kScreenSat = kScreenSatTiles;
 
 __device__ __forceinline__ uint64_t shfl_xor_u64(uint64_t v, int off) {
     uint32_t lo = (uint32_t)v, hi = (uint32_t)(v >> 32);
@@ -96,39 +97,14 @@ k_row_minmax_topk(const float* __restrict__ S, int64_t M, int64_t ld, int k, flo
     if (threadIdx.x == 0) n_valid[row] = kk;
 }
 
-// Finishes the fused similarity epilogue: per query, min/max over the per-tile (min, max) pairs
-// and the k best of the per-tile 8-best rank keys (every global top-8 member is in its tile's top-8).
-// Strided form: tile t of row r lives at part_mm[r * row_stride + t * tile_stride] (keys: 8 per entry), so the
-// same kernel merges the per-rank candidates of a fact-sharded stage A ([rank, query] layout after the all-gather).
-// idx_offset is added to every key's index (local fact row -> global row); with raw_keys != null the 8 best
-// keys are written raw (no normalisation) for a later cross-rank merge.
-__global__ void __launch_bounds__(kSelThreads)
-k_merge_minmax_topk(const float2* __restrict__ part_mm, const uint64_t* __restrict__ part_keys, int n_tiles,
-                    int64_t row_stride, int64_t tile_stride, uint32_t idx_offset, int64_t M, int k,
-                    float2* __restrict__ minmax, int* __restrict__ top_idx, float* __restrict__ top_score,
-                    int* __restrict__ n_valid, uint64_t* __restrict__ raw_keys) {
+// The end of a row's merge, one CTA per row: each thread holds min / max and its K best keys of part of the row; the
+// block reduces min / max into minmax[row] and pops the k best keys (K = kMaxSmallK) into top_idx / top_score
+// (normalised) or raw_keys, n_valid[row] = min(k, M).
+__device__ __forceinline__ void finish_minmax_topk(int row, float mn, float mx, uint64_t (&best)[kMaxSmallK], int64_t M,
+                                                   int k, float2* __restrict__ minmax, int* __restrict__ top_idx,
+                                                   float* __restrict__ top_score, int* __restrict__ n_valid,
+                                                   uint64_t* __restrict__ raw_keys) {
     constexpr int K = kMaxSmallK;
-    const int row = blockIdx.x;
-    float mn = INFINITY, mx = -INFINITY;
-    uint64_t best[K];
-#pragma unroll
-    for (int j = 0; j < K; ++j) best[j] = 0ull;
-    for (int t = threadIdx.x; t < n_tiles; t += kSelThreads) {
-        const size_t e = (size_t)row * row_stride + (size_t)t * tile_stride;
-        const float2 mm = __ldg(part_mm + e);
-        mn = fminf(mn, mm.x);
-        mx = fmaxf(mx, mm.y);
-        const uint64_t* kp = part_keys + e * K;
-#pragma unroll
-        for (int i = 0; i < K; ++i) {
-            uint64_t key = __ldg(kp + i);
-            if (key != 0ull) key -= (uint64_t)idx_offset;        // the index is stored as 0xffffffff - idx
-            if (key > best[K - 1]) {
-#pragma unroll
-                for (int j = 0; j < K; ++j) if (key > best[j]) { const uint64_t tmp = best[j]; best[j] = key; key = tmp; }
-            }
-        }
-    }
     __shared__ float s_mn[kSelThreads / 32], s_mx[kSelThreads / 32];
     __shared__ uint64_t s_key[kSelThreads / 32];
     __shared__ uint64_t s_pick;
@@ -174,6 +150,49 @@ k_merge_minmax_topk(const float2* __restrict__ part_mm, const uint64_t* __restri
         __syncthreads();
     }
     if (threadIdx.x == 0 && n_valid) n_valid[row] = kk;
+}
+
+
+// Finishes the fused similarity epilogue: per query, min/max over the per-tile (min, max) pairs
+// and the k best of the per-tile 8-best rank keys (every global top-8 member is in its tile's top-8).
+// Strided form: tile t of row r lives at part_mm[r * row_stride + t * tile_stride] (keys: 8 per entry), so the
+// same kernel merges the per-rank candidates of a fact-sharded stage A ([rank, query] layout after the all-gather).
+// idx_offset is added to every key's index (local fact row -> global row); with raw_keys != null the 8 best
+// keys are written raw (no normalisation) for a later cross-rank merge.  With gate != null the kernel runs only when
+// *gate != 0 (the exact fallback of the stage-A screen), and then the first CTA counts it in *fallbacks.
+__global__ void __launch_bounds__(kSelThreads)
+k_merge_minmax_topk(const float2* __restrict__ part_mm, const uint64_t* __restrict__ part_keys, int n_tiles,
+                    int64_t row_stride, int64_t tile_stride, uint32_t idx_offset, int64_t M, int k,
+                    float2* __restrict__ minmax, int* __restrict__ top_idx, float* __restrict__ top_score,
+                    int* __restrict__ n_valid, uint64_t* __restrict__ raw_keys, const int* __restrict__ gate,
+                    unsigned long long* __restrict__ fallbacks) {
+    constexpr int K = kMaxSmallK;
+    const int row = blockIdx.x;
+    if (gate) {
+        if (*reinterpret_cast<const volatile int*>(gate) == 0) return;
+        if (row == 0 && threadIdx.x == 0) atomicAdd(fallbacks, 1ull);
+    }
+    float mn = INFINITY, mx = -INFINITY;
+    uint64_t best[K];
+#pragma unroll
+    for (int j = 0; j < K; ++j) best[j] = 0ull;
+    for (int t = threadIdx.x; t < n_tiles; t += kSelThreads) {
+        const size_t e = (size_t)row * row_stride + (size_t)t * tile_stride;
+        const float2 mm = __ldg(part_mm + e);
+        mn = fminf(mn, mm.x);
+        mx = fmaxf(mx, mm.y);
+        const uint64_t* kp = part_keys + e * K;
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            uint64_t key = __ldg(kp + i);
+            if (key != 0ull) key -= (uint64_t)idx_offset;        // the index is stored as 0xffffffff - idx
+            if (key > best[K - 1]) {
+#pragma unroll
+                for (int j = 0; j < K; ++j) if (key > best[j]) { const uint64_t tmp = best[j]; best[j] = key; key = tmp; }
+            }
+        }
+    }
+    finish_minmax_topk(row, mn, mx, best, M, k, minmax, top_idx, top_score, n_valid, raw_keys);
 }
 
 // ---- exact top-k (k <= 2048) of a row by rank key: MSB radix select + bitonic sort ----
@@ -408,7 +427,250 @@ k_fold_topk(int rows, int k, uint32_t idx_offset, const int* __restrict__ slice_
     }
 }
 
+
+// ---- stage-A screen (DESIGN.md section 4, the K2 screen): candidates from the s1 = hi.hi tile lists, staged per
+// 128-query m-tile, rescored by the split K2 and selected exactly.  Any case the screen cannot prove sets *flag; the
+// chunk then reruns the exact path (gated kernels).
+__device__ __forceinline__ void raise_flag(int* flag) { atomicExch(flag, 1); }
+
+// One CTA per query: L = the 8th best s1 key over the tile lists, U = the smallest s1; every listed key with
+// s1 >= L - 2 E_q and every kept low entry with s1 <= U + 2 E_q is a candidate.  A tile whose list is full with its 8th
+// key in the band, or whose second smallest is in the band, may have dropped band members: it is saturated (all its
+// rows become candidates).
+__global__ void __launch_bounds__(kSelThreads)
+k_screen_select(const uint64_t* __restrict__ part_keys, const uint4* __restrict__ part_low, int n_tiles,
+                const float* __restrict__ err, int* __restrict__ cand_ids, float* __restrict__ cand_s1,
+                int* __restrict__ cand_n, int* __restrict__ sat, int* __restrict__ sat_n, int* flag) {
+    constexpr int K = kMaxSmallK;
+    const int row = blockIdx.x;
+    const float E = err[row];
+    if (!(E <= 3.0e38f)) {   // a non-finite bound: NaN / inf in the query or the fact planes
+        if (threadIdx.x == 0) { cand_n[row] = 0; sat_n[row] = 0; raise_flag(flag); }
+        return;
+    }
+    const uint64_t* kp_row = part_keys + (size_t)row * n_tiles * K;
+    const uint4* lo_row = part_low + (size_t)row * n_tiles;
+    uint64_t best[K];
+#pragma unroll
+    for (int j = 0; j < K; ++j) best[j] = 0ull;
+    float U = INFINITY;
+    for (int t = threadIdx.x; t < n_tiles; t += kSelThreads) {
+        U = fminf(U, __uint_as_float(__ldg(&lo_row[t].x)));
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            uint64_t key = __ldg(kp_row + (size_t)t * K + i);
+            if (key > best[K - 1]) {
+#pragma unroll
+                for (int j = 0; j < K; ++j) if (key > best[j]) { const uint64_t tmp = best[j]; best[j] = key; key = tmp; }
+            }
+        }
+    }
+    __shared__ float s_u[kSelThreads / 32];
+    __shared__ uint64_t s_key[kSelThreads / 32];
+    __shared__ uint64_t s_pick;
+    __shared__ int s_n, s_nsat;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int off = 16; off > 0; off >>= 1) U = fminf(U, __shfl_xor_sync(0xffffffffu, U, off));
+    if (lane == 0) s_u[warp] = U;
+    if (threadIdx.x == 0) { s_n = 0; s_nsat = 0; }
+    __syncthreads();
+    U = s_u[0];
+#pragma unroll
+    for (int wi = 1; wi < kSelThreads / 32; ++wi) U = fminf(U, s_u[wi]);
+    int head = 0;
+    uint64_t L = 0ull;
+    for (int round = 0; round < K; ++round) {
+        uint64_t cand = 0ull;
+#pragma unroll
+        for (int j = 0; j < K; ++j) if (j == head) cand = best[j];
+        uint64_t m = cand;
+        for (int off = 16; off > 0; off >>= 1) { const uint64_t o = shfl_xor_u64(m, off); m = o > m ? o : m; }
+        if (lane == 0) s_key[warp] = m;
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            uint64_t b = s_key[0];
+#pragma unroll
+            for (int wi = 1; wi < kSelThreads / 32; ++wi) b = s_key[wi] > b ? s_key[wi] : b;
+            s_pick = b;
+        }
+        __syncthreads();
+        L = s_pick;
+        if (cand != 0ull && cand == s_pick) ++head;
+        __syncthreads();
+    }
+    // fewer than 8 keys in all (F < 8): no threshold, and no list is full
+    const float band_lo = L ? __fsub_rd(key_score(L), 2.f * E) : -INFINITY;
+    const float band_hi = __fadd_ru(U, 2.f * E);
+    auto push = [&](uint32_t id, float s1) {
+        const int pos = atomicAdd(&s_n, 1);
+        if (pos < kScreenCand) {
+            cand_ids[(size_t)row * kScreenCand + pos] = (int)id;
+            cand_s1[(size_t)row * kScreenCand + pos] = s1;
+        }
+    };
+    for (int t = threadIdx.x; t < n_tiles; t += kSelThreads) {
+        const uint64_t* kp = kp_row + (size_t)t * K;
+        bool saturated = false;
+#pragma unroll
+        for (int i = 0; i < K; ++i) {
+            const uint64_t key = __ldg(kp + i);
+            if (key != 0ull && key_score(key) >= band_lo) {
+                push(key_index(key), key_score(key));
+                if (i == K - 1) saturated = true;   // a full list whose last key is in the band
+            }
+        }
+        const uint4 lo = __ldg(lo_row + t);
+        if (lo.y != 0xffffffffu && __uint_as_float(lo.x) <= band_hi) push(lo.y, __uint_as_float(lo.x));
+        if (lo.w != 0xffffffffu && __uint_as_float(lo.z) <= band_hi) {
+            push(lo.w, __uint_as_float(lo.z));
+            saturated = true;
+        }
+        if (saturated) {
+            const int pos = atomicAdd(&s_nsat, 1);
+            if (pos < kScreenSat) sat[(size_t)row * kScreenSat + pos] = t;
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        cand_n[row] = min(s_n, kScreenCand);
+        sat_n[row] = min(s_nsat, kScreenSat);
+        if (s_n > kScreenCand || s_nsat > kScreenSat) raise_flag(flag);
+    }
+}
+
+// One CTA per query: every candidate row (listed, or in a saturated tile) of the query's m-tile mt = row / 128 gets
+// one slot, claimed through pos_of[mt, f] (-1 = none, set by the caller): f goes to column f mod 256 of the m-tile's
+// first staged tile whose column is free.  pos_of then holds f's staged column, j * 256 + f mod 256.
+__global__ void __launch_bounds__(kSelThreads)
+k_screen_stage(const int* __restrict__ cand_ids, const int* __restrict__ cand_n, const int* __restrict__ sat,
+               const int* __restrict__ sat_n, int64_t F, int stage_tiles, int* __restrict__ pos_of,
+               int* __restrict__ slot_ids, int* __restrict__ res_count, int* __restrict__ stage_count, int* flag) {
+    const int row = blockIdx.x, mt = row / 128;
+    int* pos = pos_of + (size_t)mt * F;
+    auto claim = [&](int64_t f) {
+        if (atomicCAS(pos + f, -1, -2) != -1) return;
+        const int c = (int)(f & 255);
+        const int j = atomicAdd(res_count + mt * 256 + c, 1);
+        if (j >= stage_tiles) { raise_flag(flag); return; }
+        slot_ids[((size_t)mt * stage_tiles + j) * 256 + c] = (int)f;
+        pos[f] = j * 256 + c;
+        atomicMax(stage_count + mt, j + 1);
+    };
+    const int n = cand_n[row];
+    for (int i = threadIdx.x; i < n; i += kSelThreads) claim(cand_ids[(size_t)row * kScreenCand + i]);
+    const int ns = sat_n[row];
+    for (int s = 0; s < ns; ++s)
+        for (int c = threadIdx.x; c < 256; c += kSelThreads) {   // the tile's 256 rows
+            const int64_t f = (int64_t)sat[(size_t)row * kScreenSat + s] * 256 + c;
+            if (f < F) claim(f);
+        }
+}
+
+// One warp per staged slot of a live staged tile: its fact's hi / lo rows (zeros for an empty slot) into the staging
+// planes, row (mt * stage_tiles + j) * 256 + c
+__global__ void __launch_bounds__(256)
+k_screen_gather(const int* __restrict__ slot_ids, const int* __restrict__ stage_count, int stage_tiles,
+                const uint4* __restrict__ e_hi, const uint4* __restrict__ e_lo, int dim, uint4* __restrict__ st_hi,
+                uint4* __restrict__ st_lo) {
+    const int slot = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, mt = blockIdx.y;
+    if (slot / 256 >= __ldg(stage_count + mt)) return;
+    const size_t r = (size_t)mt * stage_tiles * 256 + slot;
+    const int id = __ldg(slot_ids + r);
+    const int n16 = dim / 8;
+    for (int i = lane; i < n16; i += 32) {
+        st_hi[r * n16 + i] = id >= 0 ? __ldg(e_hi + (size_t)id * n16 + i) : make_uint4(0u, 0u, 0u, 0u);
+        st_lo[r * n16 + i] = id >= 0 ? __ldg(e_lo + (size_t)id * n16 + i) : make_uint4(0u, 0u, 0u, 0u);
+    }
+}
+
+// One CTA per query: the exact min / max and k best over the rescored staged columns of its m-tile (every candidate
+// is there, with the bits K2 gives it), after checking |s4 - s1| <= E_q on each listed candidate.
+__global__ void __launch_bounds__(kSelThreads)
+k_screen_finish(const float* __restrict__ S, int stage_tiles, const int* __restrict__ slot_ids,
+                const int* __restrict__ stage_count, const int* __restrict__ pos_of, int64_t F,
+                const int* __restrict__ cand_ids, const float* __restrict__ cand_s1, const int* __restrict__ cand_n,
+                const float* __restrict__ err, int k, float2* __restrict__ minmax, int* __restrict__ top_idx,
+                float* __restrict__ top_score, int* __restrict__ n_valid, int* flag) {
+    constexpr int K = kMaxSmallK;
+    const int row = blockIdx.x, mt = row / 128;
+    const int64_t ld = (int64_t)stage_tiles * 256;
+    const float* s = S + (size_t)row * ld;
+    const int* ids = slot_ids + (size_t)mt * ld;
+    const int cols = __ldg(stage_count + mt) * 256;
+    float mn = INFINITY, mx = -INFINITY;
+    uint64_t best[K];
+#pragma unroll
+    for (int j = 0; j < K; ++j) best[j] = 0ull;
+    for (int c = threadIdx.x; c < cols; c += kSelThreads) {
+        const int id = __ldg(ids + c);
+        if (id < 0) continue;
+        const float f = __ldg(s + c);
+        mn = fminf(mn, f);
+        mx = fmaxf(mx, f);
+        uint64_t key = rank_key(f, (uint32_t)id);
+        if (key > best[K - 1]) {
+#pragma unroll
+            for (int j = 0; j < K; ++j) if (key > best[j]) { const uint64_t tmp = best[j]; best[j] = key; key = tmp; }
+        }
+    }
+    const float E = err[row];
+    const int* pos = pos_of + (size_t)mt * F;
+    const int n = cand_n[row];
+    for (int i = threadIdx.x; i < n; i += kSelThreads) {
+        const int p = pos[cand_ids[(size_t)row * kScreenCand + i]];
+        if (p < 0 || !(fabsf(s[p] - cand_s1[(size_t)row * kScreenCand + i]) <= E)) raise_flag(flag);
+    }
+    finish_minmax_topk(row, mn, mx, best, F, k, minmax, top_idx, top_score, n_valid, nullptr);
+}
+
 }  // namespace
+
+int screen_select(const uint64_t* part_keys, const uint4* part_low, int rows, int n_tiles, const float* err,
+                  int* cand_ids, float* cand_s1, int* cand_n, int* sat, int* sat_n, int* flag, cudaStream_t stream) {
+    if (rows == 0) return 0;
+    k_screen_select<<<rows, kSelThreads, 0, stream>>>(part_keys, part_low, n_tiles, err, cand_ids, cand_s1, cand_n,
+                                                      sat, sat_n, flag);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int screen_stage(const int* cand_ids, const int* cand_n, const int* sat, const int* sat_n, int rows, int64_t F,
+                 int stage_tiles, int* pos_of, int* slot_ids, int* res_count, int* stage_count, int* flag,
+                 cudaStream_t stream) {
+    if (rows == 0) return 0;
+    k_screen_stage<<<rows, kSelThreads, 0, stream>>>(cand_ids, cand_n, sat, sat_n, F, stage_tiles, pos_of, slot_ids,
+                                                     res_count, stage_count, flag);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int screen_gather(const int* slot_ids, const int* stage_count, int m_tiles, int stage_tiles, const void* e_hi,
+                  const void* e_lo, int dim, void* st_hi, void* st_lo, cudaStream_t stream) {
+    HRAG_CHECK(dim % 8 == 0, "screen_gather: dim must be a multiple of 8");
+    if (m_tiles == 0) return 0;
+    k_screen_gather<<<dim3((unsigned)(stage_tiles * 256 / 8), (unsigned)m_tiles), 256, 0, stream>>>(
+        slot_ids, stage_count, stage_tiles, static_cast<const uint4*>(e_hi), static_cast<const uint4*>(e_lo), dim,
+        static_cast<uint4*>(st_hi), static_cast<uint4*>(st_lo));
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int screen_finish(const float* S, int rows, int stage_tiles, const int* slot_ids, const int* stage_count,
+                  const int* pos_of, int64_t F, const int* cand_ids, const float* cand_s1, const int* cand_n,
+                  const float* err, int k, float2* minmax, int* top_idx, float* top_score, int* n_valid, int* flag,
+                  cudaStream_t stream) {
+    HRAG_CHECK(k >= 1 && k <= kMaxSmallK, "screen_finish: k must be in [1, 8]");
+    if (rows == 0) return 0;
+    k_screen_finish<<<rows, kSelThreads, 0, stream>>>(S, stage_tiles, slot_ids, stage_count, pos_of, F, cand_ids,
+                                                      cand_s1, cand_n, err, k, minmax, top_idx, top_score, n_valid,
+                                                      flag);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
 
 int fold_topk(int rows, int k, int64_t idx_offset, const int* slice_ids, const float* slice_scores,
               const float2* slice_mm, int* run_ids, float* run_scores, float2* run_mm, int first, cudaStream_t stream) {
@@ -473,6 +735,18 @@ int merge_minmax_topk(const float2* part_mm, const uint64_t* part_keys, int rows
                                 n_valid, nullptr, stream);
 }
 
+int merge_minmax_topk_gated(const float2* part_mm, const uint64_t* part_keys, int rows, int n_tiles, int64_t M, int k,
+                            float2* minmax, int* top_idx, float* top_score, int* n_valid, const int* gate,
+                            unsigned long long* fallbacks, cudaStream_t stream) {
+    HRAG_CHECK(k >= 1 && k <= kMaxSmallK, "merge_minmax_topk: k must be in [1, 8]");
+    if (rows == 0) return 0;
+    k_merge_minmax_topk<<<rows, kSelThreads, 0, stream>>>(part_mm, part_keys, n_tiles, n_tiles, 1, 0u, M, k, minmax,
+                                                          top_idx, top_score, n_valid, nullptr, gate, fallbacks);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
 int merge_minmax_topk_ex(const float2* part_mm, const uint64_t* part_keys, int rows, int n_tiles, int64_t row_stride,
                          int64_t tile_stride, int64_t idx_offset, int64_t M, int k, float2* minmax, int* top_idx,
                          float* top_score, int* n_valid, uint64_t* raw_keys, cudaStream_t stream) {
@@ -481,7 +755,7 @@ int merge_minmax_topk_ex(const float2* part_mm, const uint64_t* part_keys, int r
     if (rows == 0) return 0;
     k_merge_minmax_topk<<<rows, kSelThreads, 0, stream>>>(part_mm, part_keys, n_tiles, row_stride, tile_stride,
                                                           (uint32_t)idx_offset, M, k, minmax, top_idx, top_score,
-                                                          n_valid, raw_keys);
+                                                          n_valid, raw_keys, nullptr, nullptr);
     count_launch(1);
     HRAG_CUDA(cudaGetLastError());
     return 0;

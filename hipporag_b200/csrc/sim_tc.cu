@@ -141,6 +141,17 @@ struct TcParams {
     uint64_t* cand_keys;      // [Bq, cand_cap]
     int* cand_count;          // [Bq]
     int cand_cap;
+    // fused epilogue of the exact fallback (FUSE == 1): with gate != null the kernel runs only when *gate != 0
+    const int* gate;
+    // screen epilogue (FUSE == 4, hi planes only): per (query, tile) the 8 best keys of s1 = hi.hi into part_keys and
+    // the two smallest s1 with their rows into part_low {s1 bits, row, s1 bits, row}; err [Bq] = the per-query bound
+    // E_q on |s4 - s1|, so the tile lists may drop only keys below the running bound minus 2 E_q
+    const float* err;
+    uint4* part_low;          // [Bq, num_n_tiles]
+    // staged rescore (FUSE == 3): the B rows of m-tile mt are its own stage_tiles staged tiles, of which the first
+    // stage_count[mt] are live; scores are stored as in FUSE 0 into S [Bq, stage_tiles * 256]
+    int stage_tiles;
+    const int* stage_count;   // [num_m_tiles]
 };
 
 constexpr int kFuseK = 8;
@@ -183,7 +194,9 @@ __device__ __forceinline__ void merge_best_xor(uint64_t (&best)[kFuseK], int off
             if ((k & stride) == 0) cmp_swap_desc(best[k], best[k + stride]);
 }
 
-template <bool SPLIT, int FUSE>          // FUSE: 0 = store scores, 1 = min/max + 8 best per tile, 2 = threshold append
+// FUSE: 0 = store scores, 1 = min/max + 8 best per tile, 2 = threshold append, 3 = store scores of staged tiles,
+// 4 = screen (8 best and 2 smallest per tile, bound gate widened by 2 E_q)
+template <bool SPLIT, int FUSE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ CUtensorMap map_q_lo,
          const __grid_constant__ CUtensorMap map_e_hi, const __grid_constant__ CUtensorMap map_e_lo, TcParams p) {
@@ -204,6 +217,7 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nkb = (p.dim + BKs - 1) / BKs;
     const int total_tiles = p.num_m_tiles * p.num_n_tiles;
+    if (FUSE == 1 && p.gate != nullptr && *reinterpret_cast<const volatile int*>(p.gate) == 0) return;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), CONSUMER_WARPS); }
@@ -228,11 +242,13 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
             uint32_t phase = 0;
             for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
                 const int mt = t % p.num_m_tiles, nt = t / p.num_m_tiles;
+                if (FUSE == 3 && nt >= __ldg(p.stage_count + mt)) continue;
+                const int brow = FUSE == 3 ? (mt * p.stage_tiles + nt) * BN : nt * BN;
                 // L2 prefetch of this CTA's share of the NEXT embedding tile: the num_m_tiles CTAs that
                 // will work on it each pull every num_m_tiles-th k-block, a whole tile ahead, so the
                 // later TMA loads of all of them are L2 hits instead of num_m_tiles DRAM reads
                 const int tn = t + gridDim.x;
-                if (tn < total_tiles) {
+                if (FUSE != 3 && tn < total_tiles) {
                     const int mtn = tn % p.num_m_tiles, ntn = tn / p.num_m_tiles;
                     for (int kb = mtn; kb < nkb; kb += p.num_m_tiles) {
                         tma_prefetch_l2_2d(&map_e_hi, kb * BKs, ntn * BN);
@@ -244,10 +260,10 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                     mbar_expect_tx(full_bar(stage), STAGE_BYTES);
                     const uint32_t sa = base + stage * STAGE_BYTES;
                     tma_load_2d(sa, &map_q_hi, full_bar(stage), kb * BKs, mt * BM);
-                    tma_load_2d(sa + OFF_B_HI, &map_e_hi, full_bar(stage), kb * BKs, nt * BN);
+                    tma_load_2d(sa + OFF_B_HI, &map_e_hi, full_bar(stage), kb * BKs, brow);
                     if (SPLIT) {
                         tma_load_2d(sa + OFF_A_LO, &map_q_lo, full_bar(stage), kb * BKs, mt * BM);
-                        tma_load_2d(sa + OFF_B_LO, &map_e_lo, full_bar(stage), kb * BKs, nt * BN);
+                        tma_load_2d(sa + OFF_B_LO, &map_e_lo, full_bar(stage), kb * BKs, brow);
                     }
                     if (++stage == STAGES) { stage = 0; phase ^= 1u; }
                 }
@@ -266,6 +282,7 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
     uint32_t phase = 0;
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
         const int mt = t % p.num_m_tiles, nt = t / p.num_m_tiles;
+        if (FUSE == 3 && nt >= __ldg(p.stage_count + mt)) continue;
         int prev_stage = -1;
         for (int kb = 0; kb < nkb; ++kb) {
             mbar_wait(full_bar(stage), phase);
@@ -377,6 +394,67 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                     if (best[kFuseK - 1] > thr)
                         atomicMax(reinterpret_cast<unsigned long long*>(p.bound + q), (unsigned long long)best[kFuseK - 1]);
                 }
+            } else if (FUSE == 4) {
+                // As FUSE 1, in s1 space, with the bound's cut lowered by 2 E_q: a key the gate drops is below every
+                // key the candidate band of its query can hold (select.cu: screen_select).  A lane's own 8th best
+                // still cuts unwidened: a list that drops keys that way is full, and a full list whose 8th key lies in
+                // the band marks its tile saturated.  The two smallest valid scores per row are kept beside the list.
+                const bool live = q < p.Bq;
+                const uint64_t thr = live ? __ldcg(reinterpret_cast<const unsigned long long*>(p.bound + q)) : 0ull;
+                const float cut_thr = __fsub_rd(key_score(thr), live ? 2.f * __ldg(p.err + q) : 0.f);
+                float cut = cut_thr;
+                float m1 = INFINITY, m2 = INFINITY;
+                uint32_t i1 = 0xffffffffu, i2 = 0xffffffffu;
+                uint64_t best[kFuseK];
+#pragma unroll
+                for (int k = 0; k < kFuseK; ++k) best[k] = 0ull;
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j) {
+                    bool pass[2];
+#pragma unroll
+                    for (int c = 0; c < 2; ++c) {
+                        const int col = 8 * j + c0 + c;
+                        const float f = d[4 * j + 2 * h + c];
+                        const bool valid = col < n_valid;
+                        if (valid && f < m2) {
+                            const uint32_t idx = (uint32_t)(n0 + col);
+                            if (f < m1) { m2 = m1; i2 = i1; m1 = f; i1 = idx; }
+                            else { m2 = f; i2 = idx; }
+                        }
+                        pass[c] = live && valid && !(f < cut);
+                    }
+                    if (__any_sync(0xffffffffu, pass[0] || pass[1])) {
+#pragma unroll
+                        for (int c = 0; c < 2; ++c)
+                            if (pass[c]) insert_best(best, acc_rank_key(d[4 * j + 2 * h + c], (uint32_t)(n0 + 8 * j + c0 + c)));
+                        cut = best[kFuseK - 1] > thr ? key_score(best[kFuseK - 1]) : cut_thr;
+                    }
+                }
+#pragma unroll
+                for (int off = 1; off <= 2; off <<= 1) {
+                    const float o1 = __shfl_xor_sync(0xffffffffu, m1, off), o2 = __shfl_xor_sync(0xffffffffu, m2, off);
+                    const uint32_t oi1 = __shfl_xor_sync(0xffffffffu, i1, off), oi2 = __shfl_xor_sync(0xffffffffu, i2, off);
+                    // the two smallest of two sorted pairs: the smaller head, then the smaller of the other head and
+                    // the winner's second
+                    const bool ofirst = o1 < m1 || (o1 == m1 && oi1 < i1);
+                    const float l = ofirst ? m1 : o1, w2 = ofirst ? o2 : m2;
+                    const uint32_t li = ofirst ? i1 : oi1, w2i = ofirst ? oi2 : i2;
+                    m1 = ofirst ? o1 : m1;
+                    i1 = ofirst ? oi1 : i1;
+                    const bool lfirst = l < w2 || (l == w2 && li < w2i);
+                    m2 = lfirst ? l : w2;
+                    i2 = lfirst ? li : w2i;
+                    merge_best_xor(best, off);
+                }
+                if (q < p.Bq && (lane & 3) == 0) {
+                    const size_t o = (size_t)q * p.num_n_tiles + nt;
+                    p.part_low[o] = make_uint4(__float_as_uint(m1), i1, __float_as_uint(m2), i2);
+#pragma unroll
+                    for (int k = 0; k < kFuseK; k += 2)
+                        *reinterpret_cast<ulonglong2*>(p.part_keys + o * kFuseK + k) = make_ulonglong2(best[k], best[k + 1]);
+                    if (best[kFuseK - 1] > thr)
+                        atomicMax(reinterpret_cast<unsigned long long*>(p.bound + q), (unsigned long long)best[kFuseK - 1]);
+                }
             } else {
                 if (q < p.Bq) {
                     float* row = p.S + (size_t)q * p.ldS + n0;
@@ -412,6 +490,55 @@ k_split_bf16(const float* __restrict__ x, int64_t n, __nv_bfloat16* __restrict__
             hi[j] = h;
             lo[j] = __float2bfloat16_rn(x[j] - __bfloat162float(h));
         }
+    }
+}
+
+// Upper bounds on the L2 norms of bf16 rows: one warp per row, fp32 sums of squares.  A non-finite norm becomes +inf,
+// so a NaN or an infinity in a plane turns every bound built on it into +inf (the screen then falls back).
+__device__ __forceinline__ float warp_row_norm(const __nv_bfloat16* __restrict__ x, int dim, int lane) {
+    float s = 0.f;
+    for (int i = 2 * lane; i < dim; i += 64) {
+        const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(x + i));
+        s = fmaf(v.x, v.x, fmaf(v.y, v.y, s));
+    }
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+    const float n = sqrtf(s);
+    return n <= 3.0e38f ? n : INFINITY;
+}
+
+// nmax[0] / nmax[1] = max(themselves, the largest row norm of hi / lo over `rows` rows): float bits of non-negative
+// values order as unsigned integers
+__global__ void __launch_bounds__(256)
+k_plane_norm_max(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo, int64_t rows, int dim,
+                 unsigned int* __restrict__ nmax) {
+    const int64_t r = ((int64_t)blockIdx.x * 256 + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (r >= rows) return;
+    const float nh = warp_row_norm(hi + (size_t)r * dim, dim, lane), nl = warp_row_norm(lo + (size_t)r * dim, dim, lane);
+    if (lane == 0) {
+        atomicMax(nmax, __float_as_uint(nh));
+        atomicMax(nmax + 1, __float_as_uint(nl));
+    }
+}
+
+// E_q >= |s4 - s1| for query row q against any fact row, s4 / s1 the split / hi-only K2 accumulators (DESIGN.md
+// section 4, the stage-A screen): the three dropped products by Cauchy-Schwarz with the fact planes' largest row norms
+// Hf / Lf, plus the fp32 accumulation of both GEMMs at a relative error of 2^-21 per k16 step (dim / 16 steps for s1,
+// 4 dim / 16 for s4) on the sum of |products| <= (|qh| + |ql|)(Hf + Lf); the whole raised by 2^-10 for the rounding of
+// the norms and of this sum.
+__global__ void __launch_bounds__(256)
+k_query_err(const __nv_bfloat16* __restrict__ q_hi, const __nv_bfloat16* __restrict__ q_lo, int Bq, int dim,
+            const unsigned int* __restrict__ nmax, float* __restrict__ err) {
+    const int q = (blockIdx.x * 256 + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (q >= Bq) return;
+    const float nh = warp_row_norm(q_hi + (size_t)q * dim, dim, lane), nl = warp_row_norm(q_lo + (size_t)q * dim, dim, lane);
+    if (lane == 0) {
+        const float Hf = __uint_as_float(nmax[0]), Lf = __uint_as_float(nmax[1]);
+        const float steps = 5.f * (float)((dim + 15) / 16);
+        const float e = nh * Lf + nl * Hf + nl * Lf + steps * 0x1p-21f * (nh + nl) * (Hf + Lf);
+        err[q] = e * (1.f + 0x1p-10f);
     }
 }
 
@@ -481,6 +608,7 @@ int sim_tc_threshold(const void* q_hi, const void* q_lo, int Bq, const void* e_h
     TcParams p;
     p.Bq = Bq; p.M = M; p.dim = dim; p.S = nullptr; p.ldS = 0; p.part_mm = nullptr; p.part_keys = nullptr;
     p.bound = nullptr; p.thr = thr; p.cand_keys = cand_keys; p.cand_count = cand_count; p.cand_cap = cand_cap;
+    p.gate = nullptr; p.err = nullptr; p.part_low = nullptr; p.stage_tiles = 0; p.stage_count = nullptr;
     p.num_m_tiles = (int)ceil_div(Bq, BM);
     p.num_n_tiles = (int)ceil_div(M, BN);
     const int grid = (int)std::min<int64_t>((int64_t)p.num_m_tiles * p.num_n_tiles, num_sms);
@@ -493,7 +621,7 @@ int sim_tc_threshold(const void* q_hi, const void* q_lo, int Bq, const void* e_h
 
 int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const void* e_lo, int64_t M, int dim,
            int n_seg, float* S, int64_t ldS, float2* part_mm, uint64_t* part_keys, uint64_t* part_bound, int n_ctas,
-           cudaStream_t stream) {
+           cudaStream_t stream, const int* gate) {
     HRAG_CHECK(dim % 8 == 0, "sim_tc: embedding dim must be a multiple of 8 (TMA row pitch)");
     HRAG_CHECK(n_seg == 1 || n_seg == 4, "sim_tc: n_seg must be 1 (bf16) or 4 (split)");
     HRAG_CHECK(part_mm == nullptr || (part_keys != nullptr && part_bound != nullptr), "sim_tc: fused buffers missing");
@@ -518,6 +646,7 @@ int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const v
     const bool fuse = part_mm != nullptr;
     if (fuse) HRAG_CUDA(cudaMemsetAsync(part_bound, 0, (size_t)Bq * sizeof(uint64_t), stream));
     p.thr = 0.f; p.cand_keys = nullptr; p.cand_count = nullptr; p.cand_cap = 0;
+    p.gate = gate; p.err = nullptr; p.part_low = nullptr; p.stage_tiles = 0; p.stage_count = nullptr;
     HRAG_CHECK(fuse || (S != nullptr && ldS % 4 == 0), "sim_tc: score buffer missing");
     p.num_m_tiles = (int)ceil_div(Bq, BM);
     p.num_n_tiles = (int)ceil_div(M, BN);
@@ -527,6 +656,80 @@ int sim_tc(const void* q_hi, const void* q_lo, int Bq, const void* e_hi, const v
     else if (n_seg == 4) k_sim_tc<true, 0><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
     else if (fuse) k_sim_tc<false, 1><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
     else k_sim_tc<false, 0><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int sim_tc_screen(const void* q_hi, int Bq, const void* e_hi, int64_t M, int dim, const float* err,
+                  uint64_t* part_keys, uint4* part_low, uint64_t* part_bound, int n_ctas, cudaStream_t stream) {
+    HRAG_CHECK(dim % 8 == 0, "sim_tc_screen: embedding dim must be a multiple of 8 (TMA row pitch)");
+    if (Bq == 0 || M == 0) return 0;
+    static bool attr_set = false;
+    if (!attr_set) {
+        HRAG_CUDA(cudaFuncSetAttribute(k_sim_tc<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+        attr_set = true;
+    }
+    CUtensorMap mq, me;
+    HRAG_TRY(make_map(&mq, q_hi, Bq, dim, BK, BM));
+    HRAG_TRY(make_map(&me, e_hi, M, dim, BK, BN));
+    TcParams p{};
+    p.Bq = Bq; p.M = M; p.dim = dim; p.part_keys = part_keys; p.bound = part_bound; p.err = err; p.part_low = part_low;
+    p.num_m_tiles = (int)ceil_div(Bq, BM);
+    p.num_n_tiles = (int)ceil_div(M, BN);
+    HRAG_CUDA(cudaMemsetAsync(part_bound, 0, (size_t)Bq * sizeof(uint64_t), stream));
+    const int64_t tiles = (int64_t)p.num_m_tiles * p.num_n_tiles;
+    const int grid = (int)std::min<int64_t>(tiles, std::max(n_ctas, 1));
+    k_sim_tc<false, 4><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mq, mq, me, me, p);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int sim_tc_staged(const void* q_hi, const void* q_lo, int Bq, const void* st_hi, const void* st_lo, int stage_tiles,
+                  const int* stage_count, int dim, float* S, int n_ctas, cudaStream_t stream) {
+    HRAG_CHECK(dim % 8 == 0, "sim_tc_staged: embedding dim must be a multiple of 8 (TMA row pitch)");
+    if (Bq == 0) return 0;
+    static bool attr_set = false;
+    if (!attr_set) {
+        HRAG_CUDA(cudaFuncSetAttribute(k_sim_tc<true, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM_BYTES));
+        attr_set = true;
+    }
+    TcParams p{};
+    p.Bq = Bq; p.dim = dim; p.S = S;
+    p.num_m_tiles = (int)ceil_div(Bq, BM);
+    p.num_n_tiles = stage_tiles;
+    p.stage_tiles = stage_tiles; p.stage_count = stage_count;
+    p.M = (int64_t)stage_tiles * BN;          // every staged tile is 256 columns wide (empty slots masked later)
+    p.ldS = (int64_t)stage_tiles * BN;
+    CUtensorMap mqh, mql, meh, mel;
+    const int64_t rows = (int64_t)p.num_m_tiles * stage_tiles * BN;
+    HRAG_TRY(make_map(&mqh, q_hi, Bq, dim, BK / 2, BM));
+    HRAG_TRY(make_map(&mql, q_lo, Bq, dim, BK / 2, BM));
+    HRAG_TRY(make_map(&meh, st_hi, rows, dim, BK / 2, BN));
+    HRAG_TRY(make_map(&mel, st_lo, rows, dim, BK / 2, BN));
+    const int64_t tiles = (int64_t)p.num_m_tiles * stage_tiles;
+    const int grid = (int)std::min<int64_t>(tiles, std::max(n_ctas, 1));
+    k_sim_tc<true, 3><<<grid, TC_THREADS, SMEM_BYTES, stream>>>(mqh, mql, meh, mel, p);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int plane_norm_max(const void* hi, const void* lo, int64_t rows, int dim, unsigned int* nmax, cudaStream_t stream) {
+    if (rows <= 0) return 0;
+    k_plane_norm_max<<<(unsigned)ceil_div(rows * 32, 256), 256, 0, stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(hi), reinterpret_cast<const __nv_bfloat16*>(lo), rows, dim, nmax);
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int query_err(const void* q_hi, const void* q_lo, int Bq, int dim, const unsigned int* nmax, float* err,
+              cudaStream_t stream) {
+    if (Bq <= 0) return 0;
+    k_query_err<<<(unsigned)ceil_div((int64_t)Bq * 32, 256), 256, 0, stream>>>(
+        reinterpret_cast<const __nv_bfloat16*>(q_hi), reinterpret_cast<const __nv_bfloat16*>(q_lo), Bq, dim, nmax, err);
     count_launch(1);
     HRAG_CUDA(cudaGetLastError());
     return 0;

@@ -107,6 +107,14 @@ int invalidate_solves(hrag_t* h) {
 
 int resolve_spans(hrag_t* h) {
     HRAG_CUDA(cudaStreamSynchronize(h->stream));
+    if (h->scr.fallbacks.p) {
+        // the stage-A screen's fallbacks, counted on the device by work ordered before the end of `stream`
+        unsigned long long n = 0;
+        HRAG_CUDA(cudaMemcpyAsync(&n, h->scr.fallbacks.p, sizeof(n), cudaMemcpyDeviceToHost, h->stream));
+        if (n) HRAG_CUDA(cudaMemsetAsync(h->scr.fallbacks.p, 0, sizeof(n), h->stream));
+        HRAG_CUDA(cudaStreamSynchronize(h->stream));
+        h->stats.stage_a_fallbacks += (int64_t)n;
+    }
     if (h->p2p && h->p2p_err.p) {
         int err = 0;
         HRAG_CUDA(cudaMemcpy(&err, h->p2p_err.p, sizeof(int), cudaMemcpyDeviceToHost));

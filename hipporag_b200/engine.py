@@ -652,6 +652,18 @@ class Engine:
         side through the slot map (tests, benchmarks: both give the same bytes); False restores the default."""
         _lib.check(self._lib.hrag_debug_dense_first_sweep(self._h, 1 if on else 0))
 
+    def debug_exact_stage_a(self, on: bool = True):
+        """Make stage A run the split similarity GEMM over all facts instead of the hi.hi screen and the split rescore
+        of its candidates (tests, benchmarks: both give the same bytes); False restores the default."""
+        _lib.check(self._lib.hrag_debug_exact_stage_a(self._h, 1 if on else 0))
+
+    def debug_fact_minmax(self) -> np.ndarray:
+        """[rows, 2] fp32: the per-query (min, max) fact scores of the last device stage-A chunk (tests)."""
+        buf = np.empty((1024, 2), dtype=np.float32)
+        n = C.c_int64()
+        _lib.check(self._lib.hrag_debug_fact_minmax(self._h, _ptr(buf), buf.shape[0], C.byref(n)))
+        return buf[:n.value].copy()
+
     def debug_scores(self, which: int) -> np.ndarray:
         cols = self.n_facts if which == 0 else self.n_passages
         buf = np.empty(1024 * max(cols, 1), dtype=np.float32)

@@ -58,6 +58,8 @@ typedef struct hrag_stats {
     double ppr_error_bound;  /* a-posteriori bound on the relative L1 error of the PPR vectors of that call:   */
                              /* mixed solver: ppr_residual x the predicted contraction of the refinement round; */
                              /* hrag_ppr_f64: 2 ppr_residual / (1 - damping), rigorous (no model constant)     */
+    int64_t stage_a_fallbacks; /* stage-A chunks whose hi.hi screen could not prove its candidates and that    */
+                               /* reran the split GEMM over all facts (read at the end of each stage call)    */
 } hrag_stats_t;
 
 const char* hrag_last_error(void);
@@ -159,6 +161,10 @@ int hrag_load_embeddings_chunk(hrag_t* h, int which, int64_t row0, int64_t n_row
  * (which = 0), the update entries and sharded handles (world > 1) are rejected; h2d_bytes counts the streamed plane
  * bytes.  A reload or hrag_destroy frees the pinned memory.  The passage planes are always resident. */
 int hrag_set_fact_memory(hrag_t* h, int64_t max_device_bytes);
+/* The budget covers the fact planes only.  Resident planes of at least 65,536 facts also take the stage-A screen's
+ * scratch at the first stage-A call (one GPU, HRAG_SIM_BF16X3): about 0.6 GB at 2.75 M facts x 768 for a
+ * 1,024-query chunk (per m-tile staging planes 48 x 256 x d x 4 bytes, per query and 256-fact tile 16 bytes, per
+ * m-tile and fact 4 bytes). */
 /* What the last fact load chose: on_host (1 = pinned host planes), the ring's slice_rows (0 when resident), the
  * device bytes of the fact planes (the ring, or the resident planes) and the pinned host bytes (0 when resident). */
 int hrag_fact_planes_info(hrag_t* h, int* on_host, int64_t* slice_rows, int64_t* device_bytes, int64_t* host_bytes);
@@ -406,6 +412,9 @@ int hrag_reset_stats(hrag_t* h);
 /* Raw device buffers for tests/benchmarks: which = 0 fact scores of the last stage A
  * sub-batch, 1 passage scores of the last stage B sub-batch. */
 int hrag_debug_copy(hrag_t* h, int which, float* host_out, int64_t max_elems, int64_t* n_written);
+/* The per-query (min, max) fact scores of the last device stage-A chunk (<= 1024 rows of 2 floats; 0 rows after a
+ * stage A over host fact planes). */
+int hrag_debug_fact_minmax(hrag_t* h, float* host_out, int64_t max_rows, int64_t* n_rows);
 /* One plane of the loaded graph, byte for byte (tests compare the ingest planes): plane = 0 row_ptr int32[n_rows + 1],
  * 1 cv int2[nnz], 2 val_lo fp32[nnz] (empty without the fp64 operator), 3 row_order int32[n_rows], 4 long_rows
  * int32[n_long], 5 long_seg_ptr int32[n_long + 1] (empty when n_long = 0), 6 segs int4[n_seg].  *n_written = the
@@ -430,6 +439,9 @@ int hrag_debug_sim_ctas(hrag_t* h, int n);
  * node-range-sharded handles do, instead of reading it through the slot map (tests and benchmarks compare the two
  * forms; the results are the same bit for bit); 0 restores the default. */
 int hrag_debug_dense_first_sweep(hrag_t* h, int on);
+/* on != 0: stage A runs the split GEMM over all facts instead of the hi.hi screen and the split rescore of its
+ * candidates (tests and benchmarks compare the two; the results are the same bit for bit); 0 restores the default. */
+int hrag_debug_exact_stage_a(hrag_t* h, int on);
 
 #ifdef __cplusplus
 }

@@ -2,10 +2,14 @@
 """Stage A's fact GEMM (K2, k_sim_tc with the fused top-8 epilogue) alone, then the chunk-overlap scan of
 retrieve_resident.
 
-    python tools/stage_a_bench.py [--workload C3] [--reps 5] [--steps 2] [--scan 0,40,48,54,56,66] [--out FILE]
+    python tools/stage_a_bench.py [--workload C3] [--reps 5] [--steps 2] [--scan=0,-1,40,48] [--exact] [--out FILE]
 
 K2 alone: stage_a on the workload's queries (1,024-query chunks) on the whole GPU; `ms_per_chunk` is the library's
 sim_fact span (bf16 split of the queries + the GEMM, CUDA events) divided by the chunks, the median of --reps calls.
+With the stage-A screen (the default; --exact runs the split GEMM over all facts instead) the span holds the screen
+and the rescore; `screen_parts` then gives each part's kernel time per chunk from one profiled stage_a call
+(torch.profiler): the screen (query split and bound, hi.hi GEMM), the candidate selection and staging, the split
+rescore, the final selection, and the gated exact fallback (0 unless a chunk fell back).
 The scan: one retrieve_resident step (the bench.py step) per G, CUDA events around --steps steps after a warm-up step;
 G = 0 is the rule in overlap_ctas, G = -1 runs the chunks one after the other without the overlap.  The G values
 alternate within each of --rounds rounds.  One JSON line per measurement, then a summary with the card's name and
@@ -35,6 +39,27 @@ def card():
     return info
 
 
+PARTS = (("screen", ("k_split_bf16", "k_query_err", "k_sim_tc<false, 4>")),
+         ("select", ("k_screen_select", "k_screen_stage", "k_screen_gather")),
+         ("rescore", ("k_sim_tc<true, 3>",)),
+         ("finish", ("k_screen_finish",)),
+         ("exact_fallback", ("k_sim_tc<true, 1>", "k_merge_minmax_topk")))
+
+
+def screen_parts(e, qf, chunks):
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        e.stage_a(qf, bench.LINK_TOP_K)
+        torch.cuda.synchronize()
+    ms = {name: 0.0 for name, _ in PARTS}
+    for ev in prof.key_averages():
+        for name, keys in PARTS:
+            if any(k in ev.key for k in keys):
+                ms[name] += ev.device_time_total / 1e3
+    return {name: round(v / chunks, 3) for name, v in ms.items()}
+
+
 def emit(rec, out):
     line = json.dumps(rec)
     print(line, flush=True)
@@ -51,6 +76,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=1)
     ap.add_argument("--scan", default="0,-1,40,48,56,66")
     ap.add_argument("--out", default="")
+    ap.add_argument("--exact", action="store_true", help="run stage A without the screen")
     args = ap.parse_args()
     import torch
     from hipporag_b200 import Engine
@@ -64,6 +90,8 @@ def main():
     e.load_graph_csr(kg.n_nodes, *wl.csr)
     e.load_tables(kg.passage_vid, kg.fact_subj_vid, kg.fact_obj_vid, kg.ent_chunk_count)
     e.load_embeddings(wl.fe, wl.pe)
+    if args.exact:
+        e.debug_exact_stage_a(True)
     chunks = -(-Q // 1024)
     summary = {"workload": args.workload, "queries": Q, "facts": kg.n_facts, "dim": w["dim"], **info}
 
@@ -81,6 +109,9 @@ def main():
     med = float(np.median(k2))
     summary["k2_alone_ms_per_chunk"] = {"min": round(min(k2), 3), "median": round(med, 3), "max": round(max(k2), 3)}
     summary["k2_alone_tflops_issued"] = round(flop / (med * 1e-3) / 1e12, 1)
+    summary["stage_a_fallbacks"] = e.stats()["stage_a_fallbacks"]
+    if not args.exact:
+        summary["screen_parts_ms_per_chunk"] = screen_parts(e, qf, chunks)
 
     # ---- G scan of retrieve_resident
     out_ids = torch.empty((Q, bench.TOPK), dtype=torch.int32, device=device)
