@@ -58,6 +58,7 @@ SIGNATURES = {
     "hrag_load_embeddings_chunk": (C.c_int, [_p, C.c_int, _i64, _i64, _p, C.c_int]),
     "hrag_set_mutable": (C.c_int, [_p, C.c_int]),
     "hrag_set_fact_memory": (C.c_int, [_p, _i64]),
+    "hrag_set_fact_placement": (C.c_int, [_p, C.c_int]),
     "hrag_fact_planes_info": (C.c_int, [_p, C.POINTER(C.c_int), C.POINTER(_i64), C.POINTER(_i64), C.POINTER(_i64)]),
     "hrag_index_reserve": (C.c_int, [_p, _i64, _i64, _i64, _i64]),
     "hrag_index_append": (C.c_int, [_p, _i64, _i64, _p, _p, _p, _i64, _p, _i64, _p, _p, _p, _i32, _p, _p, C.c_int]),

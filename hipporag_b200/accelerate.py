@@ -217,7 +217,7 @@ def _resident_knn_applies(query_ids, key_ids, query_vecs, key_vecs, thr: float) 
 def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_workers: int = 1,
                filter_chunk: int = 256, ppr_tol: float = 0.0, cache: bool = True, run_ppr_fp64: bool = False,
                incremental: bool = False, fact_device_bytes: Optional[int] = None, attach: Optional[bytes] = None,
-               knn_device_bytes: Optional[int] = None, **engine_opts):
+               knn_device_bytes: Optional[int] = None, fact_lo_on_host: bool = False, **engine_opts):
     """Rebinds the hot-path methods of ``rag`` (a reference ``HippoRAG`` instance) in place.
 
     ``filter_workers > 1`` (SURVEY.md 8(f)-1) runs the per-query recognition-memory filter calls (LLM HTTP
@@ -251,6 +251,11 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     Stage A then streams the planes once per call, so ``filter_workers > 1`` streams them once per ``filter_chunk``
     queries: give it a large ``filter_chunk``.  Host planes cannot be updated in place: with ``incremental=True``
     every ``index()`` / ``delete()`` takes the full reload.
+    ``fact_lo_on_host=True`` (``Engine.set_fact_placement``, needs ``fact_device_bytes``): over the budget only the lo
+    fact plane goes to pinned host memory and the hi plane stays resident, so stage A runs the stage-A screen at
+    about its resident cost and reads only the candidates' lo rows over PCIe, with the same results; the budget must
+    hold the hi plane (rows x dim x 2 bytes) plus two 256-row lo slices.  Like host planes it cannot be updated in
+    place: with ``incremental=True`` every ``index()`` / ``delete()`` takes the full reload.
     ``knn_device_bytes`` (``Engine.knn_set_memory``, needs ``incremental=True``: only the resident self-KNN index uses
     it): device memory the synonymy KNN index's planes may take; larger planes are kept in pinned host memory and
     streamed through the GPU by every update, with the same synonymy edges and ``last_knn`` values.
@@ -258,15 +263,18 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
     ``prepare_retrieval_objects`` has run, the index fingerprint is checked against the owner's (a mismatch raises)
     and the engine maps the owner's index read-only (``Engine.attach``) instead of uploading one; only the fact
     triples the filter needs are read on the host (from the cache, else ``extract_tables``).  ``index()`` /
-    ``delete()`` then raise: the owner updates the index (see ``share``).  ``attach`` excludes ``incremental`` and
-    ``fact_device_bytes`` (ValueError).
+    ``delete()`` then raise: the owner updates the index (see ``share``).  ``attach`` excludes ``incremental``,
+    ``fact_device_bytes`` and ``fact_lo_on_host`` (ValueError).
     ``engine_opts`` go to ``Engine.set_options``.
     """
     from hipporag.utils.misc_utils import QuerySolution
 
-    if attach is not None and (incremental or fact_device_bytes is not None):
+    if attach is not None and (incremental or fact_device_bytes is not None or fact_lo_on_host):
         raise ValueError("accelerate(attach=...) serves another process's index read-only: it excludes "
-                         "incremental=True and fact_device_bytes")
+                         "incremental=True, fact_device_bytes and fact_lo_on_host")
+    if fact_lo_on_host and fact_device_bytes is None:
+        raise ValueError("accelerate(fact_lo_on_host=True) places the fact planes under a device budget: give "
+                         "fact_device_bytes as well")
     if knn_device_bytes is not None and not incremental:
         raise ValueError("accelerate(knn_device_bytes=...) bounds the resident synonymy KNN index, which only "
                          "incremental=True keeps")
@@ -292,6 +300,8 @@ def accelerate(rag, device: int = 0, engine: Optional[Engine] = None, filter_wor
         state["mutable_set"] = incremental
         if fact_device_bytes is not None:     # before every load, which is what applies it
             state["engine"].set_fact_memory(fact_device_bytes)
+            if fact_lo_on_host:
+                state["engine"].set_fact_placement(True)
         if knn_device_bytes is not None:      # before every KNN index update, which is what applies it
             state["engine"].knn_set_memory(knn_device_bytes)
         return state["engine"]

@@ -24,6 +24,7 @@ int split_queries(hrag_t* h, const float* dQ, int Bq, cudaStream_t s) {
 
 // n_ctas: persistent CTAs of the tensor-core GEMM (h->num_sms unless it shares the GPU with PPR sweeps)
 int sim_dispatch(hrag_t* h, const float* dQ, int Bq, int which, float* S, int64_t ldS, cudaStream_t s, int n_ctas) {
+    HRAG_CHECK(which == 1 || !h->fplanes.held(), "internal: sim_dispatch on fact planes in host memory");
     if (h->sim_mode == HRAG_SIM_FP32 || h->emb[which].hi.p == nullptr) {   // dim % 8 != 0 has no TMA layout
         HRAG_CHECK(h->emb[which].f32 != nullptr, "similarity: the fp32 embedding matrix was not kept (streamed upload); "
                                                  "only the tensor-core modes are available");
@@ -67,7 +68,7 @@ int fact_norms_update(hrag_t* h, int64_t row0, int64_t n, bool reset) {
 // Below 65,536 facts the split K2 takes a fraction of a millisecond per chunk and the screen's dozen extra launches
 // cost more than they save (MuSiQue-1k, 10,734 facts: 0.9 against 0.7 ms per 64-query step).
 constexpr int64_t kScreenMinFacts = 65536;
-static bool screened(const hrag_t* h) {
+bool screened(const hrag_t* h) {
     return h->world == 1 && h->sim_mode == HRAG_SIM_BF16X3 && !h->debug_exact_stage_a && h->emb[0].hi.p != nullptr &&
            h->emb[0].nmax.p != nullptr && h->emb[0].rows >= kScreenMinFacts;
 }
@@ -78,9 +79,10 @@ static bool screened(const hrag_t* h) {
 // gives over all facts, bit for bit (same query row, same column, same k sequence), and the candidates hold the k best
 // and the minimum, so the outputs are those of the exact path.  When the screen cannot prove that (a non-finite bound,
 // a cap overflowed, or a rescored score outside the bound) it raises scr.flag, and the gated exact path below reruns
-// the chunk and counts it.
-static int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, float* d_top_score,
-                            int* d_nvalid, cudaStream_t s, int n_ctas) {
+// the chunk and counts it.  With the lo plane in host memory the staged lo rows come from the mapped plane, and the
+// flag is the caller's (chunk_flag): fact_stream.cu reruns the flagged chunks with the lo plane streamed.
+int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, float* d_top_score, int* d_nvalid,
+                     cudaStream_t s, int n_ctas, int* chunk_flag, unsigned long long* lo_bytes) {
     const int64_t F = h->emb[0].rows;
     const int nt = sim_tc_n_tiles(F), mtiles = (int)ceil_div(Bq, 128), ST = kScreenStageTiles;
     auto& c = h->scr;
@@ -103,7 +105,10 @@ static int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_
     HRAG_TRY(c.st_S.ensure((size_t)Bq * ST * 256 * sizeof(float)));
     HRAG_TRY(c.flag.ensure(sizeof(int)));
     if (c.fallbacks.p == nullptr) HRAG_TRY(c.fallbacks.zeros(sizeof(unsigned long long)));
-    int* flag = c.flag.as<int>();
+    const bool lo_host = h->fplanes.lo_only();
+    HRAG_CHECK(lo_host == (chunk_flag != nullptr) && lo_host == (lo_bytes != nullptr),
+               "internal: screened_stage_a: a chunk flag and a byte count go with the lo plane in host memory");
+    int* flag = lo_host ? chunk_flag : c.flag.as<int>();
     const EmbMem& e = h->emb[0];
     const int dim = h->dim;
     {
@@ -126,8 +131,12 @@ static int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_
         HRAG_TRY(screen_stage(c.cand_ids.as<int>(), c.cand_n.as<int>(), c.sat.as<int>(), c.sat_n.as<int>(), Bq, F, ST,
                               c.pos_of.as<int>(), c.slot_ids.as<int>(), c.res_count.as<int>(), c.stage_count.as<int>(),
                               flag, s));
-        HRAG_TRY(screen_gather(c.slot_ids.as<int>(), c.stage_count.as<int>(), mtiles, ST, e.hi.p, e.lo.p, dim,
-                               c.st_hi.p, c.st_lo.p, s));
+        if (lo_host)
+            HRAG_TRY(screen_gather_mapped(c.slot_ids.as<int>(), c.stage_count.as<int>(), mtiles, ST, e.hi.p,
+                                          h->fplanes.lo_dev, dim, c.st_hi.p, c.st_lo.p, lo_bytes, s));
+        else
+            HRAG_TRY(screen_gather(c.slot_ids.as<int>(), c.stage_count.as<int>(), mtiles, ST, e.hi.p, e.lo.p, dim,
+                                   c.st_hi.p, c.st_lo.p, s));
     }
     {
         StageTimer tm(h, ST_SIM_FACT, s);
@@ -140,6 +149,7 @@ static int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_
                                c.pos_of.as<int>(), F, c.cand_ids.as<int>(), c.cand_s1.as<float>(), c.cand_n.as<int>(),
                                c.err.as<float>(), k, h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, flag, s));
     }
+    if (lo_host) return 0;
     // the exact path, run only when the flag is up (kernels that find it down return at once)
     {
         StageTimer tm(h, ST_SIM_FACT, s);
@@ -162,6 +172,7 @@ int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, flo
         HRAG_CUDA(cudaMemsetAsync(d_nvalid, 0, (size_t)Bq * sizeof(int), s));
         return 0;
     }
+    HRAG_CHECK(!h->fplanes.held(), "internal: dev_stage_a on fact planes in host memory (fact_stream_stage_a)");
     const int64_t ld = pad4(F);
     HRAG_TRY(h->mm_fact.ensure((size_t)Bq * sizeof(float2)));
     h->last_mm_rows = Bq;
@@ -360,7 +371,7 @@ int dev_stage_b_solve_f64(hrag_t* h, int Bq, const float* S, const float2* mm_pa
 // above it (C3 scan: G = 28 +121 ms per step, G = 44 +5 ms).  DESIGN.md section 4 K2 has the scans of G.
 int overlap_ctas(const hrag_t* h, int Bq, const SweepPlan& plan) {
     constexpr double kGemmFlopPerSmMs = 2.49e9, kScreenFlopPerSmMs = 0.66e9;
-    const bool screen = screened(h);
+    const bool screen = !h->fplanes.held() && screened(h);   // fact planes in host memory: stage A ran up front
     const double kSweepNnzPerMs = screen ? 4.20e7 : 3.80e7;
     const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
     const int64_t fact_rows = h->fplanes.held() ? 0 : h->emb[0].rows;   // streamed planes: stage A ran up front

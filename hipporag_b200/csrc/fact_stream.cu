@@ -11,7 +11,15 @@
 //
 // The ring walker (stream_slices, handle.h) and the fill (planes_fill) take any plane set (HostPlanes): the synonymy
 // KNN index streams its planes through them too when they exceed the hrag_knn_set_memory budget (knn_index.cu).
+//
+// HRAG_FACT_LO_ON_HOST keeps the hi plane resident and only the lo plane here, mapped (DESIGN.md section 7h).  Stage A
+// then runs the stage-A screen per query chunk (api.cu screened_stage_a): the hi.hi screen over the resident hi plane,
+// the staged candidates' lo rows read from the mapped plane by the gather.  One flag per chunk; after the call's
+// chunks the flags are read at once and a flagged chunk reruns the split K2 with hi in place and lo streamed through
+// the lo-only ring.  The routes that need every lo row stream the lo plane only (stream_slices' lo-only form).
 #include <algorithm>
+#include <cstring>
+#include <vector>
 
 #include "handle.h"
 
@@ -32,13 +40,18 @@ const char* kNoFp32 = "similarity: the fact planes are held in host memory (hrag
 
 }  // namespace
 
-int HostPlanes::alloc(size_t bytes, int64_t slice, int dim) {
+int HostPlanes::alloc(size_t bytes, int64_t slice, int dim, bool lo_only) {
     release();
-    HRAG_CUDA(cudaHostAlloc(&hi, bytes, cudaHostAllocDefault));
-    HRAG_CUDA(cudaHostAlloc(&lo, bytes, cudaHostAllocDefault));
+    if (lo_only) {
+        HRAG_CUDA(cudaHostAlloc(&lo, bytes, cudaHostAllocMapped));
+        HRAG_CUDA(cudaHostGetDevicePointer(&lo_dev, lo, 0));
+    } else {
+        HRAG_CUDA(cudaHostAlloc(&hi, bytes, cudaHostAllocDefault));
+        HRAG_CUDA(cudaHostAlloc(&lo, bytes, cudaHostAllocDefault));
+    }
     plane_bytes = bytes;
     slice_rows = slice;
-    HRAG_TRY(ring.ensure((size_t)2 * slice * dim * 4));
+    HRAG_TRY(ring.ensure((size_t)2 * slice * dim * (lo_only ? 2 : 4)));
     HRAG_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
     for (int i = 0; i < 2; ++i) {
         HRAG_CUDA(cudaEventCreateWithFlags(&loaded[i], cudaEventDisableTiming));
@@ -51,7 +64,7 @@ void HostPlanes::release() {
     if (copy) cudaStreamSynchronize(copy);
     if (hi) cudaFreeHost(hi);
     if (lo) cudaFreeHost(lo);
-    hi = lo = nullptr;
+    hi = lo = lo_dev = nullptr;
     plane_bytes = 0;
     slice_rows = 0;
     ring.reset();
@@ -88,24 +101,43 @@ int host_planes_plan(int64_t budget, const std::string& who, const char* setter,
     return 0;
 }
 
-int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows) {
+int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows,
+                     bool* lo_only) {
     *slice_rows = 0;
+    *lo_only = false;
     const int64_t plane_bytes = rows * (int64_t)dim * 4;   // hi + lo
     if (h->fact_budget <= 0 || plane_bytes <= h->fact_budget) return 0;
     HRAG_CHECK(h->world == 1, who + ": fact planes in host memory (hrag_set_fact_memory) serve one GPU only; a "
                                     "node-range-sharded handle (world > 1) keeps its fact slice resident");
     HRAG_CHECK(dim % 8 == 0, who + ": fact planes in host memory need dim % 8 == 0 (the tensor-core layout)");
-    return host_planes_plan(h->fact_budget, who, "hrag_set_fact_memory", rows, dim, slice_rows);
+    if (h->fact_placement != HRAG_FACT_LO_ON_HOST)
+        return host_planes_plan(h->fact_budget, who, "hrag_set_fact_memory", rows, dim, slice_rows);
+    // the hi plane resident, the rest of the budget a ring of two lo slices
+    const int64_t hi_bytes = rows * (int64_t)dim * 2, lo_row = (int64_t)dim * 2;
+    const int64_t slice = (h->fact_budget - hi_bytes) / (2 * lo_row) / kSliceAlign * kSliceAlign;
+    HRAG_CHECK(h->fact_budget >= hi_bytes && slice >= kSliceAlign,
+               who + ": HRAG_FACT_LO_ON_HOST keeps the hi fact plane of " + std::to_string(hi_bytes) +
+                   " bytes resident, and it with a lo ring of two 256-row slices (" +
+                   std::to_string(2 * kSliceAlign * lo_row) + " bytes) exceeds the hrag_set_fact_memory budget of " +
+                   std::to_string(h->fact_budget) + " bytes");
+    *slice_rows = slice;
+    *lo_only = true;
+    return 0;
 }
 
-int fact_planes_alloc(hrag_t* h, int64_t slice_rows) {
+int fact_planes_alloc(hrag_t* h, int64_t slice_rows, bool lo_only) {
     h->fplanes.release();
-    return h->fplanes.alloc((size_t)h->emb[0].rows * h->dim * 2, slice_rows, h->dim);
+    EmbMem& e = h->emb[0];
+    if (lo_only) {   // the resident hi plane and the norm maxima its fill raises from zero
+        HRAG_TRY(e.hi.ensure((size_t)e.rows * h->dim * 2));
+        HRAG_TRY(e.nmax.zeros(2 * sizeof(float)));
+    }
+    return h->fplanes.alloc((size_t)e.rows * h->dim * 2, slice_rows, h->dim, lo_only);
 }
 
 int planes_fill(hrag_t* h, HostPlanes& ps, int dim, int64_t row0, int64_t n, const float* src, bool src_on_device,
-                const BeforeWrite& before_write) {
-    const int64_t d = dim, S = ps.slice_rows;
+                const BeforeWrite& before_write, char* hi_dev) {
+    const int64_t d = dim, S = hi_dev ? ps.slice_rows / 2 : ps.slice_rows;   // rows per step
     char* stage = ps.ring.as<char>();
     char* split = stage + (size_t)S * d * 4;
     for (int64_t r = 0; r < n; r += S) {
@@ -116,12 +148,14 @@ int planes_fill(hrag_t* h, HostPlanes& ps, int dim, int64_t row0, int64_t n, con
             HRAG_CUDA(cudaMemcpyAsync(stage, x, ne * 4, cudaMemcpyHostToDevice, h->stream));
             x = reinterpret_cast<const float*>(stage);
         }
-        HRAG_TRY(split_bf16(x, (int64_t)ne, split, split + (size_t)S * d * 2, h->stream));
-        if (before_write) HRAG_TRY(before_write(r, m, split, split + (size_t)S * d * 2));
         const size_t at = (size_t)(row0 + r) * d * 2;
-        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(ps.hi) + at, split, ne * 2, cudaMemcpyDeviceToHost, h->stream));
-        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(ps.lo) + at, split + (size_t)S * d * 2, ne * 2,
-                                  cudaMemcpyDeviceToHost, h->stream));
+        char* hi = hi_dev ? hi_dev + at : split;   // lo_only: the hi rows go straight to the resident plane
+        char* lo = hi_dev ? split : split + (size_t)S * d * 2;
+        HRAG_TRY(split_bf16(x, (int64_t)ne, hi, lo, h->stream));
+        if (before_write) HRAG_TRY(before_write(r, m, hi, lo));
+        if (!hi_dev)
+            HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(ps.hi) + at, hi, ne * 2, cudaMemcpyDeviceToHost, h->stream));
+        HRAG_CUDA(cudaMemcpyAsync(static_cast<char*>(ps.lo) + at, lo, ne * 2, cudaMemcpyDeviceToHost, h->stream));
     }
     HRAG_CUDA(cudaStreamSynchronize(h->stream));
     return 0;
@@ -129,9 +163,16 @@ int planes_fill(hrag_t* h, HostPlanes& ps, int dim, int64_t row0, int64_t n, con
 
 // Ring half 0 stages up to slice_rows fp32 rows (slice_rows x dim x 4 bytes: exactly one half), half 1 takes their
 // split (hi rows, then lo rows), which goes back to the pinned planes.  split_bf16 is element-wise, so the planes are
-// byte for byte those of a resident load.
+// byte for byte those of a resident load.  lo_only: the hi rows go to the resident plane, and the split rows raise the
+// norm maxima, as fact_norms_update raises them over resident planes (a maximum: any order of rows gives its bits).
 int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool src_on_device) {
-    return planes_fill(h, h->fplanes, h->dim, row0, n, src, src_on_device);
+    FactPlanes& fp = h->fplanes;
+    if (!fp.lo_only()) return planes_fill(h, fp, h->dim, row0, n, src, src_on_device);
+    EmbMem& e = h->emb[0];
+    auto norms = [&](int64_t, int64_t m, const char* hi, const char* lo) {
+        return plane_norm_max(hi, lo, m, h->dim, e.nmax.as<unsigned int>(), h->stream);
+    };
+    return planes_fill(h, fp, h->dim, row0, n, src, src_on_device, norms, e.hi.as<char>());
 }
 
 // Queries per pass: their bf16 hi / lo splits (dim x 4 bytes each) stay on the device for the whole pass and are
@@ -142,13 +183,10 @@ int64_t fact_stream_pass_cap(const hrag_t* h) {
     return std::max<int64_t>(kPassChunk, (int64_t)kPassSplitBytes / per_query / kPassChunk * kPassChunk);
 }
 
-int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* d_top_idx,
-                        float* d_top_score, int* d_nvalid) {
+// The split K2 over every fact, the planes streamed once per pass (lo only when lo_only: hi is read in place).
+static int streamed_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* d_top_idx,
+                            float* d_top_score, int* d_nvalid) {
     FactPlanes& fp = h->fplanes;
-    HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, std::string("stage A ") + kNoFp32);
-    h->last_fact_rows = 0;
-    h->last_mm_rows = 0;
-    if (B == 0) return 0;
     const int64_t F = h->emb[0].rows, d = h->dim, S = fp.slice_rows;
     const int64_t n_slices = ceil_div(F, S);
     const bool fused = !h->keep_fact_scores && k <= kFusedK;
@@ -262,7 +300,7 @@ int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int 
             if (fused && s > 0) cur = 1 - cur;
             return 0;
         };
-        HRAG_TRY(stream_slices(h, fp, d, 0, F, n_seg == 4, body));
+        HRAG_TRY(stream_slices(h, fp, d, 0, F, n_seg == 4, body, fp.lo_only() ? h->emb[0].hi.as<char>() : nullptr));
         if (!fused) {
             StageTimer tm(h, ST_SEL_FACT);
             HRAG_TRY(topk_normalize((int)Bp, k, F, run_mm, d_top_idx + p0 * k, d_top_score + p0 * k, d_nvalid + p0,
@@ -270,6 +308,78 @@ int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int 
         }
     }
     return 0;
+}
+
+// Queries per screened chunk with the lo plane in host memory: the screen's partials (part_keys, part_low, part_mm)
+// take 88 bytes per query and 256-fact tile; the chunk keeps them within kLoHostPartialBytes in multiples of 128
+// queries (one m-tile), at most kPassChunk (the resident chunk): 1,024 at 2.75 M facts, 128 at 17 M.  A smaller chunk
+// reads the hi plane once more per chunk.
+constexpr int64_t kLoHostPartialBytes = int64_t(1) << 30;
+static int64_t lo_host_chunk(const hrag_t* h) {
+    const int64_t per_query = 88 * (int64_t)sim_tc_n_tiles(std::max<int64_t>(h->emb[0].rows, 1));
+    return std::min<int64_t>(kPassChunk, std::max<int64_t>(128, kLoHostPartialBytes / per_query / 128 * 128));
+}
+
+// The screen over chunks of lo_host_chunk queries, each raising its own flag; then the flags and the lo bytes the
+// gathers read are copied back at once (the one synchronise of the call), and each flagged chunk reruns exactly
+// (streamed_stage_a: the split K2, lo streamed) over its outputs and counts as a fallback.
+static int lo_host_screened_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* d_top_idx,
+                                    float* d_top_score, int* d_nvalid) {
+    const int64_t d = h->dim, chunk = lo_host_chunk(h), n_chunks = ceil_div(B, chunk);
+    const int n_ctas = h->debug_sim_ctas > 0 ? h->debug_sim_ctas : h->num_sms;
+    const size_t flag_bytes = sizeof(unsigned long long) + (size_t)n_chunks * sizeof(int);
+    HRAG_TRY(h->scr.call_flags.ensure(flag_bytes));
+    HRAG_TRY(h->mm_fact.ensure((size_t)std::min<int64_t>(chunk, B) * sizeof(float2)));
+    if (!q_on_device) HRAG_TRY(h->d_q.ensure((size_t)std::min<int64_t>(chunk, B) * d * 4));
+    unsigned long long* lo_bytes = h->scr.call_flags.as<unsigned long long>();
+    int* flags = reinterpret_cast<int*>(lo_bytes + 1);
+    HRAG_CUDA(cudaMemsetAsync(lo_bytes, 0, flag_bytes, h->stream));
+    auto chunk_queries = [&](int64_t q0, int nb, const float** x) -> int {   // device fp32 queries of the chunk
+        *x = q + (size_t)q0 * d;
+        if (!q_on_device) {
+            HRAG_TRY(h2d(h, h->d_q.p, *x, (size_t)nb * d * 4));
+            *x = h->d_q.as<float>();
+        }
+        return 0;
+    };
+    for (int64_t c = 0; c < n_chunks; ++c) {
+        const int64_t q0 = c * chunk;
+        const int nb = (int)std::min<int64_t>(chunk, B - q0);
+        const float* x = nullptr;
+        HRAG_TRY(chunk_queries(q0, nb, &x));
+        HRAG_TRY(screened_stage_a(h, nb, x, k, d_top_idx + q0 * k, d_top_score + q0 * k, d_nvalid + q0, h->stream,
+                                  n_ctas, flags + c, lo_bytes));
+    }
+    std::vector<char> host(flag_bytes);
+    HRAG_CUDA(cudaMemcpyAsync(host.data(), lo_bytes, flag_bytes, cudaMemcpyDeviceToHost, h->stream));
+    HRAG_CUDA(cudaStreamSynchronize(h->stream));
+    unsigned long long gathered = 0;
+    std::memcpy(&gathered, host.data(), sizeof(gathered));
+    h->stats.h2d_bytes += (int64_t)gathered;
+    for (int64_t c = 0; c < n_chunks; ++c) {
+        int flagged = 0;
+        std::memcpy(&flagged, host.data() + sizeof(gathered) + (size_t)c * sizeof(int), sizeof(int));
+        if (!flagged) continue;
+        const int64_t q0 = c * chunk;
+        const int nb = (int)std::min<int64_t>(chunk, B - q0);
+        const float* x = nullptr;
+        HRAG_TRY(chunk_queries(q0, nb, &x));
+        HRAG_TRY(streamed_stage_a(h, nb, x, true, k, d_top_idx + q0 * k, d_top_score + q0 * k, d_nvalid + q0));
+        h->stats.stage_a_fallbacks += 1;
+    }
+    h->last_mm_rows = n_chunks == 1 ? B : 0;   // mm_fact holds the one chunk's (min, max)
+    return 0;
+}
+
+int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* d_top_idx,
+                        float* d_top_score, int* d_nvalid) {
+    HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, std::string("stage A ") + kNoFp32);
+    h->last_fact_rows = 0;
+    h->last_mm_rows = 0;
+    if (B == 0) return 0;
+    if (h->fplanes.lo_only() && !h->keep_fact_scores && k <= kFusedK && screened(h))
+        return lo_host_screened_stage_a(h, B, q, q_on_device, k, d_top_idx, d_top_score, d_nvalid);
+    return streamed_stage_a(h, B, q, q_on_device, k, d_top_idx, d_top_score, d_nvalid);
 }
 
 // K2 writes a score tile up to its 256-column end, clipped at ldS columns from the pointer it is given.  A slice that
@@ -293,7 +403,7 @@ int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ld
                                         (size_t)ns * sizeof(float), (size_t)nb, cudaMemcpyDeviceToDevice, h->stream));
         return 0;
     };
-    return stream_slices(h, fp, h->dim, 0, F, n_seg == 4, body);
+    return stream_slices(h, fp, h->dim, 0, F, n_seg == 4, body, fp.lo_only() ? h->emb[0].hi.as<char>() : nullptr);
 }
 
 }  // namespace hrag
@@ -312,13 +422,26 @@ int hrag_set_fact_memory(hrag_t* h, int64_t max_device_bytes) {
     return 0;
 }
 
+int hrag_set_fact_placement(hrag_t* h, int placement) {
+    HRAG_CHECK(h, "hrag_set_fact_placement: null handle");
+    HRAG_CHECK(placement == HRAG_FACT_PLANES_BY_BUDGET || placement == HRAG_FACT_LO_ON_HOST,
+               "hrag_set_fact_placement: placement must be HRAG_FACT_PLANES_BY_BUDGET (0) or HRAG_FACT_LO_ON_HOST (1)");
+    HRAG_CHECK(h->world == 1 || placement == HRAG_FACT_PLANES_BY_BUDGET,
+               "hrag_set_fact_placement: fact planes in host memory serve one GPU only; a node-range-sharded handle "
+               "(world > 1) keeps its fact slice resident");
+    h->fact_placement = placement;
+    return 0;
+}
+
 int hrag_fact_planes_info(hrag_t* h, int* on_host, int64_t* slice_rows, int64_t* device_bytes, int64_t* host_bytes) {
     HRAG_CHECK(h && on_host && slice_rows && device_bytes && host_bytes, "hrag_fact_planes_info: null argument");
     const FactPlanes& fp = h->fplanes;
-    *on_host = fp.held() ? 1 : 0;
+    *on_host = fp.lo_only() ? 2 : fp.held() ? 1 : 0;
     *slice_rows = fp.slice_rows;
-    *device_bytes = fp.held() ? (int64_t)fp.ring.cap : (int64_t)(h->emb[0].hi.cap + h->emb[0].lo.cap);
-    *host_bytes = fp.held() ? 2 * (int64_t)fp.plane_bytes : 0;
+    *device_bytes = fp.lo_only() ? (int64_t)(h->emb[0].hi.cap + fp.ring.cap)
+                    : fp.held()  ? (int64_t)fp.ring.cap
+                                 : (int64_t)(h->emb[0].hi.cap + h->emb[0].lo.cap);
+    *host_bytes = fp.lo_only() ? (int64_t)fp.plane_bytes : fp.held() ? 2 * (int64_t)fp.plane_bytes : 0;
     return 0;
 }
 

@@ -9,7 +9,8 @@
 //   tables    passage_vid[P], fact_subj/obj[F], ent_chunk_count[N]                                         (resident)
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
 //             facts over the hrag_set_fact_memory budget: the planes in pinned host memory, and on the device a
-//             ring of two slices (fact_stream.cu) of at most the budget
+//             ring of two slices (fact_stream.cu) of at most the budget; under HRAG_FACT_LO_ON_HOST the hi plane
+//             resident, the lo plane in mapped pinned host memory and a ring of two lo slices
 //   shared    with hrag_index_export / hrag_index_attach the graph planes (but seg_partial), the tables and the embedding
 //             planes of an attached handle are the owner's allocations, mapped through CUDA IPC (index_share.cu)
 //   knn       self-KNN index (knn_index.cu): bf16 hi/lo [entities, d] x 2, ids / scores [entities, pad4(kmax + 1)]
@@ -130,8 +131,11 @@ struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passag
 // slice_rows rows of hi then lo (fact_stream.cu): the fact planes over the hrag_set_fact_memory budget (FactPlanes) and
 // the synonymy KNN planes over the hrag_knn_set_memory budget (KnnIndex::host).  `copy` carries the ring uploads;
 // loaded[i] marks half i filled, freed[i] the last read of half i on `stream`.  Owned and move-only: freed by release().
+// lo_only (the fact planes under HRAG_FACT_LO_ON_HOST): no hi plane here (the caller keeps it resident), lo is mapped
+// (lo_dev: its device address, which kernels read over PCIe) and a ring half holds lo [slice_rows, dim] only.
 struct HostPlanes {
     void *hi = nullptr, *lo = nullptr;   // pinned (cudaHostAlloc)
+    void* lo_dev = nullptr;              // lo_only: the device address of lo (cudaHostGetDevicePointer)
     size_t plane_bytes = 0;              // of one of them (the capacity)
     int64_t slice_rows = 0;              // a multiple of 256, the K2 tile width
     Buf ring;                            // 2 halves, each hi [slice_rows, dim] then lo [slice_rows, dim] bf16
@@ -145,14 +149,16 @@ struct HostPlanes {
     }
     ~HostPlanes() { release(); }
     void swap(HostPlanes& o) noexcept {
-        std::swap(hi, o.hi); std::swap(lo, o.lo); std::swap(plane_bytes, o.plane_bytes);
+        std::swap(hi, o.hi); std::swap(lo, o.lo); std::swap(lo_dev, o.lo_dev); std::swap(plane_bytes, o.plane_bytes);
         std::swap(slice_rows, o.slice_rows); std::swap(ring, o.ring); std::swap(copy, o.copy);
         std::swap(loaded, o.loaded); std::swap(freed, o.freed);
     }
-    // pinned planes of `bytes` each (contents lost), a ring of two `slice`-row halves at `dim`, the copy stream
-    int alloc(size_t bytes, int64_t slice, int dim);
+    // pinned planes of `bytes` each (contents lost), a ring of two `slice`-row halves at `dim`, the copy stream;
+    // lo_only: the mapped lo plane only, and lo-only ring halves
+    int alloc(size_t bytes, int64_t slice, int dim, bool lo_only = false);
     void release();
-    bool held() const { return hi != nullptr; }
+    bool held() const { return lo != nullptr; }                    // some plane is in host memory
+    bool lo_only() const { return lo != nullptr && hi == nullptr; }
 };
 
 // The resident self-KNN index (knn_index.cu), independent of the retrieval index: the bf16 hi / lo planes of its unit
@@ -171,7 +177,9 @@ struct KnnIndex {
 constexpr int kKnnComplete = 1, kKnnRefill = 2;
 
 // Fact planes held in pinned host memory (hrag_set_fact_memory with a budget below rows x dim x 4 bytes;
-// fact_stream.cu): byte for byte what a resident load builds, plus the per-pass state of a streamed stage A.
+// fact_stream.cu): byte for byte what a resident load builds, plus the per-pass state of a streamed stage A.  held():
+// the fact planes are not all resident, so stage A runs for a whole call at once (fact_stream_stage_a); lo_only():
+// HRAG_FACT_LO_ON_HOST placed them, the hi plane is emb[0].hi and only lo is here.
 struct FactPlanes : HostPlanes {
     // a pass's per-query state: fused, (min, max) [3, B] and 8 keys [3, B, 8] (two running slots and this slice's);
     // materialised, the running (min, max) [B] and one chunk's slice top-k sl_ids / sl_scores [chunk, k], sl_mm
@@ -257,6 +265,7 @@ struct hrag_handle {
     hrag::TableMem tables;
     hrag::EmbMem emb[2];
     int64_t fact_budget = 0;           // hrag_set_fact_memory: device bytes the fact planes may take (0 = no limit)
+    int fact_placement = HRAG_FACT_PLANES_BY_BUDGET;   // hrag_set_fact_placement: applied by the next fact load
     hrag::FactPlanes fplanes;          // the fact planes in pinned host memory when they exceed fact_budget
     hrag::KnnIndex knn;                // hrag_knn_index_update: the synonymy KNN of the entities, kept between calls
     int64_t knn_budget = 0;            // hrag_knn_set_memory: device bytes the KNN planes may take (0 = no limit)
@@ -308,10 +317,11 @@ struct hrag_handle {
     // m-tile pos_of [m, F], slot_ids [m, 48, 256], res_count [m, 256], stage_count [m], the staging planes st_hi / st_lo
     // [m * 48 * 256, d] and the rescored scores st_S [Bq, 48 * 256]; flag: this chunk falls back; fallbacks: counted
     // on the device, drained into stats by resolve_spans.  About 0.6 GB at C3 (F = 2.75 M, d = 768), on top of the
-    // fused buffers and outside the hrag_set_fact_memory budget
+    // fused buffers and outside the hrag_set_fact_memory budget.  lo on the host (fact_stream.cu): call_flags holds
+    // the lo bytes the gathers read (uint64) and then one flag per query chunk of the call (int32)
     struct {
         hrag::Buf err, part_low, cand_ids, cand_s1, cand_n, sat, sat_n, pos_of, slot_ids, res_count, stage_count,
-            st_hi, st_lo, st_S, flag, fallbacks;
+            st_hi, st_lo, st_S, flag, fallbacks, call_flags;
     } scr;
     hrag::Buf fs_top_idx, fs_top_score, fs_nvalid;   // hrag_retrieve_resident on host fact planes: stage A [B, k]
     hrag::Buf d_q, d_q2, d_top_idx, d_top_score, d_nvalid, d_kept_idx, d_kept_score, d_dpr, d_out_ids, d_out_scores;
@@ -457,39 +467,47 @@ int gather_rows(hrag_t* h, const void* base, size_t row_bytes, const int* row_sr
 // rejected with a message naming `who` and the entry that set the budget, `setter`.
 int host_planes_plan(int64_t budget, const std::string& who, const char* setter, int64_t rows, int dim,
                      int64_t* slice_rows);
-// fact_planes_plan, before a fact load touches the handle: host_planes_plan of the fact budget; rejects sharded
-// handles and dim % 8 != 0.  fact_planes_alloc, after reset_embeddings: the pinned planes and the ring for the
-// handle's fact rows.
-int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows);
-int fact_planes_alloc(hrag_t* h, int64_t slice_rows);
+// fact_planes_plan, before a fact load touches the handle: host_planes_plan of the fact budget, or under
+// HRAG_FACT_LO_ON_HOST the lo ring's slice rows (*lo_only set); rejects sharded handles and dim % 8 != 0.
+// fact_planes_alloc, after reset_embeddings: the pinned planes and the ring for the handle's fact rows, and under
+// lo_only the resident hi plane and the zeroed norm maxima as well.
+int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows,
+                     bool* lo_only);
+int fact_planes_alloc(hrag_t* h, int64_t slice_rows, bool lo_only);
 // Fills host plane rows [row0, row0 + n) of `ps` (dim wide) from fp32 rows (host or device): ring half 0 stages up to
 // slice_rows fp32 rows, half 1 takes their split, which goes back to the pinned planes.  before_write(r, m, hi, lo),
 // when given, runs on `stream` after rows [row0 + r, row0 + r + m) are split into hi / lo (ring half 1) and before they
-// are written back; half 0 is free then.  Returns once the rows are written.
+// are written back; half 0 is free then.  Returns once the rows are written.  lo_only planes: hi_dev is the resident
+// hi plane, which takes the hi rows directly; a step is slice_rows / 2 rows, the lo ring's bytes.
 using BeforeWrite = std::function<int(int64_t r, int64_t m, const char* hi, const char* lo)>;
 int planes_fill(hrag_t* h, HostPlanes& ps, int dim, int64_t row0, int64_t n, const float* src, bool src_on_device,
-                const BeforeWrite& before_write = nullptr);
+                const BeforeWrite& before_write = nullptr, char* hi_dev = nullptr);
 int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool src_on_device);
 // Walks rows [row0, row1) of the host planes `ps` (dim wide) on `stream`, in slices of slice_rows from row0:
 // body(s, first row, rows, hi, lo) reads slice s from its ring half while the copy stream fills the other half with
 // slice s + 1.  `both`: stream the lo plane too (HRAG_SIM_BF16 reads only hi).  Every copy is joined into `stream`
-// before its slice is read, so the caller's later work on `stream` sees the whole walk.
+// before its slice is read, so the caller's later work on `stream` sees the whole walk.  Lo-only form (ps.lo_only(),
+// hi_dev = the resident hi plane): only lo streams, and body reads hi in place (lo = hi when !both: nothing streams).
 template <class Body>
-int stream_slices(hrag_t* h, HostPlanes& ps, int64_t dim, int64_t row0, int64_t row1, bool both, Body body) {
+int stream_slices(hrag_t* h, HostPlanes& ps, int64_t dim, int64_t row0, int64_t row1, bool both, Body body,
+                  const char* hi_dev = nullptr) {
     const int64_t S = ps.slice_rows, n_slices = ceil_div(row1 - row0, S);
-    const size_t half_bytes = (size_t)S * dim * 4;
+    const bool lo_only = hi_dev != nullptr;
+    const size_t half_bytes = (size_t)S * dim * (lo_only ? 2 : 4);
     char* ring = ps.ring.as<char>();
     auto copy = [&](int64_t s) -> int {
         const int64_t r0 = row0 + s * S, n = std::min(S, row1 - r0);
         const int half = (int)(s & 1);
         char* dst = ring + half * half_bytes;
         HRAG_CUDA(cudaStreamWaitEvent(ps.copy, ps.freed[half], 0));   // the last read of this half is done
-        HRAG_CUDA(cudaMemcpyAsync(dst, static_cast<char*>(ps.hi) + (size_t)r0 * dim * 2, (size_t)n * dim * 2,
-                                  cudaMemcpyHostToDevice, ps.copy));
+        if (!lo_only)
+            HRAG_CUDA(cudaMemcpyAsync(dst, static_cast<char*>(ps.hi) + (size_t)r0 * dim * 2, (size_t)n * dim * 2,
+                                      cudaMemcpyHostToDevice, ps.copy));
         if (both)
-            HRAG_CUDA(cudaMemcpyAsync(dst + (size_t)S * dim * 2, static_cast<char*>(ps.lo) + (size_t)r0 * dim * 2,
-                                      (size_t)n * dim * 2, cudaMemcpyHostToDevice, ps.copy));
-        h->stats.h2d_bytes += (int64_t)n * dim * 2 * (both ? 2 : 1);
+            HRAG_CUDA(cudaMemcpyAsync(dst + (lo_only ? 0 : (size_t)S * dim * 2),
+                                      static_cast<char*>(ps.lo) + (size_t)r0 * dim * 2, (size_t)n * dim * 2,
+                                      cudaMemcpyHostToDevice, ps.copy));
+        h->stats.h2d_bytes += (int64_t)n * dim * 2 * ((lo_only ? 0 : 1) + (both ? 1 : 0));
         HRAG_CUDA(cudaEventRecord(ps.loaded[half], ps.copy));
         return 0;
     };
@@ -500,9 +518,11 @@ int stream_slices(hrag_t* h, HostPlanes& ps, int64_t dim, int64_t row0, int64_t 
         if (s + 1 < n_slices) HRAG_TRY(copy(s + 1));
         const int half = (int)(s & 1);
         HRAG_CUDA(cudaStreamWaitEvent(h->stream, ps.loaded[half], 0));
-        const char* e_hi = ring + half * half_bytes;
         const int64_t r0 = row0 + s * S;
-        HRAG_TRY(body(s, r0, std::min(S, row1 - r0), e_hi, e_hi + (size_t)S * dim * 2));
+        const char* h_half = ring + half * half_bytes;
+        const char* e_hi = lo_only ? hi_dev + (size_t)r0 * dim * 2 : h_half;
+        const char* e_lo = lo_only ? (both ? h_half : e_hi) : h_half + (size_t)S * dim * 2;
+        HRAG_TRY(body(s, r0, std::min(S, row1 - r0), e_hi, e_lo));
         HRAG_CUDA(cudaEventRecord(ps.freed[half], h->stream));
     }
     return 0;
@@ -514,6 +534,14 @@ int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int 
 // Raw fact scores of nb (<= 1024) device queries into S [nb, ldS], the planes streamed once.
 int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ldS);
 int64_t fact_stream_pass_cap(const hrag_t* h);
+
+// api.cu: the stage-A screen on one query chunk.  screened(h): the screen applies to this handle's facts.
+// screened_stage_a: Bq <= 1024 queries (fp32 on the device); with the lo plane in host memory (h->fplanes.lo_only())
+// it gathers the staged lo rows from the mapped plane, adds their bytes to *lo_bytes, raises *chunk_flag instead of
+// running the gated exact path (the caller reruns a flagged chunk) and counts no fallback.
+bool screened(const hrag_t* h);
+int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, float* d_top_score, int* d_nvalid,
+                     cudaStream_t s, int n_ctas, int* chunk_flag = nullptr, unsigned long long* lo_bytes = nullptr);
 
 // api.cu: emb[0].nmax (reset to 0 first when `reset`) raised to the row norms of fact plane rows [row0, row0 + n), on
 // `stream`.  Every writer of resident fact planes calls it, so nmax bounds every row the stage-A screen scores.

@@ -570,9 +570,10 @@ int hrag_debug_index(hrag_t* h, int plane, void* host_out, int64_t max_bytes, in
     const SeedTables& t = h->t;
     const EdgeList& E = h->graph.edges;
     const int64_t d = h->dim, F = h->emb[0].rows, P = h->emb[1].rows;
-    const bool host = h->fplanes.held();   // fact planes in pinned host memory (hrag_set_fact_memory)
+    // fact planes in pinned host memory (hrag_set_fact_memory): both, or lo only (the hi plane stays resident)
+    const bool host = h->fplanes.held(), host_hi = host && !h->fplanes.lo_only();
     const void* src[13] = {t.passage_vid, t.fact_subj_vid, t.fact_obj_vid, t.ent_chunk_count,
-                           host ? h->fplanes.hi : h->emb[0].hi.p, host ? h->fplanes.lo : h->emb[0].lo.p,
+                           host_hi ? h->fplanes.hi : h->emb[0].hi.p, host ? h->fplanes.lo : h->emb[0].lo.p,
                            h->emb[1].hi.p, h->emb[1].lo.p,
                            h->emb[0].f32, h->emb[1].f32, E.src.p, E.dst.p, E.w.p};
     const int64_t bytes[13] = {4 * (int64_t)t.n_passages, 4 * t.n_facts, 4 * t.n_facts,

@@ -191,6 +191,11 @@ int screen_stage(const int* cand_ids, const int* cand_n, const int* sat, const i
                  cudaStream_t stream);
 int screen_gather(const int* slot_ids, const int* stage_count, int m_tiles, int stage_tiles, const void* e_hi,
                   const void* e_lo, int dim, void* st_hi, void* st_lo, cudaStream_t stream);
+// screen_gather with the lo rows from a mapped pinned host plane (the device address of cudaHostAllocMapped memory),
+// read over PCIe; adds the lo bytes it reads to *lo_bytes (device).
+int screen_gather_mapped(const int* slot_ids, const int* stage_count, int m_tiles, int stage_tiles, const void* e_hi,
+                         const void* lo_mapped, int dim, void* st_hi, void* st_lo, unsigned long long* lo_bytes,
+                         cudaStream_t stream);
 // the outputs of merge_minmax_topk over the rescored staged columns (F facts), after the |s4 - s1| check
 int screen_finish(const float* S, int rows, int stage_tiles, const int* slot_ids, const int* stage_count,
                   const int* pos_of, int64_t F, const int* cand_ids, const float* cand_s1, const int* cand_n,

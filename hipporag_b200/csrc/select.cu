@@ -583,6 +583,52 @@ k_screen_gather(const int* __restrict__ slot_ids, const int* __restrict__ stage_
     }
 }
 
+// 16 bytes of host memory through a plain global load: the mapped lo plane is read over PCIe, where a non-coherent
+// (texture-path) load has nothing to gain
+__device__ __forceinline__ uint4 ld_global_u4(const uint4* p) {
+    uint4 v;
+    asm("ld.global.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
+    return v;
+}
+
+// k_screen_gather with the lo rows read from the mapped pinned lo plane (HRAG_FACT_LO_ON_HOST): one warp per staged
+// slot, zeros for an empty slot, the hi row from the resident plane.  A lane issues all of its 16-byte loads of a lo
+// row (up to 8 at a time: dim <= 2048 in one round) before it stores them, so every warp keeps a whole row in flight over PCIe
+// (64 warps per SM: about 100 KB per SM at dim 768).  *lo_bytes counts the lo bytes read, once per CTA.
+constexpr int kGatherInFlight = 8;
+__global__ void __launch_bounds__(256)
+k_screen_gather_mapped(const int* __restrict__ slot_ids, const int* __restrict__ stage_count, int stage_tiles,
+                       const uint4* __restrict__ e_hi, const uint4* e_lo, int dim, uint4* __restrict__ st_hi,
+                       uint4* __restrict__ st_lo, unsigned long long* __restrict__ lo_bytes) {
+    __shared__ int s_rows;
+    const int slot = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31, mt = blockIdx.y;
+    if (threadIdx.x == 0) s_rows = 0;
+    __syncthreads();
+    if (slot / 256 < __ldg(stage_count + mt)) {
+        const size_t r = (size_t)mt * stage_tiles * 256 + slot;
+        const int id = __ldg(slot_ids + r);
+        const int n16 = dim / 8;
+        if (id < 0) {
+            for (int i = lane; i < n16; i += 32) st_hi[r * n16 + i] = st_lo[r * n16 + i] = make_uint4(0u, 0u, 0u, 0u);
+        } else {
+            const uint4* src = e_lo + (size_t)id * n16;
+            for (int i0 = lane; i0 < n16; i0 += 32 * kGatherInFlight) {
+                uint4 v[kGatherInFlight];
+#pragma unroll
+                for (int j = 0; j < kGatherInFlight; ++j)
+                    if (i0 + 32 * j < n16) v[j] = ld_global_u4(src + i0 + 32 * j);
+#pragma unroll
+                for (int j = 0; j < kGatherInFlight; ++j)
+                    if (i0 + 32 * j < n16) st_lo[r * n16 + i0 + 32 * j] = v[j];
+            }
+            for (int i = lane; i < n16; i += 32) st_hi[r * n16 + i] = __ldg(e_hi + (size_t)id * n16 + i);
+            if (lane == 0) atomicAdd(&s_rows, 1);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0 && s_rows) atomicAdd(lo_bytes, (unsigned long long)s_rows * dim * 2);
+}
+
 // One CTA per query: the exact min / max and k best over the rescored staged columns of its m-tile (every candidate
 // is there, with the bits K2 gives it), after checking |s4 - s1| <= E_q on each listed candidate.
 __global__ void __launch_bounds__(kSelThreads)
@@ -653,6 +699,19 @@ int screen_gather(const int* slot_ids, const int* stage_count, int m_tiles, int 
     k_screen_gather<<<dim3((unsigned)(stage_tiles * 256 / 8), (unsigned)m_tiles), 256, 0, stream>>>(
         slot_ids, stage_count, stage_tiles, static_cast<const uint4*>(e_hi), static_cast<const uint4*>(e_lo), dim,
         static_cast<uint4*>(st_hi), static_cast<uint4*>(st_lo));
+    count_launch(1);
+    HRAG_CUDA(cudaGetLastError());
+    return 0;
+}
+
+int screen_gather_mapped(const int* slot_ids, const int* stage_count, int m_tiles, int stage_tiles, const void* e_hi,
+                         const void* lo_mapped, int dim, void* st_hi, void* st_lo, unsigned long long* lo_bytes,
+                         cudaStream_t stream) {
+    HRAG_CHECK(dim % 8 == 0, "screen_gather_mapped: dim must be a multiple of 8");
+    if (m_tiles == 0) return 0;
+    k_screen_gather_mapped<<<dim3((unsigned)(stage_tiles * 256 / 8), (unsigned)m_tiles), 256, 0, stream>>>(
+        slot_ids, stage_count, stage_tiles, static_cast<const uint4*>(e_hi), static_cast<const uint4*>(lo_mapped),
+        dim, static_cast<uint4*>(st_hi), static_cast<uint4*>(st_lo), lo_bytes);
     count_launch(1);
     HRAG_CUDA(cudaGetLastError());
     return 0;

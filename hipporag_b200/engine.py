@@ -123,8 +123,14 @@ def _stage_b_inputs(q_pass, kept_idx, kept_score, dpr_only):
 class Engine:
     """One handle = one H100.  Not thread-safe (like the reference's ``HippoRAG`` object)."""
 
-    def __init__(self, device: int = 0, shard_mode: int = 0, mutable: bool = False, fact_device_bytes: int = 0):
-        """``fact_device_bytes`` > 0 caps the device memory of the fact planes (``set_fact_memory``)."""
+    def __init__(self, device: int = 0, shard_mode: int = 0, mutable: bool = False, fact_device_bytes: int = 0,
+                 fact_lo_on_host: bool = False):
+        """``fact_device_bytes`` > 0 caps the device memory of the fact planes (``set_fact_memory``);
+        ``fact_lo_on_host`` keeps the hi plane resident and only the lo plane on the host when they exceed it
+        (``set_fact_placement``)."""
+        if fact_lo_on_host and not fact_device_bytes:
+            raise ValueError("Engine(fact_lo_on_host=True) places the fact planes under a device budget: give "
+                             "fact_device_bytes > 0 as well")
         self._lib = _lib.load()
         self._h = C.c_void_p()
         dev = (C.c_int * 1)(device)
@@ -133,6 +139,8 @@ class Engine:
             self.set_mutable()
         if fact_device_bytes:
             self.set_fact_memory(fact_device_bytes)
+        if fact_lo_on_host:
+            self.set_fact_placement(True)
         self.device = device
         self.rank, self.world = 0, 1
         self.n_nodes = 0
@@ -245,9 +253,18 @@ class Engine:
         device fact embeddings, ``knn_threshold`` on the facts and in-place updates."""
         _lib.check(self._lib.hrag_set_fact_memory(self._h, int(max_device_bytes)))
 
+    def set_fact_placement(self, lo_on_host: bool):
+        """Before the fact embeddings are loaded: where fact planes over the ``set_fact_memory`` budget go
+        (``hrag_set_fact_placement``).  ``False`` (the default): both planes in pinned host memory.  ``True``: the hi
+        plane stays resident and only the lo plane goes to pinned host memory; stage A then runs the stage-A screen
+        on the resident hi plane and reads only the staged candidates' lo rows over PCIe, with results bit for bit
+        those of resident planes.  A budget below the hi plane plus two 256-row lo slices fails the load."""
+        _lib.check(self._lib.hrag_set_fact_placement(self._h, 1 if lo_on_host else 0))
+
     def fact_planes_info(self) -> dict:
-        """Where the last fact load put the planes: ``on_host``, the ring's ``slice_rows`` (0 when resident), the
-        planes' ``device_bytes`` (the ring when on the host) and the pinned ``host_bytes``."""
+        """Where the last fact load put the planes: ``on_host`` (0 resident, 1 both planes on the host, 2 the lo
+        plane only), the ring's ``slice_rows`` (0 when resident), the planes' ``device_bytes`` (the ring, plus the hi
+        plane when only lo is on the host) and the pinned ``host_bytes``."""
         on_host, slice_rows, dev, host = C.c_int(), C.c_int64(), C.c_int64(), C.c_int64()
         _lib.check(self._lib.hrag_fact_planes_info(self._h, C.byref(on_host), C.byref(slice_rows), C.byref(dev),
                                                    C.byref(host)))

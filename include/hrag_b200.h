@@ -165,9 +165,35 @@ int hrag_set_fact_memory(hrag_t* h, int64_t max_device_bytes);
  * scratch at the first stage-A call (one GPU, HRAG_SIM_BF16X3): about 0.6 GB at 2.75 M facts x 768 for a
  * 1,024-query chunk (per m-tile staging planes 48 x 256 x d x 4 bytes, per query and 256-fact tile 16 bytes, per
  * m-tile and fact 4 bytes). */
-/* What the last fact load chose: on_host (1 = pinned host planes), the ring's slice_rows (0 when resident), the
- * device bytes of the fact planes (the ring, or the resident planes) and the pinned host bytes (0 when resident). */
+/* What the last fact load chose: on_host (1 = pinned host planes, 2 = hi plane resident and lo plane in pinned host
+ * memory, see hrag_set_fact_placement), the ring's slice_rows (0 when resident), the device bytes of the fact planes
+ * (the ring, the resident planes, or the hi plane plus the lo ring) and the pinned host bytes (0 when resident). */
 int hrag_fact_planes_info(hrag_t* h, int* on_host, int64_t* slice_rows, int64_t* device_bytes, int64_t* host_bytes);
+
+/* Where a fact load puts the planes when they exceed the hrag_set_fact_memory budget; set before the fact embeddings
+ * are loaded and applied by every later fact load.  HRAG_FACT_PLANES_BY_BUDGET (the default) is the rule above.
+ * HRAG_FACT_LO_ON_HOST keeps the hi plane resident and only the lo plane in library-owned pinned host memory (mapped,
+ * so kernels read it over PCIe):
+ *   - planes within the budget, or budget 0: resident, as by default;
+ *   - else, when the hi plane (rows x dim x 2 bytes) plus a lo ring of two 256-row slices (2 x 256 x dim x 2 bytes)
+ *     fit the budget: hi resident, lo on the host, and a ring of two lo slices, each the largest multiple of 256 rows
+ *     that fits the rest of the budget (hrag_fact_planes_info: on_host = 2);
+ *   - else the load fails, naming the hi plane's bytes and the budget (nothing falls back to both planes on the host).
+ * Stage A then runs the stage-A screen (one GPU, HRAG_SIM_BF16X3, >= 65,536 facts, linking_top_k <= 8): the hi.hi
+ * screen reads the resident hi plane, and only the lo rows of the staged candidates cross PCIe (counted in
+ * h2d_bytes).  A query chunk whose screen cannot prove its candidates reruns the split product with the lo plane
+ * streamed through the ring (stage_a_fallbacks counts it).  Every other route that needs every lo row (fewer than
+ * 65,536 facts, linking_top_k > 8, hrag_debug_keep_scores, hrag_debug_exact_stage_a, hrag_similarity /
+ * hrag_topk_similarity with which = 0) streams the lo plane only; HRAG_SIM_BF16 reads nothing from the host.  The
+ * outputs are byte for byte those of resident planes.  Rejected as with host planes: fact rows on the device for
+ * hrag_load_embeddings, HRAG_SIM_FP32 for the facts, hrag_knn_threshold (which = 0), the update entries,
+ * hrag_index_export, and sharded handles (world > 1).  The budget does not cover the screen's scratch (staging planes,
+ * per m-tile and fact 4 bytes) nor its per-chunk partials, 88 bytes per query and 256-fact tile, which grow with the
+ * fact count: under this placement the screen's query chunk is the largest multiple of 128 (at most 1,024) whose
+ * partials stay within 1 GB, 1,024 queries at 2.75 M facts, 128 at 17 M. */
+#define HRAG_FACT_PLANES_BY_BUDGET 0
+#define HRAG_FACT_LO_ON_HOST       1
+int hrag_set_fact_placement(hrag_t* h, int placement);
 
 /* Incremental updates of a loaded index: what HippoRAG.index() (HippoRAG.py:262-335: the stores append, igraph
  * add_vertices / add_edges, :1187, :1220) and HippoRAG.delete() (:337-411: the stores pop in place, igraph

@@ -56,6 +56,26 @@ f.stage_a(qf, 5)
 f.stage_a(qf, 10)
 f.similarity(0, qf[:3])
 f.topk_similarity(0, qf[:3], 40)
+# the hi fact plane resident and the lo plane in mapped pinned host memory (HRAG_FACT_LO_ON_HOST): the screen with its
+# lo gather over PCIe (k = 5), a chunk that falls back (copies of row 1024 in 12 tiles saturate more tiles than a query
+# may list) and reruns with the lo plane streamed, the streamed k = 10 path and similarity(0)
+F2 = 65_536 + 37
+rng = np.random.default_rng(6)
+fe2 = rng.standard_normal((F2, d)).astype(np.float32)
+fe2 /= np.linalg.norm(fe2, axis=1, keepdims=True)
+for t in range(4, 16):
+    fe2[t * 256:t * 256 + 10] = fe2[1024]
+q2 = fe2[rng.integers(4096, F2, 40)] + 0.05 * rng.standard_normal((40, d)).astype(np.float32)
+s = hb.Engine(0, fact_device_bytes=F2 * d * 2 + 2 * 256 * d * 2, fact_lo_on_host=True)
+s.load_embeddings(fe2, pe)
+assert s.fact_planes_info()["on_host"] == 2
+s.stage_a(q2, 5)
+q2[7] = fe2[1024]
+s.reset_stats()
+s.stage_a(q2, 5)
+assert s.stats()["stage_a_fallbacks"] == 1
+s.stage_a(q2, 10)
+s.similarity(0, q2[:3])
 print("driver ok", ids.shape)
 PY
 compute-sanitizer --tool $TOOL --error-exitcode 7 python /tmp/hrag_sanitize_driver.py 2>&1 | tail -15
