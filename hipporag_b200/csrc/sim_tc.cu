@@ -171,6 +171,33 @@ __device__ __forceinline__ uint64_t acc_rank_key(float f, uint32_t idx) {
     asm("mov.b32 %0, %1;" : "=r"(u) : "f"(f));
     return rank_key(__uint_as_float(u), idx);
 }
+// The accumulator register of bit b of a row half's pass mask (bit 2 j + c = register 4 j + 2 h + c, column
+// 8 j + 2 (lane % 4) + c), picked by a switch so that the rare insert path below is compiled once, not once per column.
+__device__ __forceinline__ float acc_at(const float (&d)[128], int h, int b) {
+    switch (b) {
+#define HRAG_ACC_CASE(i) case i: return d[4 * ((i) >> 1) + 2 * h + ((i) & 1)];
+#define HRAG_ACC_CASE8(i) HRAG_ACC_CASE(i) HRAG_ACC_CASE(i + 1) HRAG_ACC_CASE(i + 2) HRAG_ACC_CASE(i + 3) \
+                          HRAG_ACC_CASE(i + 4) HRAG_ACC_CASE(i + 5) HRAG_ACC_CASE(i + 6) HRAG_ACC_CASE(i + 7)
+        HRAG_ACC_CASE8(0) HRAG_ACC_CASE8(8) HRAG_ACC_CASE8(16) HRAG_ACC_CASE8(24)
+        HRAG_ACC_CASE8(32) HRAG_ACC_CASE8(40) HRAG_ACC_CASE8(48) HRAG_ACC_CASE8(56)
+#undef HRAG_ACC_CASE8
+#undef HRAG_ACC_CASE
+        default: return 0.f;
+    }
+}
+// best <- the 8 best of best and the keys of the columns set in `pass` (column of bit b: col0 + 8 (b >> 1) + (b & 1)).
+// The 8 best of a set of keys do not depend on the order they are inserted in, so the epilogues first mark the
+// columns that pass their gate and insert them afterwards in one loop: inserting under each column, unrolled over the
+// tile, made the epilogue too large for the instruction cache.
+__device__ __forceinline__ void insert_passing(const float (&d)[128], int h, uint64_t pass, uint32_t col0,
+                                               uint64_t (&best)[kFuseK]) {
+#pragma unroll 1
+    while (pass != 0ull) {
+        const int b = __ffsll((long long)pass) - 1;
+        pass &= pass - 1ull;
+        insert_best(best, acc_rank_key(acc_at(d, h, b), col0 + 8u * (uint32_t)(b >> 1) + (uint32_t)(b & 1)));
+    }
+}
 __device__ __forceinline__ void cmp_swap_desc(uint64_t& a, uint64_t& b) {
     const uint64_t hi = a > b ? a : b, lo = a > b ? b : a;
     a = hi;
@@ -344,21 +371,21 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                 }
             } else if (FUSE == 1) {
                 // The query's bound is the 8th best key of some set of its scores, so it is at most its global 8th
-                // best: a key below it is in no top-k (k <= 8), and the tile's list may drop it.  Only scores that are
-                // not below `cut`, the score of the bound or of this lane's own 8th best key, go through insert_best,
-                // under a warp-uniform branch that is rarely taken once the bound has risen; min / max still see every
-                // valid column.  !(f < cut) keeps every key >= the bound, ties, -0.0 and NaNs included (the empty
+                // best: a key below it is in no top-k (k <= 8), and the tile's list may drop it.  Only columns whose
+                // score is not below `cut`, the score of the bound, are marked and then inserted (few, once the bound
+                // has risen); insert_best keeps the lane's 8 best of them.  min / max still see every valid column.
+                // !(f < cut) keeps every key >= the bound, ties, -0.0 and NaNs included (the empty
                 // bound 0 decodes to a NaN cut, which passes everything).
                 const bool live = q < p.Bq;
                 const uint64_t thr = live ? __ldcg(reinterpret_cast<const unsigned long long*>(p.bound + q)) : 0ull;
-                float cut = key_score(thr);
+                const float cut = key_score(thr);
                 float mn = INFINITY, mx = -INFINITY;
                 uint64_t best[kFuseK];
 #pragma unroll
                 for (int k = 0; k < kFuseK; ++k) best[k] = 0ull;
+                uint64_t pass = 0ull;
 #pragma unroll
                 for (int j = 0; j < BN / 8; ++j) {
-                    bool pass[2];
 #pragma unroll
                     for (int c = 0; c < 2; ++c) {
                         const int col = 8 * j + c0 + c;
@@ -366,15 +393,10 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                         const bool valid = col < n_valid;
                         mn = valid ? fminf(mn, f) : mn;
                         mx = valid ? fmaxf(mx, f) : mx;
-                        pass[c] = live && valid && !(f < cut);
-                    }
-                    if (__any_sync(0xffffffffu, pass[0] || pass[1])) {
-#pragma unroll
-                        for (int c = 0; c < 2; ++c)
-                            if (pass[c]) insert_best(best, acc_rank_key(d[4 * j + 2 * h + c], (uint32_t)(n0 + 8 * j + c0 + c)));
-                        cut = key_score(best[kFuseK - 1] > thr ? best[kFuseK - 1] : thr);
+                        if (live && valid && !(f < cut)) pass |= 1ull << (2 * j + c);
                     }
                 }
+                insert_passing(d, h, pass, (uint32_t)(n0 + c0), best);
                 // merge the quad's four partial results: after two butterfly rounds every lane holds the row's
                 // min / max and its 8 best keys
 #pragma unroll
@@ -396,21 +418,21 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                 }
             } else if (FUSE == 4) {
                 // As FUSE 1, in s1 space, with the bound's cut lowered by 2 E_q: a key the gate drops is below every
-                // key the candidate band of its query can hold (select.cu: screen_select).  A lane's own 8th best
-                // still cuts unwidened: a list that drops keys that way is full, and a full list whose 8th key lies in
-                // the band marks its tile saturated.  The two smallest valid scores per row are kept beside the list.
+                // key the candidate band of its query can hold (select.cu: screen_select).  Among the marked keys
+                // insert_best keeps the lane's 8 best: a list that drops keys that way is full, and a full list whose
+                // 8th key lies in the band marks its tile saturated.  The two smallest valid scores per row are kept
+                // beside the list.
                 const bool live = q < p.Bq;
                 const uint64_t thr = live ? __ldcg(reinterpret_cast<const unsigned long long*>(p.bound + q)) : 0ull;
                 const float cut_thr = __fsub_rd(key_score(thr), live ? 2.f * __ldg(p.err + q) : 0.f);
-                float cut = cut_thr;
                 float m1 = INFINITY, m2 = INFINITY;
                 uint32_t i1 = 0xffffffffu, i2 = 0xffffffffu;
                 uint64_t best[kFuseK];
 #pragma unroll
                 for (int k = 0; k < kFuseK; ++k) best[k] = 0ull;
+                uint64_t pass = 0ull;
 #pragma unroll
                 for (int j = 0; j < BN / 8; ++j) {
-                    bool pass[2];
 #pragma unroll
                     for (int c = 0; c < 2; ++c) {
                         const int col = 8 * j + c0 + c;
@@ -421,15 +443,10 @@ k_sim_tc(const __grid_constant__ CUtensorMap map_q_hi, const __grid_constant__ C
                             if (f < m1) { m2 = m1; i2 = i1; m1 = f; i1 = idx; }
                             else { m2 = f; i2 = idx; }
                         }
-                        pass[c] = live && valid && !(f < cut);
-                    }
-                    if (__any_sync(0xffffffffu, pass[0] || pass[1])) {
-#pragma unroll
-                        for (int c = 0; c < 2; ++c)
-                            if (pass[c]) insert_best(best, acc_rank_key(d[4 * j + 2 * h + c], (uint32_t)(n0 + 8 * j + c0 + c)));
-                        cut = best[kFuseK - 1] > thr ? key_score(best[kFuseK - 1]) : cut_thr;
+                        if (live && valid && !(f < cut_thr)) pass |= 1ull << (2 * j + c);
                     }
                 }
+                insert_passing(d, h, pass, (uint32_t)(n0 + c0), best);
 #pragma unroll
                 for (int off = 1; off <= 2; off <<= 1) {
                     const float o1 = __shfl_xor_sync(0xffffffffu, m1, off), o2 = __shfl_xor_sync(0xffffffffu, m2, off);
