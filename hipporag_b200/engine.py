@@ -355,6 +355,8 @@ class Engine:
             self.dim = dim
             if which == 0:
                 self.n_facts = int(rows)
+            else:
+                self.n_passages = int(rows)
 
     def load_embeddings_streamed(self, which: int, rows: int, dim: int, chunks):
         """Upload [rows, dim] fp32 embeddings chunk by chunk without ever holding them in fp32 on the device:
@@ -373,6 +375,8 @@ class Engine:
         self.dim = dim
         if which == 0:
             self.n_facts = int(rows)
+        else:
+            self.n_passages = int(rows)
 
     # ---------------------------------------------------------------- incremental updates (mutable handles)
     def reserve(self, nodes: int = 0, edges: int = 0, facts: int = 0, passages: int = 0):

@@ -116,7 +116,7 @@ def _err_bound(q, f_all):
     Hf, Lf = np.linalg.norm(fh, axis=1).max(), np.linalg.norm(fl, axis=1).max()
     nh, nl = np.linalg.norm(qh, axis=1), np.linalg.norm(ql, axis=1)
     steps = 5 * -(-q.shape[1] // 16)
-    return (nh * Lf + nl * Hf + nl * Lf + steps * 2.0 ** -21 * (nh + nl) * (Hf + Lf)) * (1 + 2.0 ** -10)
+    return (nh * Lf + nl * Hf + nl * Lf + steps * 2.0 ** -20 * (nh + nl) * (Hf + Lf)) * (1 + 2.0 ** -10)
 
 
 def _cross(q, f):
