@@ -22,35 +22,10 @@ int split_queries(hrag_t* h, const float* dQ, int Bq, cudaStream_t s) {
     return split_bf16(dQ, (int64_t)n, h->q_hi.p, h->q_lo.p, s);
 }
 
-// n_ctas: persistent CTAs of the tensor-core GEMM (h->num_sms unless it shares the GPU with PPR sweeps)
-int sim_dispatch(hrag_t* h, const float* dQ, int Bq, int which, float* S, int64_t ldS, cudaStream_t s, int n_ctas) {
-    HRAG_CHECK(which == 1 || !h->fplanes.held(), "internal: sim_dispatch on fact planes in host memory");
-    if (h->sim_mode == HRAG_SIM_FP32 || h->emb[which].hi.p == nullptr) {   // dim % 8 != 0 has no TMA layout
-        HRAG_CHECK(h->emb[which].f32 != nullptr, "similarity: the fp32 embedding matrix was not kept (streamed upload); "
-                                                 "only the tensor-core modes are available");
-        return sim_fp32(dQ, Bq, h->emb[which].f32, h->emb[which].rows, h->dim, S, ldS, s);
-    }
-    HRAG_TRY(split_queries(h, dQ, Bq, s));
-    return sim_tc(h->q_hi.p, h->q_lo.p, Bq, h->emb[which].hi.p, h->emb[which].lo.p, h->emb[which].rows, h->dim,
-                  h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, S, ldS, nullptr, nullptr, nullptr, n_ctas, s);
-}
-
-constexpr int kFusedTopK = 8;     // candidates the GEMM epilogue / row_minmax_topk keep in registers
-bool fused_stage_a(hrag_t* h, int k) {   // tensor-core modes select facts in the GEMM epilogue (no score matrix)
-    return h->sim_mode != HRAG_SIM_FP32 && (h->emb[0].hi.p != nullptr || h->fplanes.held()) && !h->keep_fact_scores &&
-           k <= kFusedTopK;
-}
-
-int64_t chunk_a(hrag_t* h, int k) {
-    const int64_t F = std::max<int64_t>(h->emb[0].rows, 1);
-    if (fused_stage_a(h, k)) return 1024;     // partials are 72 B per (query, 256 facts): 0.8 GB at F = 2.75 M
-    int64_t c = (int64_t)(4e9 / (4.0 * (double)pad4(F)));
-    return std::max<int64_t>(1, std::min<int64_t>(c, 1024));
-}
 int64_t chunk_b(hrag_t* h) {
     const int64_t P = std::max<int64_t>(h->t.n_passages, 1);
     int64_t c = (int64_t)(4e9 / (4.0 * (double)pad4(P)));
-    return std::max<int64_t>(1, std::min<int64_t>(c, 1024));
+    return std::max<int64_t>(1, std::min<int64_t>(c, kQueryChunk));
 }
 
 int fact_norms_update(hrag_t* h, int64_t row0, int64_t n, bool reset) {
@@ -105,9 +80,12 @@ int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx
     HRAG_TRY(c.st_S.ensure((size_t)Bq * ST * 256 * sizeof(float)));
     HRAG_TRY(c.flag.ensure(sizeof(int)));
     if (c.fallbacks.p == nullptr) HRAG_TRY(c.fallbacks.zeros(sizeof(unsigned long long)));
-    const bool lo_host = h->fplanes.lo_only();
+    void* lo_mapped = nullptr;   // lo on the host: its device address, which the gather reads over PCIe
+    const PlaneSet P = emb_planes(h, 0);
+    const bool lo_host = P.on_host[1];
     HRAG_CHECK(lo_host == (chunk_flag != nullptr) && lo_host == (lo_bytes != nullptr),
                "internal: screened_stage_a: a chunk flag and a byte count go with the lo plane in host memory");
+    if (lo_host) HRAG_CUDA(cudaHostGetDevicePointer(&lo_mapped, P.plane[1], 0));
     int* flag = lo_host ? chunk_flag : c.flag.as<int>();
     const EmbMem& e = h->emb[0];
     const int dim = h->dim;
@@ -133,7 +111,7 @@ int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx
                               flag, s));
         if (lo_host)
             HRAG_TRY(screen_gather_mapped(c.slot_ids.as<int>(), c.stage_count.as<int>(), mtiles, ST, e.hi.p,
-                                          h->fplanes.lo_dev, dim, c.st_hi.p, c.st_lo.p, lo_bytes, s));
+                                          lo_mapped, dim, c.st_hi.p, c.st_lo.p, lo_bytes, s));
         else
             HRAG_TRY(screen_gather(c.slot_ids.as<int>(), c.stage_count.as<int>(), mtiles, ST, e.hi.p, e.lo.p, dim,
                                    c.st_hi.p, c.st_lo.p, s));
@@ -162,91 +140,6 @@ int screened_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx
                                    c.fallbacks.as<unsigned long long>(), s);
 }
 
-// Stage A on device pointers, Bq <= chunk_a, on stream s (h->stream when world > 1: the all-gathers run there).
-int dev_stage_a(hrag_t* h, int Bq, const float* d_qf, int k, int* d_top_idx, float* d_top_score, int* d_nvalid,
-                cudaStream_t s, int n_ctas) {
-    const int64_t F = h->emb[0].rows;
-    if ((h->world > 1 ? h->n_facts_global : F) == 0) {   // no facts: get_fact_scores returns an empty array (HippoRAG.py:1454-1456)
-        HRAG_CUDA(cudaMemsetAsync(d_top_idx, 0xff, (size_t)Bq * k * sizeof(int), s));
-        HRAG_CUDA(cudaMemsetAsync(d_top_score, 0, (size_t)Bq * k * sizeof(float), s));
-        HRAG_CUDA(cudaMemsetAsync(d_nvalid, 0, (size_t)Bq * sizeof(int), s));
-        return 0;
-    }
-    HRAG_CHECK(!h->fplanes.held(), "internal: dev_stage_a on fact planes in host memory (fact_stream_stage_a)");
-    const int64_t ld = pad4(F);
-    HRAG_TRY(h->mm_fact.ensure((size_t)Bq * sizeof(float2)));
-    h->last_mm_rows = Bq;
-    if (fused_stage_a(h, k) && screened(h)) {
-        HRAG_TRY(screened_stage_a(h, Bq, d_qf, k, d_top_idx, d_top_score, d_nvalid, s, n_ctas));
-        h->last_fact_rows = 0;
-        return 0;
-    }
-    if (fused_stage_a(h, k)) {
-        const int nt = sim_tc_n_tiles(F);
-        HRAG_TRY(h->part_mm.ensure((size_t)Bq * nt * sizeof(float2)));
-        HRAG_TRY(h->part_keys.ensure((size_t)Bq * nt * 8 * sizeof(uint64_t)));
-        HRAG_TRY(h->part_bound.ensure((size_t)Bq * sizeof(uint64_t)));
-        {
-            StageTimer tm(h, ST_SIM_FACT, s);
-            HRAG_TRY(split_queries(h, d_qf, Bq, s));
-            HRAG_TRY(sim_tc(h->q_hi.p, h->q_lo.p, Bq, h->emb[0].hi.p, h->emb[0].lo.p, F, h->dim,
-                            h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1, nullptr, 0, h->part_mm.as<float2>(),
-                            h->part_keys.as<uint64_t>(), h->part_bound.as<uint64_t>(), n_ctas, s));
-        }
-        if (h->world > 1) {
-            // facts are sharded by row range (SURVEY.md 8(e)): local GEMM + local top-8 -> all-gather of 8 candidates
-            // and (min, max) per query -> the same merge kernel over the `world` candidate lists
-            HRAG_TRY(h->xr_mm.ensure((size_t)h->world * Bq * sizeof(float2)));
-            HRAG_TRY(h->xr_keys.ensure((size_t)h->world * Bq * 8 * sizeof(uint64_t)));
-            float2* mm_all = h->xr_mm.as<float2>();
-            uint64_t* keys_all = h->xr_keys.as<uint64_t>();
-            {
-                StageTimer tm(h, ST_SEL_FACT, s);
-                HRAG_TRY(merge_minmax_topk_ex(h->part_mm.as<float2>(), h->part_keys.as<uint64_t>(), Bq, nt, nt, 1,
-                                              h->fact_row_lo, F, 8, mm_all + (size_t)h->rank * Bq, nullptr, nullptr,
-                                              nullptr, keys_all + (size_t)h->rank * Bq * 8, s));
-            }
-            {
-                StageTimer tc(h, ST_COMM, s);
-                HRAG_NCCL(g_nccl.AllGather(mm_all + (size_t)h->rank * Bq, mm_all, (size_t)Bq * sizeof(float2), ncclInt8,
-                                           h->comm, s));
-                HRAG_NCCL(g_nccl.AllGather(keys_all + (size_t)h->rank * Bq * 8, keys_all, (size_t)Bq * 8 * sizeof(uint64_t),
-                                           ncclInt8, h->comm, s));
-            }
-            StageTimer tm(h, ST_SEL_FACT, s);
-            HRAG_TRY(merge_minmax_topk_ex(mm_all, keys_all, Bq, h->world, 1, Bq, 0, h->n_facts_global, k,
-                                          h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, nullptr, s));
-        } else {
-            StageTimer tm(h, ST_SEL_FACT, s);
-            HRAG_TRY(merge_minmax_topk(h->part_mm.as<float2>(), h->part_keys.as<uint64_t>(), Bq, nt, F, k,
-                                       h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, s));
-        }
-        h->last_fact_rows = 0;
-        return 0;
-    }
-    HRAG_CHECK(h->world == 1, "node-range sharding: stage A needs the tensor-core similarity with linking_top_k <= 8 "
-                              "(the fact rows are sharded; the fp32 / materialised paths are single-GPU)");
-    HRAG_TRY(h->S_fact.ensure((size_t)Bq * ld * sizeof(float)));
-    {
-        StageTimer tm(h, ST_SIM_FACT, s);
-        HRAG_TRY(sim_dispatch(h, d_qf, Bq, 0, h->S_fact.as<float>(), ld, s, n_ctas));
-    }
-    {
-        StageTimer tm(h, ST_SEL_FACT, s);
-        if (k <= kFusedTopK) {
-            HRAG_TRY(row_minmax_topk(h->S_fact.as<float>(), Bq, F, ld, k, h->mm_fact.as<float2>(), d_top_idx,
-                                     d_top_score, d_nvalid, s));
-        } else {   // linking_top_k > 8 (config_utils.py:184): exact radix select on the materialised scores
-            HRAG_TRY(row_minmax_topk(h->S_fact.as<float>(), Bq, F, ld, 0, h->mm_fact.as<float2>(), nullptr, nullptr,
-                                     nullptr, s));
-            HRAG_TRY(row_topk(h->S_fact.as<float>(), Bq, F, ld, k, d_top_idx, d_top_score, s));
-            HRAG_TRY(topk_normalize(Bq, k, F, h->mm_fact.as<float2>(), d_top_idx, d_top_score, d_nvalid, s));
-        }
-    }
-    h->last_fact_rows = Bq;
-    return 0;
-}
-
 // Stage B's similarity part on stream s, Bq <= chunk_b: passage scores into S_buf [Bq, pad4(P)] and their per-row
 // (min, max) into mm_buf.
 int dev_stage_b_sim(hrag_t* h, int Bq, const float* d_qp, hrag::Buf& S_buf, hrag::Buf& mm_buf, cudaStream_t s,
@@ -257,7 +150,7 @@ int dev_stage_b_sim(hrag_t* h, int Bq, const float* d_qp, hrag::Buf& S_buf, hrag
     HRAG_TRY(S_buf.ensure((size_t)Bq * ld * sizeof(float)));
     HRAG_TRY(mm_buf.ensure((size_t)Bq * sizeof(float2)));
     StageTimer tm(h, ST_SIM_PASS, s);
-    HRAG_TRY(sim_dispatch(h, d_qp, Bq, 1, S_buf.as<float>(), ld, s, n_ctas));
+    HRAG_TRY(sim_scores(h, 1, d_qp, Bq, S_buf.as<float>(), ld, s, n_ctas));
     HRAG_TRY(row_minmax_topk(S_buf.as<float>(), Bq, P, ld, 0, mm_buf.as<float2>(), nullptr, nullptr, nullptr, s));
     h->last_pass_S = &S_buf;
     h->last_pass_rows = Bq;
@@ -371,10 +264,11 @@ int dev_stage_b_solve_f64(hrag_t* h, int Bq, const float* S, const float2* mm_pa
 // above it (C3 scan: G = 28 +121 ms per step, G = 44 +5 ms).  DESIGN.md section 4 K2 has the scans of G.
 int overlap_ctas(const hrag_t* h, int Bq, const SweepPlan& plan) {
     constexpr double kGemmFlopPerSmMs = 2.49e9, kScreenFlopPerSmMs = 0.66e9;
-    const bool screen = !h->fplanes.held() && screened(h);   // fact planes in host memory: stage A ran up front
+    const bool up_front = emb_planes(h, 0).streams();   // fact planes in host memory: stage A ran up front
+    const bool screen = !up_front && screened(h);
     const double kSweepNnzPerMs = screen ? 4.20e7 : 3.80e7;
     const int n_seg = h->sim_mode == HRAG_SIM_BF16X3 ? 4 : 1;
-    const int64_t fact_rows = h->fplanes.held() ? 0 : h->emb[0].rows;   // streamed planes: stage A ran up front
+    const int64_t fact_rows = up_front ? 0 : h->emb[0].rows;
     const double split_cols = (screen ? (double)kScreenStageTiles * 256 : (double)fact_rows) + (double)h->emb[1].rows;
     const double t_gemm = 2.0 * n_seg * Bq * split_cols * h->dim / kGemmFlopPerSmMs +
                           (screen ? 2.0 * Bq * (double)fact_rows * h->dim / kScreenFlopPerSmMs : 0.0);
@@ -535,21 +429,11 @@ int hrag_stage_a(hrag_t* h, int32_t B, const float* q_fact, int32_t k, int32_t* 
     HRAG_CHECK(B >= 0 && k >= 1 && k <= kMaxKeptFacts, "hrag_stage_a: k (linking_top_k) must be in [1, 32]");
     HRAG_CHECK(h->dim > 0, "hrag_stage_a: embeddings not loaded");
     HRAG_CUDA(cudaSetDevice(h->device));
-    const int64_t chunk = chunk_a(h, k);
-    HRAG_TRY(h->d_q.ensure((size_t)std::min<int64_t>(chunk, B) * h->dim * sizeof(float)));
     HRAG_TRY(h->d_top_idx.ensure((size_t)std::max(B, 1) * k * sizeof(int)));
     HRAG_TRY(h->d_top_score.ensure((size_t)std::max(B, 1) * k * sizeof(float)));
     HRAG_TRY(h->d_nvalid.ensure((size_t)std::max(B, 1) * sizeof(int)));
-    if (h->fplanes.held())   // fact planes in host memory: one pass over them per fact_stream_pass_cap queries
-        HRAG_TRY(fact_stream_stage_a(h, B, q_fact, false, k, h->d_top_idx.as<int>(), h->d_top_score.as<float>(),
-                                     h->d_nvalid.as<int>()));
-    for (int64_t q0 = 0; q0 < B && !h->fplanes.held(); q0 += chunk) {
-        const int nb = (int)std::min<int64_t>(chunk, B - q0);
-        HRAG_TRY(h2d(h, h->d_q.p, q_fact + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
-        HRAG_TRY(dev_stage_a(h, nb, h->d_q.as<float>(), k, h->d_top_idx.as<int>() + q0 * k,
-                             h->d_top_score.as<float>() + q0 * k, h->d_nvalid.as<int>() + q0, h->stream,
-                             h->debug_sim_ctas > 0 ? h->debug_sim_ctas : h->num_sms));
-    }
+    HRAG_TRY(fact_stage_a(h, B, q_fact, false, k, h->d_top_idx.as<int>(), h->d_top_score.as<float>(),
+                          h->d_nvalid.as<int>(), h->stream, h->debug_sim_ctas > 0 ? h->debug_sim_ctas : h->num_sms));
     if (B > 0) {
         HRAG_TRY(d2h(h, top_idx, h->d_top_idx.p, (size_t)B * k * sizeof(int)));
         HRAG_TRY(d2h(h, top_score, h->d_top_score.p, (size_t)B * k * sizeof(float)));
@@ -627,32 +511,33 @@ int hrag_retrieve_resident(hrag_t* h, int32_t B, const float* d_q_fact, const fl
         HRAG_TRY(top_score[s]->ensure((size_t)chunk * k * sizeof(float)));
         HRAG_TRY(nvalid[s]->ensure((size_t)chunk * sizeof(int)));
     }
-    // fact planes in host memory: stage A of the whole call first, in one pass over the planes (per
-    // fact_stream_pass_cap queries), into fs_top_* [B, k]; the chunks below then skip their stage A
-    const bool streamed = h->fplanes.held();
-    if (streamed) {
+    // stage A per chunk, or, when a fact plane streams, of the whole call first in one walk over the planes (per
+    // pass of queries) into fs_top_* [B, k]; the chunks below then skip their stage A
+    const bool up_front = emb_planes(h, 0).streams();
+    if (up_front) {
         HRAG_TRY(h->fs_top_idx.ensure((size_t)std::max(B, 1) * k * sizeof(int)));
         HRAG_TRY(h->fs_top_score.ensure((size_t)std::max(B, 1) * k * sizeof(float)));
         HRAG_TRY(h->fs_nvalid.ensure((size_t)std::max(B, 1) * sizeof(int)));
-        HRAG_TRY(fact_stream_stage_a(h, B, d_q_fact, true, k, h->fs_top_idx.as<int>(), h->fs_top_score.as<float>(),
-                                     h->fs_nvalid.as<int>()));
+        HRAG_TRY(fact_stage_a(h, B, d_q_fact, true, k, h->fs_top_idx.as<int>(), h->fs_top_score.as<float>(),
+                              h->fs_nvalid.as<int>(), h->stream,
+                              h->debug_sim_ctas > 0 ? h->debug_sim_ctas : h->num_sms));
     }
     // chunk c's similarity part on stream sim_s into slot c % 2 (stage A, then the passage GEMM + min/max)
     auto slot = [&](int64_t c) { return overlap ? (int)(c & 1) : 0; };
     auto similarity = [&](int64_t c, cudaStream_t sim_s, int n_ctas) -> int {
         const int64_t q0 = c * chunk;
         const int nb = (int)std::min<int64_t>(chunk, B - q0), s = slot(c);
-        if (!streamed)
-            HRAG_TRY(dev_stage_a(h, nb, d_q_fact + (size_t)q0 * h->dim, k, top_idx[s]->as<int>(),
-                                 top_score[s]->as<float>(), nvalid[s]->as<int>(), sim_s, n_ctas));
+        if (!up_front)
+            HRAG_TRY(fact_stage_a(h, nb, d_q_fact + (size_t)q0 * h->dim, true, k, top_idx[s]->as<int>(),
+                                  top_score[s]->as<float>(), nvalid[s]->as<int>(), sim_s, n_ctas));
         return dev_stage_b_sim(h, nb, d_q_pass + (size_t)q0 * h->dim, *S_pass[s], *mm_pass[s], sim_s, n_ctas);
     };
     // chunk c's solve part on `stream` (identity recognition-memory filter: the candidates are the kept facts)
     auto solve = [&](int64_t c) -> int {
         const int64_t q0 = c * chunk;
         const int nb = (int)std::min<int64_t>(chunk, B - q0), s = slot(c);
-        const int* kept_idx = streamed ? h->fs_top_idx.as<int>() + q0 * k : top_idx[s]->as<int>();
-        const float* kept_score = streamed ? h->fs_top_score.as<float>() + q0 * k : top_score[s]->as<float>();
+        const int* kept_idx = up_front ? h->fs_top_idx.as<int>() + q0 * k : top_idx[s]->as<int>();
+        const float* kept_score = up_front ? h->fs_top_score.as<float>() + q0 * k : top_score[s]->as<float>();
         return dev_stage_b_solve(h, nb, S_pass[s]->as<float>(), mm_pass[s]->as<float2>(), kept_idx, kept_score, k,
                                  nullptr, damping, passage_node_weight, link_top_k, topk, iters, tol,
                                  d_out_ids + q0 * topk, d_out_scores + q0 * topk);
@@ -693,7 +578,7 @@ int hrag_similarity(hrag_t* h, int which, int32_t B, const float* q, float* out)
     HRAG_CHECK(h->dim > 0 && h->emb[which].rows > 0, "hrag_similarity: embeddings not loaded");
     HRAG_CUDA(cudaSetDevice(h->device));
     const int64_t M = h->emb[which].rows, ld = pad4(M);
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>((int64_t)(2e9 / (4.0 * (double)ld)), 1024));
+    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>((int64_t)(2e9 / (4.0 * (double)ld)), kQueryChunk));
     hrag::Buf& Sb = which == 0 ? h->S_fact : h->S_pass;
     hrag::Buf& mm = which == 0 ? h->mm_fact : h->mm_pass;
     HRAG_TRY(Sb.ensure((size_t)std::min<int64_t>(chunk, std::max(B, 1)) * ld * sizeof(float)));
@@ -702,8 +587,7 @@ int hrag_similarity(hrag_t* h, int which, int32_t B, const float* q, float* out)
     for (int64_t q0 = 0; q0 < B; q0 += chunk) {
         const int nb = (int)std::min<int64_t>(chunk, B - q0);
         HRAG_TRY(h2d(h, h->d_q.p, q + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
-        if (which == 0 && h->fplanes.held()) HRAG_TRY(fact_stream_scores(h, nb, h->d_q.as<float>(), Sb.as<float>(), ld));
-        else HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld, h->stream, h->num_sms));
+        HRAG_TRY(sim_scores(h, which, h->d_q.as<float>(), nb, Sb.as<float>(), ld, h->stream, h->num_sms));
         HRAG_TRY(row_minmax_topk(Sb.as<float>(), nb, M, ld, 0, mm.as<float2>(), nullptr, nullptr, nullptr, h->stream));
         HRAG_TRY(minmax_apply(Sb.as<float>(), nb, M, ld, mm.as<float2>(), h->stream));
         HRAG_CUDA(cudaMemcpy2DAsync(out + (size_t)q0 * M, (size_t)M * sizeof(float), Sb.p, (size_t)ld * sizeof(float),
@@ -722,7 +606,7 @@ int hrag_topk_similarity(hrag_t* h, int which, int32_t B, const float* q, int32_
     HRAG_CHECK(h->dim > 0 && h->emb[which].rows > 0, "hrag_topk_similarity: embeddings not loaded");
     HRAG_CUDA(cudaSetDevice(h->device));
     const int64_t M = h->emb[which].rows, ld = pad4(M);
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>((int64_t)(4e9 / (4.0 * (double)ld)), 1024));
+    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>((int64_t)(4e9 / (4.0 * (double)ld)), kQueryChunk));
     hrag::Buf& Sb = which == 0 ? h->S_fact : h->S_pass;
     const int64_t cb = std::min<int64_t>(chunk, std::max(B, 1));
     HRAG_TRY(Sb.ensure((size_t)cb * ld * sizeof(float)));
@@ -734,10 +618,7 @@ int hrag_topk_similarity(hrag_t* h, int which, int32_t B, const float* q, int32_
         HRAG_TRY(h2d(h, h->d_q.p, q + (size_t)q0 * h->dim, (size_t)nb * h->dim * sizeof(float)));
         {
             StageTimer tm(h, which == 0 ? ST_SIM_FACT : ST_SIM_PASS);
-            if (which == 0 && h->fplanes.held())
-                HRAG_TRY(fact_stream_scores(h, nb, h->d_q.as<float>(), Sb.as<float>(), ld));
-            else
-                HRAG_TRY(sim_dispatch(h, h->d_q.as<float>(), nb, which, Sb.as<float>(), ld, h->stream, h->num_sms));
+            HRAG_TRY(sim_scores(h, which, h->d_q.as<float>(), nb, Sb.as<float>(), ld, h->stream, h->num_sms));
         }
         {
             StageTimer tm(h, ST_TOPK);
@@ -755,7 +636,7 @@ int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float mi
                        int32_t* out_ids, float* out_scores, int32_t* n_found) {
     HRAG_CHECK(h && q && out_ids && out_scores && n_found && (which == 0 || which == 1), "hrag_knn_threshold: bad arguments");
     HRAG_CHECK(kmax >= 1 && kmax <= kCandidateCap && B >= 0, "hrag_knn_threshold: kmax must be in [1, 512]");
-    HRAG_CHECK(which == 1 || !h->fplanes.held(),
+    HRAG_CHECK(!emb_planes(h, which).streams(),
                "hrag_knn_threshold: the fact planes are held in host memory (hrag_set_fact_memory); the threshold "
                "search runs on resident planes only");
     HRAG_CHECK(h->dim > 0 && h->emb[which].rows > 0 && h->emb[which].hi.p != nullptr,
@@ -763,7 +644,7 @@ int hrag_knn_threshold(hrag_t* h, int which, int32_t B, const float* q, float mi
     HRAG_CHECK(h->sim_mode != HRAG_SIM_FP32, "hrag_knn_threshold: the threshold epilogue lives in the tensor-core kernel");
     HRAG_CUDA(cudaSetDevice(h->device));
     const int64_t M = h->emb[which].rows;
-    const int64_t chunk = 1024;
+    const int64_t chunk = kQueryChunk;
     const int64_t cb = std::min<int64_t>(chunk, std::max(B, 1));
     HRAG_TRY(h->d_q.ensure((size_t)cb * h->dim * sizeof(float)));
     HRAG_TRY(h->part_keys.ensure((size_t)cb * kCandidateCap * sizeof(uint64_t)));

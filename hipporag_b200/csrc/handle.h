@@ -10,7 +10,8 @@
 //   emb       bf16 hi/lo planes [rows, d] x 2 (wgmma similarity); fp32 [rows, d] only when uploaded whole    (resident)
 //             facts over the hrag_set_fact_memory budget: the planes in pinned host memory, and on the device a
 //             ring of two slices (fact_stream.cu) of at most the budget; under HRAG_FACT_LO_ON_HOST the hi plane
-//             resident, the lo plane in mapped pinned host memory and a ring of two lo slices
+//             resident, the lo plane in mapped pinned host memory and a ring of two lo slices.  Where each plane
+//             is: emb_planes; every path walks the planes with stream_slices, whatever their placement
 //   shared    with hrag_index_export / hrag_index_attach the graph planes (but seg_partial), the tables and the embedding
 //             planes of an attached handle are the owner's allocations, mapped through CUDA IPC (index_share.cu)
 //   knn       self-KNN index (knn_index.cu): bf16 hi/lo [entities, d] x 2, ids / scores [entities, pad4(kmax + 1)]
@@ -128,17 +129,15 @@ struct EmbMem {                   // one embedding matrix (0 = facts, 1 = passag
     int64_t rows = 0;             // rows held by THIS handle (node-range sharding: the rank's slice of the facts)
 };
 // bf16 hi / lo planes [rows, dim] held in pinned host memory and streamed through a device ring of two halves, each
-// slice_rows rows of hi then lo (fact_stream.cu): the fact planes over the hrag_set_fact_memory budget (FactPlanes) and
-// the synonymy KNN planes over the hrag_knn_set_memory budget (KnnIndex::host).  `copy` carries the ring uploads;
-// loaded[i] marks half i filled, freed[i] the last read of half i on `stream`.  Owned and move-only: freed by release().
-// lo_only (the fact planes under HRAG_FACT_LO_ON_HOST): no hi plane here (the caller keeps it resident), lo is mapped
-// (lo_dev: its device address, which kernels read over PCIe) and a ring half holds lo [slice_rows, dim] only.
+// slice_rows rows of the planes held here, hi then lo (fact_stream.cu): the fact planes over the hrag_set_fact_memory
+// budget (FactPlanes) and the synonymy KNN planes over the hrag_knn_set_memory budget (KnnIndex::host).  `copy`
+// carries the ring uploads; loaded[i] marks half i filled, freed[i] the last read of half i on `stream`.  Owned and
+// move-only: freed by release().  Under HRAG_FACT_LO_ON_HOST only lo is held (hi stays null), and it is mapped.
 struct HostPlanes {
-    void *hi = nullptr, *lo = nullptr;   // pinned (cudaHostAlloc)
-    void* lo_dev = nullptr;              // lo_only: the device address of lo (cudaHostGetDevicePointer)
+    void *hi = nullptr, *lo = nullptr;   // pinned (cudaHostAlloc); null: that plane is not held here
     size_t plane_bytes = 0;              // of one of them (the capacity)
     int64_t slice_rows = 0;              // a multiple of 256, the K2 tile width
-    Buf ring;                            // 2 halves, each hi [slice_rows, dim] then lo [slice_rows, dim] bf16
+    Buf ring;                            // 2 halves, each [slice_rows, dim] bf16 per plane held
     cudaStream_t copy = nullptr;
     cudaEvent_t loaded[2] = {nullptr, nullptr}, freed[2] = {nullptr, nullptr};
     HostPlanes() = default;
@@ -149,17 +148,39 @@ struct HostPlanes {
     }
     ~HostPlanes() { release(); }
     void swap(HostPlanes& o) noexcept {
-        std::swap(hi, o.hi); std::swap(lo, o.lo); std::swap(lo_dev, o.lo_dev); std::swap(plane_bytes, o.plane_bytes);
+        std::swap(hi, o.hi); std::swap(lo, o.lo); std::swap(plane_bytes, o.plane_bytes);
         std::swap(slice_rows, o.slice_rows); std::swap(ring, o.ring); std::swap(copy, o.copy);
         std::swap(loaded, o.loaded); std::swap(freed, o.freed);
     }
     // pinned planes of `bytes` each (contents lost), a ring of two `slice`-row halves at `dim`, the copy stream;
-    // lo_only: the mapped lo plane only, and lo-only ring halves
-    int alloc(size_t bytes, int64_t slice, int dim, bool lo_only = false);
+    // !with_hi: the mapped lo plane only
+    int alloc(size_t bytes, int64_t slice, int dim, bool with_hi = true);
     void release();
     bool held() const { return lo != nullptr; }                    // some plane is in host memory
-    bool lo_only() const { return lo != nullptr && hi == nullptr; }
 };
+
+// Where each plane of one hi / lo set lives, as the walker (stream_slices) and the fill (planes_fill) read it:
+// plane[p] is a device address (read in place) or, when on_host[p], a pinned host address (streamed through host's
+// ring).  plane_set builds it from the device planes and the host planes of a set; emb_planes is the one answer for
+// the embedding matrices.
+struct PlaneSet {
+    char* plane[2] = {nullptr, nullptr};   // hi, lo
+    bool on_host[2] = {false, false};
+    const HostPlanes* host = nullptr;
+    bool streams() const { return on_host[0] || on_host[1]; }
+    int64_t host_bytes() const {
+        return streams() ? (int64_t)host->plane_bytes * ((on_host[0] ? 1 : 0) + (on_host[1] ? 1 : 0)) : 0;
+    }
+};
+inline PlaneSet plane_set(const Buf& hi, const Buf& lo, const HostPlanes* host) {
+    PlaneSet P;
+    P.on_host[0] = host && host->hi;
+    P.on_host[1] = host && host->lo;
+    P.plane[0] = P.on_host[0] ? static_cast<char*>(host->hi) : hi.as<char>();
+    P.plane[1] = P.on_host[1] ? static_cast<char*>(host->lo) : lo.as<char>();
+    P.host = host;
+    return P;
+}
 
 // The resident self-KNN index (knn_index.cu), independent of the retrieval index: the bf16 hi / lo planes of its unit
 // rows, and per row the first kmax keys with score >= thr, best first.  A list row is `width` = pad4(kmax + 1) int32
@@ -177,14 +198,13 @@ struct KnnIndex {
 constexpr int kKnnComplete = 1, kKnnRefill = 2;
 
 // Fact planes held in pinned host memory (hrag_set_fact_memory with a budget below rows x dim x 4 bytes;
-// fact_stream.cu): byte for byte what a resident load builds, plus the per-pass state of a streamed stage A.  held():
-// the fact planes are not all resident, so stage A runs for a whole call at once (fact_stream_stage_a); lo_only():
-// HRAG_FACT_LO_ON_HOST placed them, the hi plane is emb[0].hi and only lo is here.
+// fact_stream.cu): byte for byte what a resident load builds, plus the state of a stage A over several slices.  Which
+// plane is where: emb_planes(h, 0).
 struct FactPlanes : HostPlanes {
     // a pass's per-query state: fused, (min, max) [3, B] and 8 keys [3, B, 8] (two running slots and this slice's);
     // materialised, the running (min, max) [B] and one chunk's slice top-k sl_ids / sl_scores [chunk, k], sl_mm
     Buf run_mm, run_keys, sl_ids, sl_scores, sl_mm;
-    Buf tail;                            // hrag_similarity's scores of a ragged last slice (fact_stream_scores)
+    Buf tail;                            // sim_scores' scores of a ragged last slice
     FactPlanes() = default;
     FactPlanes(const FactPlanes&) = delete;
     FactPlanes& operator=(const FactPlanes&) = delete;
@@ -390,6 +410,12 @@ inline int d2h(hrag_t* h, void* dst, const void* src, size_t bytes) {
     return 0;
 }
 
+// The one answer to "which plane of embedding matrix `which` is where": only the facts' may be in host memory.
+inline PlaneSet emb_planes(const hrag_t* h, int which) {
+    return plane_set(h->emb[which].hi, h->emb[which].lo, which == 0 ? &h->fplanes : nullptr);
+}
+
+constexpr int kQueryChunk = 1024;  // queries per similarity GEMM launch (stage A, stage B, the similarity entries)
 constexpr int kSeedSlots = kSeedSlotsPerQuery;   // 2 phrases per kept fact, <= 32 kept facts
 constexpr float kMixedT = 64.f;    // residual scale: r ~ 5e-4 x, keeps it in fp16's normal range
 constexpr double kDefaultTol = 1e-6;     // relative L1 accuracy of the PPR vector when the caller passes tol <= 0
@@ -468,46 +494,49 @@ int gather_rows(hrag_t* h, const void* base, size_t row_bytes, const int* row_sr
 int host_planes_plan(int64_t budget, const std::string& who, const char* setter, int64_t rows, int dim,
                      int64_t* slice_rows);
 // fact_planes_plan, before a fact load touches the handle: host_planes_plan of the fact budget, or under
-// HRAG_FACT_LO_ON_HOST the lo ring's slice rows (*lo_only set); rejects sharded handles and dim % 8 != 0.
-// fact_planes_alloc, after reset_embeddings: the pinned planes and the ring for the handle's fact rows, and under
-// lo_only the resident hi plane and the zeroed norm maxima as well.
+// HRAG_FACT_LO_ON_HOST the lo ring's slice rows (*hi_resident set); rejects sharded handles and dim % 8 != 0.
+// fact_planes_alloc, after reset_embeddings: the pinned planes and the ring for the handle's fact rows, and with
+// hi_resident the resident hi plane and the zeroed norm maxima as well.
 int fact_planes_plan(const hrag_t* h, const std::string& who, int64_t rows, int dim, int64_t* slice_rows,
-                     bool* lo_only);
-int fact_planes_alloc(hrag_t* h, int64_t slice_rows, bool lo_only);
-// Fills host plane rows [row0, row0 + n) of `ps` (dim wide) from fp32 rows (host or device): ring half 0 stages up to
-// slice_rows fp32 rows, half 1 takes their split, which goes back to the pinned planes.  before_write(r, m, hi, lo),
-// when given, runs on `stream` after rows [row0 + r, row0 + r + m) are split into hi / lo (ring half 1) and before they
-// are written back; half 0 is free then.  Returns once the rows are written.  lo_only planes: hi_dev is the resident
-// hi plane, which takes the hi rows directly; a step is slice_rows / 2 rows, the lo ring's bytes.
+                     bool* hi_resident);
+int fact_planes_alloc(hrag_t* h, int64_t slice_rows, bool hi_resident);
+// Fills plane rows [row0, row0 + n) of `P` (dim wide, some plane on the host) from fp32 rows (host or device): ring
+// half 0 stages as many fp32 rows as its bytes hold, half 1 takes their split; a host plane's rows go back to the
+// pinned plane, a resident plane takes its rows directly.  before_write(r, m, hi, lo), when given, runs on `stream`
+// after rows [row0 + r, row0 + r + m) are split into hi / lo and before they are written back; half 0 is free then.
+// Returns once the rows are written.
 using BeforeWrite = std::function<int(int64_t r, int64_t m, const char* hi, const char* lo)>;
-int planes_fill(hrag_t* h, HostPlanes& ps, int dim, int64_t row0, int64_t n, const float* src, bool src_on_device,
-                const BeforeWrite& before_write = nullptr, char* hi_dev = nullptr);
+int planes_fill(hrag_t* h, const PlaneSet& P, int dim, int64_t row0, int64_t n, const float* src, bool src_on_device,
+                const BeforeWrite& before_write = nullptr);
 int fact_planes_fill(hrag_t* h, int64_t row0, int64_t n, const float* src, bool src_on_device);
-// Walks rows [row0, row1) of the host planes `ps` (dim wide) on `stream`, in slices of slice_rows from row0:
-// body(s, first row, rows, hi, lo) reads slice s from its ring half while the copy stream fills the other half with
-// slice s + 1.  `both`: stream the lo plane too (HRAG_SIM_BF16 reads only hi).  Every copy is joined into `stream`
-// before its slice is read, so the caller's later work on `stream` sees the whole walk.  Lo-only form (ps.lo_only(),
-// hi_dev = the resident hi plane): only lo streams, and body reads hi in place (lo = hi when !both: nothing streams).
+// Walks rows [row0, row1) of the planes `P` (dim wide): body(s, first row, rows, hi, lo) reads slice s.  Both planes
+// resident: body runs once over [row0, row1) with their device addresses, and the walk records, copies and counts
+// nothing.  Else slices of slice_rows from row0 on `stream`: a plane on the host is read from its ring half while the
+// copy stream fills the other half with slice s + 1, a resident plane in place.  `both`: the lo plane is read too
+// (HRAG_SIM_BF16 reads only hi; lo = hi when lo is not copied).  Every copy is joined into `stream` before its slice
+// is read, so the caller's later work on `stream` sees the whole walk.
 template <class Body>
-int stream_slices(hrag_t* h, HostPlanes& ps, int64_t dim, int64_t row0, int64_t row1, bool both, Body body,
-                  const char* hi_dev = nullptr) {
+int stream_slices(hrag_t* h, const PlaneSet& P, int64_t dim, int64_t row0, int64_t row1, bool both, Body body) {
+    const size_t rb = (size_t)dim * 2;
+    if (!P.streams()) return body(0, row0, row1 - row0, P.plane[0] + row0 * rb, P.plane[1] + row0 * rb);
+    const HostPlanes& ps = *P.host;
     const int64_t S = ps.slice_rows, n_slices = ceil_div(row1 - row0, S);
-    const bool lo_only = hi_dev != nullptr;
-    const size_t half_bytes = (size_t)S * dim * (lo_only ? 2 : 4);
+    const bool copy_lo = both && P.on_host[1];
+    const size_t lo_at = P.on_host[0] ? (size_t)S * rb : 0;   // of the lo rows in a ring half
+    const size_t half_bytes = lo_at + (P.on_host[1] ? (size_t)S * rb : 0);
     char* ring = ps.ring.as<char>();
     auto copy = [&](int64_t s) -> int {
         const int64_t r0 = row0 + s * S, n = std::min(S, row1 - r0);
         const int half = (int)(s & 1);
         char* dst = ring + half * half_bytes;
         HRAG_CUDA(cudaStreamWaitEvent(ps.copy, ps.freed[half], 0));   // the last read of this half is done
-        if (!lo_only)
-            HRAG_CUDA(cudaMemcpyAsync(dst, static_cast<char*>(ps.hi) + (size_t)r0 * dim * 2, (size_t)n * dim * 2,
+        if (P.on_host[0])
+            HRAG_CUDA(cudaMemcpyAsync(dst, P.plane[0] + (size_t)r0 * rb, (size_t)n * rb, cudaMemcpyHostToDevice,
+                                      ps.copy));
+        if (copy_lo)
+            HRAG_CUDA(cudaMemcpyAsync(dst + lo_at, P.plane[1] + (size_t)r0 * rb, (size_t)n * rb,
                                       cudaMemcpyHostToDevice, ps.copy));
-        if (both)
-            HRAG_CUDA(cudaMemcpyAsync(dst + (lo_only ? 0 : (size_t)S * dim * 2),
-                                      static_cast<char*>(ps.lo) + (size_t)r0 * dim * 2, (size_t)n * dim * 2,
-                                      cudaMemcpyHostToDevice, ps.copy));
-        h->stats.h2d_bytes += (int64_t)n * dim * 2 * ((lo_only ? 0 : 1) + (both ? 1 : 0));
+        h->stats.h2d_bytes += (int64_t)n * (int64_t)rb * ((P.on_host[0] ? 1 : 0) + (copy_lo ? 1 : 0));
         HRAG_CUDA(cudaEventRecord(ps.loaded[half], ps.copy));
         return 0;
     };
@@ -520,23 +549,29 @@ int stream_slices(hrag_t* h, HostPlanes& ps, int64_t dim, int64_t row0, int64_t 
         HRAG_CUDA(cudaStreamWaitEvent(h->stream, ps.loaded[half], 0));
         const int64_t r0 = row0 + s * S;
         const char* h_half = ring + half * half_bytes;
-        const char* e_hi = lo_only ? hi_dev + (size_t)r0 * dim * 2 : h_half;
-        const char* e_lo = lo_only ? (both ? h_half : e_hi) : h_half + (size_t)S * dim * 2;
+        const char* e_hi = P.on_host[0] ? h_half : P.plane[0] + (size_t)r0 * rb;
+        const char* e_lo = copy_lo ? h_half + lo_at : P.on_host[1] ? e_hi : P.plane[1] + (size_t)r0 * rb;
         HRAG_TRY(body(s, r0, std::min(S, row1 - r0), e_hi, e_lo));
         HRAG_CUDA(cudaEventRecord(ps.freed[half], h->stream));
     }
     return 0;
 }
-// Stage A of B queries (host or device fp32 [B, dim]) in passes of at most fact_stream_pass_cap queries, each
-// streaming the planes once: the outputs of dev_stage_a, bit for bit, for all B queries (device [B, k], [B]).
-int fact_stream_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* d_top_idx,
-                        float* d_top_score, int* d_nvalid);
-// Raw fact scores of nb (<= 1024) device queries into S [nb, ldS], the planes streamed once.
-int fact_stream_scores(hrag_t* h, int nb, const float* d_q, float* S, int64_t ldS);
-int64_t fact_stream_pass_cap(const hrag_t* h);
+// fused_stage_a: stage A selects the facts in the GEMM epilogue (tensor-core modes, k <= 8, no kept scores);
+// chunk_a: queries per stage-A chunk over the resident facts.
+bool fused_stage_a(const hrag_t* h, int k);
+int64_t chunk_a(const hrag_t* h, int k);
+// Stage A of B queries (fp32 [B, dim], host or device) into device top_idx / top_score [B, k] and nvalid [B], on
+// stream s with n_ctas GEMM CTAs: the split K2 walked over the fact planes (or the stage-A screen), in passes of a
+// query chunk on resident planes and of fact_stream_pass_cap queries, each walking the planes once, when one streams
+// (on `stream` then).  Every placement gives the same outputs, bit for bit.
+int fact_stage_a(hrag_t* h, int B, const float* q, bool q_on_device, int k, int* top_idx, float* top_score,
+                 int* nvalid, cudaStream_t s, int n_ctas);
+// Raw scores of nb (<= 1024) device queries against embedding matrix `which` into S [nb, ldS] on stream s: the
+// tensor-core GEMM walked over the planes, or sim_fp32 over resident fp32 rows.
+int sim_scores(hrag_t* h, int which, const float* dQ, int nb, float* S, int64_t ldS, cudaStream_t s, int n_ctas);
 
 // api.cu: the stage-A screen on one query chunk.  screened(h): the screen applies to this handle's facts.
-// screened_stage_a: Bq <= 1024 queries (fp32 on the device); with the lo plane in host memory (h->fplanes.lo_only())
+// screened_stage_a: Bq <= 1024 queries (fp32 on the device); with the lo plane in host memory
 // it gathers the staged lo rows from the mapped plane, adds their bytes to *lo_bytes, raises *chunk_flag instead of
 // running the gated exact path (the caller reruns a flagged chunk) and counts no fallback.
 bool screened(const hrag_t* h);

@@ -117,7 +117,7 @@ int64_t owned_device_bytes(const hrag_t* h) {
     return n;
 }
 
-bool holds_index(const hrag_t* h) { return h->g.cv || h->t.passage_vid || h->dim > 0 || h->fplanes.held(); }
+bool holds_index(const hrag_t* h) { return h->g.cv || h->t.passage_vid || h->dim > 0 || emb_planes(h, 0).streams(); }
 
 // The attached handle's index goes: every mapping is closed (Buf::reset bumps g_buf_generation, so no captured solve
 // that points into them is replayed).  The caller has synchronised `stream`.
@@ -178,7 +178,7 @@ int hrag_index_export(hrag_t* h, void* blob, int64_t cap, int64_t* size) {
                who + ": the handle is attached to another process's index; only the process that loaded it exports it");
     HRAG_CHECK(h->g.cv && h->t.passage_vid && h->dim > 0, who + ": no index loaded (graph, tables and embeddings)");
     HRAG_CHECK(h->world == 1, who + ": a node-range-sharded handle (world > 1) cannot be shared");
-    HRAG_CHECK(!h->fplanes.held(), who + ": the fact planes are held in pinned host memory (hrag_set_fact_memory), "
+    HRAG_CHECK(!emb_planes(h, 0).streams(), who + ": the fact planes are held in pinned host memory (hrag_set_fact_memory), "
                                          "which belongs to this process alone; load them resident to share the index");
     for (int w = 0; w < 2; ++w)
         HRAG_CHECK(!(h->emb[w].f32 && !h->emb[w].own.p),

@@ -211,7 +211,7 @@ int check_updatable(hrag_t* h, const std::string& who) {
     HRAG_CHECK(h, who + ": null handle");
     HRAG_TRY(check_index_private(h, who));
     HRAG_CHECK(h->world == 1, who + ": a node-range-sharded handle (world > 1) cannot be updated in place; reload it");
-    HRAG_CHECK(!h->fplanes.held(), who + ": the fact planes are held in host memory (hrag_set_fact_memory) and cannot "
+    HRAG_CHECK(!emb_planes(h, 0).streams(), who + ": the fact planes are held in host memory (hrag_set_fact_memory) and cannot "
                                          "be updated in place; reload the index");
     HRAG_CHECK(h->g.cv, who + ": no graph loaded");
     HRAG_CHECK(h->mutable_index, who + ": the handle is not mutable: call hrag_set_mutable(h, 1) before the graph is "
@@ -570,10 +570,8 @@ int hrag_debug_index(hrag_t* h, int plane, void* host_out, int64_t max_bytes, in
     const SeedTables& t = h->t;
     const EdgeList& E = h->graph.edges;
     const int64_t d = h->dim, F = h->emb[0].rows, P = h->emb[1].rows;
-    // fact planes in pinned host memory (hrag_set_fact_memory): both, or lo only (the hi plane stays resident)
-    const bool host = h->fplanes.held(), host_hi = host && !h->fplanes.lo_only();
-    const void* src[13] = {t.passage_vid, t.fact_subj_vid, t.fact_obj_vid, t.ent_chunk_count,
-                           host_hi ? h->fplanes.hi : h->emb[0].hi.p, host ? h->fplanes.lo : h->emb[0].lo.p,
+    const PlaneSet fp = emb_planes(h, 0);   // a fact plane may be in pinned host memory (hrag_set_fact_memory)
+    const void* src[13] = {t.passage_vid, t.fact_subj_vid, t.fact_obj_vid, t.ent_chunk_count, fp.plane[0], fp.plane[1],
                            h->emb[1].hi.p, h->emb[1].lo.p,
                            h->emb[0].f32, h->emb[1].f32, E.src.p, E.dst.p, E.w.p};
     const int64_t bytes[13] = {4 * (int64_t)t.n_passages, 4 * t.n_facts, 4 * t.n_facts,

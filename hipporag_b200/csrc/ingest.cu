@@ -193,8 +193,8 @@ int hrag_load_embeddings(hrag_t* h, int which, int64_t rows, int32_t dim, const 
     HRAG_CHECK(h->dim == 0 || h->dim == dim || h->emb[1 - which].rows == 0,
                "hrag_load_embeddings: fact and passage embeddings must share dim");
     int64_t slice_rows = 0;   // > 0: the fact planes go to pinned host memory (hrag_set_fact_memory)
-    bool lo_only = false;     // only the lo plane does (HRAG_FACT_LO_ON_HOST)
-    if (which == 0) HRAG_TRY(fact_planes_plan(h, "hrag_load_embeddings", rows, dim, &slice_rows, &lo_only));
+    bool hi_resident = false;   // only the lo plane does (HRAG_FACT_LO_ON_HOST)
+    if (which == 0) HRAG_TRY(fact_planes_plan(h, "hrag_load_embeddings", rows, dim, &slice_rows, &hi_resident));
     HRAG_CHECK(!slice_rows || !on_device,
                "hrag_load_embeddings: the fact planes exceed the hrag_set_fact_memory budget and go to host memory; "
                "pass the fp32 fact rows from host memory (on the device they would take the memory the budget keeps "
@@ -204,7 +204,7 @@ int hrag_load_embeddings(hrag_t* h, int which, int64_t rows, int32_t dim, const 
     EmbMem& e = h->emb[which];
     if (e.rows == 0) return 0;
     if (slice_rows) {   // no fp32 copy is kept, as with the streamed loader
-        HRAG_TRY(fact_planes_alloc(h, slice_rows, lo_only));
+        HRAG_TRY(fact_planes_alloc(h, slice_rows, hi_resident));
         return fact_planes_fill(h, 0, e.rows, emb, false);
     }
     if (on_device) e.f32 = emb;   // caller keeps it alive
@@ -227,11 +227,11 @@ int hrag_load_embeddings_begin(hrag_t* h, int which, int64_t rows, int32_t dim) 
     HRAG_CHECK(h->dim == 0 || h->dim == dim || h->emb[1 - which].rows == 0,
                "hrag_load_embeddings_begin: fact and passage embeddings must share dim");
     int64_t slice_rows = 0;
-    bool lo_only = false;
-    if (which == 0) HRAG_TRY(fact_planes_plan(h, "hrag_load_embeddings_begin", rows, dim, &slice_rows, &lo_only));
+    bool hi_resident = false;
+    if (which == 0) HRAG_TRY(fact_planes_plan(h, "hrag_load_embeddings_begin", rows, dim, &slice_rows, &hi_resident));
     HRAG_CUDA(cudaSetDevice(h->device));
     reset_embeddings(h, which, rows, dim);
-    if (slice_rows) return fact_planes_alloc(h, slice_rows, lo_only);
+    if (slice_rows) return fact_planes_alloc(h, slice_rows, hi_resident);
     const size_t n = (size_t)std::max<int64_t>(h->emb[which].rows, 1) * dim;
     HRAG_TRY(h->emb[which].hi.ensure(n * 2));
     HRAG_TRY(h->emb[which].lo.ensure(n * 2));
@@ -246,7 +246,7 @@ int hrag_load_embeddings_chunk(hrag_t* h, int which, int64_t row0, int64_t n_row
     HRAG_CHECK(h && (which == 0 || which == 1) && emb, "hrag_load_embeddings_chunk: bad arguments");
     HRAG_TRY(check_index_private(h, "hrag_load_embeddings_chunk"));
     const EmbMem& e = h->emb[which];
-    const bool host_planes = which == 0 && h->fplanes.held();   // both planes, or lo only (fact_planes_fill)
+    const bool host_planes = emb_planes(h, which).streams();   // both planes, or lo only (fact_planes_fill)
     HRAG_CHECK((e.hi.p != nullptr || host_planes) && e.f32 == nullptr,
                "hrag_load_embeddings_chunk: call hrag_load_embeddings_begin first");
     HRAG_CUDA(cudaSetDevice(h->device));

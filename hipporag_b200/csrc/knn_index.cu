@@ -19,15 +19,15 @@
 // Scores come from the same K2 accumulators whatever the tile a pair falls in, so the lists equal a fresh all-pairs
 // run.  Every argument is checked before the index is touched; a failure after that clears it (the next call builds).
 //
-// Planes over the hrag_knn_set_memory budget live in pinned host memory (KnnIndex::host) and stream through the ring
-// walker of the fact planes (stream_slices, handle.h); the lists stay on the device.  Each step then runs as
-// above with these changes: in step 1 the rows are split through the ring by planes_fill, and before a chunk is
-// written back the held rows its kept rows come from are copied into ring half 0 and compared there; in steps 3 - 4
-// the query rows are staged on the device in passes of up to kHostPass rows, the keys stream slice by slice, and each
-// query's 512 candidates persist across the slices (moved to rows of the key range after every slice); in step 5 the
-// overflowing rows are scored one key slice at a time and each slice's exact top-k is folded into the row's list by
-// k_knn_merge.  A (score desc, id asc) fold of per-slice top-kmax lists is the top-kmax of their union, so the lists
-// are those of the resident planes, bit for bit.
+// Planes over the hrag_knn_set_memory budget live in pinned host memory (KnnIndex::host); the lists stay on the
+// device.  Steps 3 - 5 walk the keys with the walker of the fact planes (stream_slices, handle.h), one slice on device
+// planes: the query rows are read in place or gathered (device planes, passes of kChunk) or staged (host planes,
+// passes of up to kHostPass), each query's 512 candidates persist across the key slices (moved to rows of the key
+// range after every slice but the first), and in step 5 the overflowing rows are scored one key slice at a time and
+// each slice's exact top-k is folded into the row's list by k_knn_merge.  A (score desc, id asc) fold of per-slice
+// top-kmax lists is the top-kmax of their union, so the lists do not depend on the placement, bit for bit.  In step 1
+// host rows are split through the ring by planes_fill, and before a chunk is written back the held rows its kept rows
+// come from are copied into ring half 0 and compared there.
 #include <algorithm>
 #include <cmath>
 #include <cstring>
@@ -198,133 +198,70 @@ int launch_merge(hrag_t* h, int n, const int* rows, int64_t r0, const int* cand_
 // Scratch of one update call (freed on return).
 struct Scratch { Buf q_hi, q_lo, cand, count, prev, out_ids, out_scores, found, rows, redo_rows, S; };
 
-// The query rows (`list` (host) of n_q rows, or the range [r0, r0 + n_q)) against keys [key0, key0 + M): each
-// query's list becomes the first kmax of its keys >= thr there, merged with the list it has when `merge`.
-int run_queries(hrag_t* h, Scratch& s, const std::vector<int>* list, int64_t r0, int64_t n_q, int64_t key0, int64_t M,
-                bool merge) {
-    if (n_q == 0 || M == 0) return 0;
-    KnnIndex& K = h->knn;
-    cudaStream_t st = h->stream;
-    const size_t rb = (size_t)K.dim * 2;
-    const void* e_hi = static_cast<const char*>(K.hi.p) + (size_t)key0 * rb;
-    const void* e_lo = static_cast<const char*>(K.lo.p) + (size_t)key0 * rb;
-    const int* d_rows = nullptr;
-    if (list) {
-        HRAG_TRY(s.rows.ensure((size_t)n_q * 4));
-        HRAG_TRY(h2d(h, s.rows.p, list->data(), (size_t)n_q * 4));
-        d_rows = s.rows.as<int>();
-    }
-    HRAG_TRY(s.q_hi.ensure((size_t)kChunk * rb));
-    HRAG_TRY(s.q_lo.ensure((size_t)kChunk * rb));
-    HRAG_TRY(s.cand.ensure((size_t)kChunk * kCandidateCap * sizeof(uint64_t)));
-    HRAG_TRY(s.count.ensure((size_t)kChunk * 4));
-    HRAG_TRY(s.found.ensure((size_t)kChunk * 4));
-    HRAG_TRY(s.out_ids.ensure((size_t)kChunk * K.kmax * 4));
-    HRAG_TRY(s.out_scores.ensure((size_t)kChunk * K.kmax * 4));
-    std::vector<int> found((size_t)kChunk), over;   // over: positions in the query set whose candidates overflowed
-    for (int64_t q0 = 0; q0 < n_q; q0 += kChunk) {
-        const int nb = (int)std::min<int64_t>(kChunk, n_q - q0);
-        const void *qh = static_cast<const char*>(K.hi.p) + (size_t)(r0 + q0) * rb,
-                   *ql = static_cast<const char*>(K.lo.p) + (size_t)(r0 + q0) * rb;
-        if (d_rows) {
-            HRAG_TRY(gather_rows(h, K.hi.p, rb, d_rows + q0, nb, s.q_hi.p));
-            HRAG_TRY(gather_rows(h, K.lo.p, rb, d_rows + q0, nb, s.q_lo.p));
-            qh = s.q_hi.p, ql = s.q_lo.p;
-        }
-        HRAG_CUDA(cudaMemsetAsync(s.count.p, 0, (size_t)nb * 4, st));
-        {
-            StageTimer tm(h, ST_SIM_FACT);
-            HRAG_TRY(sim_tc_threshold(qh, ql, nb, e_hi, e_lo, M, K.dim, 4, K.thr, s.cand.as<uint64_t>(),
-                                      s.count.as<int>(), kCandidateCap, h->num_sms, st));
-        }
-        {
-            StageTimer tm(h, ST_TOPK);
-            HRAG_TRY(sort_candidates(s.cand.as<uint64_t>(), s.count.as<int>(), nb, kCandidateCap, K.kmax,
-                                     s.out_ids.as<int>(), s.out_scores.as<float>(), s.found.as<int>(), st));
-            HRAG_TRY(launch_merge(h, nb, d_rows ? d_rows + q0 : nullptr, r0 + q0, s.out_ids.as<int>(),
-                                  s.out_scores.as<float>(), K.kmax, s.found.as<int>(), key0, merge));
-        }
-        HRAG_TRY(d2h(h, found.data(), s.found.p, (size_t)nb * 4));
-        HRAG_CUDA(cudaStreamSynchronize(st));
-        for (int b = 0; b < nb; ++b)
-            if (found[b] > kCandidateCap) over.push_back((int)(q0 + b));
-    }
-    if (over.empty()) return 0;
-
-    // the overflow redo: score GEMM + exact top-k over the same key range, merged as above
-    std::vector<int> tgt(over.size());
-    for (size_t i = 0; i < over.size(); ++i) tgt[i] = list ? (*list)[over[i]] : (int)(r0 + over[i]);
-    const int64_t n_over = (int64_t)tgt.size(), ld = (M + 3) & ~(int64_t)3;
-    const int k = (int)std::min<int64_t>(K.kmax, M);
-    const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(kChunk, (int64_t)(kRedoBytes / (4.0 * (double)ld))));
-    HRAG_TRY(s.redo_rows.ensure((size_t)n_over * 4));
-    HRAG_TRY(h2d(h, s.redo_rows.p, tgt.data(), (size_t)n_over * 4));
-    HRAG_TRY(s.S.ensure((size_t)std::min(chunk, n_over) * ld * 4));
-    for (int64_t o0 = 0; o0 < n_over; o0 += chunk) {
-        const int nb = (int)std::min<int64_t>(chunk, n_over - o0);
-        const int* r = s.redo_rows.as<int>() + o0;
-        HRAG_TRY(gather_rows(h, K.hi.p, rb, r, nb, s.q_hi.p));
-        HRAG_TRY(gather_rows(h, K.lo.p, rb, r, nb, s.q_lo.p));
-        {
-            StageTimer tm(h, ST_SIM_FACT);
-            HRAG_TRY(sim_tc(s.q_hi.p, s.q_lo.p, nb, e_hi, e_lo, M, K.dim, 4, s.S.as<float>(), ld, nullptr, nullptr,
-                            nullptr, h->num_sms, st));
-        }
-        {
-            StageTimer tm(h, ST_TOPK);
-            HRAG_TRY(row_topk(s.S.as<float>(), nb, M, ld, k, s.out_ids.as<int>(), s.out_scores.as<float>(), st));
-            HRAG_TRY(launch_merge(h, nb, r, 0, s.out_ids.as<int>(), s.out_scores.as<float>(), k, nullptr, key0, merge));
-        }
-    }
-    HRAG_CUDA(cudaStreamSynchronize(st));   // the scratch is freed on return
-    return 0;
-}
-
 // Host planes: rows of the pinned planes into dense device rows dst_hi / dst_lo (row i = list[i], or r0 + i without a
 // list), one copy per run of consecutive rows.
-int stage_rows(hrag_t* h, const HostPlanes& P, size_t rb, const int* list, int64_t r0, int64_t n, char* dst_hi,
+int stage_rows(hrag_t* h, const PlaneSet& P, size_t rb, const int* list, int64_t r0, int64_t n, char* dst_hi,
                char* dst_lo) {
     for (int64_t i = 0; i < n;) {
         const int64_t first = list ? list[i] : r0 + i;
         int64_t j = list ? i + 1 : n;
         while (j < n && list[j] == list[j - 1] + 1) ++j;
         const size_t at = (size_t)first * rb, bytes = (size_t)(j - i) * rb;
-        HRAG_TRY(h2d(h, dst_hi + (size_t)i * rb, static_cast<const char*>(P.hi) + at, bytes));
-        HRAG_TRY(h2d(h, dst_lo + (size_t)i * rb, static_cast<const char*>(P.lo) + at, bytes));
+        HRAG_TRY(h2d(h, dst_hi + (size_t)i * rb, P.plane[0] + at, bytes));
+        HRAG_TRY(h2d(h, dst_lo + (size_t)i * rb, P.plane[1] + at, bytes));
         i = j;
     }
     return 0;
 }
 
-// run_queries on host planes: the query rows are staged on the device in passes of up to kHostPass, and each pass
-// streams the keys [key0, key0 + M) through the ring once.  A query's candidate buffer and count persist across the
-// key slices, so the overflow test sees every key >= thr in the range, as one GEMM over it does.
-int host_queries(hrag_t* h, Scratch& s, const std::vector<int>* list, int64_t r0, int64_t n_q, int64_t key0, int64_t M,
-                 bool merge) {
+// Query rows i < n (row list[i] (host; d_list: the same on the device), or r0 + i) of the planes, for the GEMMs:
+// resident rows without a list are read in place, with one gathered into s.q_hi / s.q_lo; host rows are staged there.
+int query_rows(hrag_t* h, Scratch& s, const PlaneSet& P, const int* list, const int* d_list, int64_t r0, int64_t n,
+               const void** qh, const void** ql) {
+    const size_t rb = (size_t)h->knn.dim * 2;
+    *qh = s.q_hi.p;
+    *ql = s.q_lo.p;
+    if (P.streams()) return stage_rows(h, P, rb, list, r0, n, s.q_hi.as<char>(), s.q_lo.as<char>());
+    if (list) {
+        HRAG_TRY(gather_rows(h, P.plane[0], rb, d_list, n, s.q_hi.p));
+        return gather_rows(h, P.plane[1], rb, d_list, n, s.q_lo.p);
+    }
+    *qh = P.plane[0] + (size_t)r0 * rb;
+    *ql = P.plane[1] + (size_t)r0 * rb;
+    return 0;
+}
+
+// The query rows (`list` (host) of n_q rows, or the range [r0, r0 + n_q)) against keys [key0, key0 + M): each
+// query's list becomes the first kmax of its keys >= thr there, merged with the list it has when `merge`.  Passes of
+// kChunk query rows on resident planes, of up to kHostPass staged rows on host planes, each walking the key slices
+// once; a query's candidate buffer and count persist across the slices (moved to rows of the key range after each
+// slice but the first), so the overflow test sees every key >= thr in the range, as one GEMM over it does.
+int run_queries(hrag_t* h, Scratch& s, const std::vector<int>* list, int64_t r0, int64_t n_q, int64_t key0, int64_t M,
+                bool merge) {
     if (n_q == 0 || M == 0) return 0;
     KnnIndex& K = h->knn;
-    HostPlanes& P = K.host;
+    const PlaneSet P = plane_set(K.hi, K.lo, &K.host);
     cudaStream_t st = h->stream;
     const size_t rb = (size_t)K.dim * 2;
-    const int64_t Qp = std::min(n_q, kHostPass);
+    const int64_t Qp = P.streams() ? std::min(n_q, kHostPass) : kChunk;
     HRAG_TRY(s.q_hi.ensure((size_t)Qp * rb));
     HRAG_TRY(s.q_lo.ensure((size_t)Qp * rb));
-    char* q_hi = s.q_hi.as<char>();
-    char* q_lo = s.q_lo.as<char>();
     HRAG_TRY(s.cand.ensure((size_t)Qp * kCandidateCap * sizeof(uint64_t)));
     HRAG_TRY(s.count.ensure((size_t)Qp * 4));
-    HRAG_TRY(s.prev.ensure((size_t)Qp * 4));
+    if (P.streams()) HRAG_TRY(s.prev.ensure((size_t)Qp * 4));
     HRAG_TRY(s.found.ensure((size_t)Qp * 4));
     HRAG_TRY(s.out_ids.ensure((size_t)kChunk * K.kmax * 4));
     HRAG_TRY(s.out_scores.ensure((size_t)kChunk * K.kmax * 4));
-    if (list) HRAG_TRY(s.rows.ensure((size_t)Qp * 4));
+    if (list) HRAG_TRY(s.rows.ensure((size_t)std::min(n_q, Qp) * 4));
     uint64_t* cand = s.cand.as<uint64_t>();
     int* count = s.count.as<int>();
     std::vector<int> found((size_t)Qp), over;   // over: positions in the query set whose candidates overflowed
     for (int64_t p0 = 0; p0 < n_q; p0 += Qp) {
         const int64_t np = std::min(Qp, n_q - p0);
-        HRAG_TRY(stage_rows(h, P, rb, list ? list->data() + p0 : nullptr, r0 + p0, np, q_hi, q_lo));
-        if (list) HRAG_TRY(h2d(h, s.rows.p, list->data() + p0, (size_t)np * 4));
+        const int* plist = list ? list->data() + p0 : nullptr;
+        if (list) HRAG_TRY(h2d(h, s.rows.p, plist, (size_t)np * 4));
+        const void *q_hi = nullptr, *q_lo = nullptr;
+        HRAG_TRY(query_rows(h, s, P, plist, s.rows.as<int>(), r0 + p0, np, &q_hi, &q_lo));
         HRAG_CUDA(cudaMemsetAsync(count, 0, (size_t)np * 4, st));
         auto slice = [&](int64_t, int64_t a, int64_t ns, const void* e_hi, const void* e_lo) -> int {
             for (int64_t q0 = 0; q0 < np; q0 += kChunk) {
@@ -332,8 +269,9 @@ int host_queries(hrag_t* h, Scratch& s, const std::vector<int>* list, int64_t r0
                 if (a > key0)
                     HRAG_CUDA(cudaMemcpyAsync(s.prev.as<int>() + q0, count + q0, (size_t)nb * 4,
                                               cudaMemcpyDeviceToDevice, st));
-                HRAG_TRY(sim_tc_threshold(q_hi + (size_t)q0 * rb, q_lo + (size_t)q0 * rb, nb, e_hi, e_lo, ns, K.dim, 4,
-                                          K.thr, cand + (size_t)q0 * kCandidateCap, count + q0, kCandidateCap,
+                HRAG_TRY(sim_tc_threshold(static_cast<const char*>(q_hi) + (size_t)q0 * rb,
+                                          static_cast<const char*>(q_lo) + (size_t)q0 * rb, nb, e_hi, e_lo, ns, K.dim,
+                                          4, K.thr, cand + (size_t)q0 * kCandidateCap, count + q0, kCandidateCap,
                                           h->num_sms, st));
                 if (a > key0) {
                     k_knn_shift<<<nb, 64, 0, st>>>(cand + (size_t)q0 * kCandidateCap, count + q0,
@@ -369,7 +307,7 @@ int host_queries(hrag_t* h, Scratch& s, const std::vector<int>* list, int64_t r0
     // slice replaces it unless `merge`), cut at thr
     std::vector<int> tgt(over.size());
     for (size_t i = 0; i < over.size(); ++i) tgt[i] = list ? (*list)[over[i]] : (int)(r0 + over[i]);
-    const int64_t n_over = (int64_t)tgt.size(), ld = (P.slice_rows + 3) & ~(int64_t)3;
+    const int64_t n_over = (int64_t)tgt.size(), ld = (P.streams() ? P.host->slice_rows + 3 : M + 3) & ~(int64_t)3;
     const int64_t chunk = std::max<int64_t>(1, std::min<int64_t>(kChunk, (int64_t)(kRedoBytes / (4.0 * (double)ld))));
     HRAG_TRY(s.redo_rows.ensure((size_t)n_over * 4));
     HRAG_TRY(h2d(h, s.redo_rows.p, tgt.data(), (size_t)n_over * 4));
@@ -377,7 +315,8 @@ int host_queries(hrag_t* h, Scratch& s, const std::vector<int>* list, int64_t r0
     for (int64_t o0 = 0; o0 < n_over; o0 += chunk) {
         const int nb = (int)std::min<int64_t>(chunk, n_over - o0);
         const int* r = s.redo_rows.as<int>() + o0;
-        HRAG_TRY(stage_rows(h, P, rb, tgt.data() + o0, 0, nb, q_hi, q_lo));
+        const void *q_hi = nullptr, *q_lo = nullptr;
+        HRAG_TRY(query_rows(h, s, P, tgt.data() + o0, r, 0, nb, &q_hi, &q_lo));
         auto slice = [&](int64_t sl, int64_t a, int64_t ns, const void* e_hi, const void* e_lo) -> int {
             const int64_t lds = (ns + 3) & ~(int64_t)3;
             const int k = (int)std::min<int64_t>(K.kmax, ns);
@@ -427,7 +366,7 @@ int fill_host(hrag_t* h, int64_t rows, int dim, const float* emb, bool on_device
         }
         return 0;
     };
-    return planes_fill(h, P, dim, 0, rows, emb, on_device, verify);
+    return planes_fill(h, plane_set(h->knn.hi, h->knn.lo, &P), dim, 0, rows, emb, on_device, verify);
 }
 
 // The planes of an index of `rows` rows, the first `keep` of them kept, placed in pinned host memory with a ring of
@@ -581,11 +520,10 @@ int hrag_knn_index_update(hrag_t* h, int64_t rows, int32_t dim, const float* emb
         K.width = width;
         K.thr = min_score;
         K.held = true;
-        auto queries = on_host ? host_queries : run_queries;
         if (build) {
             K.rows = rows;
             Scratch s;
-            HRAG_TRY(queries(h, s, nullptr, 0, rows, 0, rows, false));
+            HRAG_TRY(run_queries(h, s, nullptr, 0, rows, 0, rows, false));
             *mode = 0;
             return 0;
         }
@@ -624,9 +562,9 @@ int hrag_knn_index_update(hrag_t* h, int64_t rows, int32_t dim, const float* emb
         K.rows = rows;
         Scratch s;
         // 3. kept rows x new keys, merged; 4. refilled rows and new rows x all keys, replaced
-        HRAG_TRY(queries(h, s, nullptr, 0, n_kept, n_kept, rows - n_kept, true));
-        HRAG_TRY(queries(h, s, &refill, 0, (int64_t)refill.size(), 0, rows, false));
-        HRAG_TRY(queries(h, s, nullptr, n_kept, rows - n_kept, 0, rows, false));
+        HRAG_TRY(run_queries(h, s, nullptr, 0, n_kept, n_kept, rows - n_kept, true));
+        HRAG_TRY(run_queries(h, s, &refill, 0, (int64_t)refill.size(), 0, rows, false));
+        HRAG_TRY(run_queries(h, s, nullptr, n_kept, rows - n_kept, 0, rows, false));
         *mode = 1;
         return 0;
     };

@@ -65,7 +65,7 @@ def test_two_rank_sharded_sweeps_match_oracle(tmp_path, n):
 
 
 def _stage_a_worker(rank, world, port, fe, Q, k, out_path):
-    """Fact-sharded stage A, host logic (api.cu dev_stage_a with world > 1): every rank scores ITS fact rows
+    """Fact-sharded stage A, host logic (fact_stream.cu fact_stage_a with world > 1): every rank scores ITS fact rows
     [rank * ceil(F / world), ...), keeps its 8 best (score desc, row asc) and its (min, max); one all-gather of
     those per query; the merge of the `world` candidate lists is the global top-k and the global min / max."""
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
