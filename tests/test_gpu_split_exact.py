@@ -463,32 +463,25 @@ def test_screen_case_premise(screened):
     """The screen case's design, checked in numpy: the bands L - 2 E_q and U + 2 E_q of every query hold exactly its
     planted rows, lo decides each query's top 8 and minimum, and the screen's caps hold -- at most 256 listed
     candidates and 8 saturated tiles per query (a tile whose list's 8th key, or whose second smallest, lies in a band)
-    and at most 48 staged tiles per 128-query m-tile (one per candidate row sharing a column f mod 256) -- so no chunk
-    should fall back."""
+    and at most 48 staged tiles per 128-query m-tile (one per candidate row sharing a column f mod 256), as the model
+    of test_gpu_screen_caps counts them -- so no chunk should fall back."""
+    from tests.test_gpu_screen_caps import screen_bound, screen_model
     c = screened
     s4, s1 = c["s4"].astype(np.float64), c["s1"].astype(np.float64)
-    E = _err_bound64(c["qh"], c["ql"], c["eh"], c["el"]) * (1 + 2.0 ** -10)
+    E = screen_bound(c["qh"], c["ql"], c["eh"], c["el"])
     assert significant_bits(c) <= 22
-    staged = [set(), set()]
+    model = screen_model(c["s1"], c["s4"], E, np.arange(B_SCREEN))
     for b in range(B_SCREEN):
         top, bottom = c["tops"][b], c["bottoms"][b]
-        L = np.sort(s1[b])[-8]
-        U = s1[b].min()
-        assert set(np.nonzero(s1[b] >= L - 2 * E[b])[0]) == set(top), b
-        assert set(np.nonzero(s1[b] <= U + 2 * E[b])[0]) == set(bottom), b
+        acc = model["acc"][b]
+        assert set(np.nonzero(s1[b] >= acc["L"] - 2 * E[b])[0]) == set(top), b
+        assert set(np.nonzero(s1[b] <= acc["U"] + 2 * E[b])[0]) == set(bottom), b
         assert np.all(s1[b, top] == s1[b, top[0]]) and np.all(s1[b, bottom] == s1[b, bottom[0]])
         assert np.unique(s4[b, top]).size > 4 and np.unique(s4[b, bottom]).size > 1
-        sat = {t for t, n in enumerate(np.bincount(np.asarray(top) // 256)) if n >= 8}
-        sat |= {t for t, n in enumerate(np.bincount(np.asarray(bottom) // 256)) if n >= 2}
-        assert len(top) + len(bottom) <= 256 and len(sat) <= 8
+        assert acc["n"] <= 256 and len(acc["sat"]) <= 8
         if b in (0, 128):
-            assert sat == {1}                                   # query 0's 14 rows in tile 1
-        rows = set(top) | set(bottom)
-        for t in sat:
-            rows |= set(range(256 * t, min(256 * t + 256, F_SCREEN)))
-        staged[b // 128] |= rows
-    for rows in staged:
-        assert np.bincount(np.asarray(sorted(rows)) % 256).max() <= 48
+            assert acc["sat"] == [1]                            # query 0's 14 rows in tile 1
+    assert max(ch["max_col"] for ch in model["chunks"]) <= 48 and model["fallbacks"] == 0
 
 
 def _assert_stage_a_exact(e, case, ks, what, fallbacks=0, minmax=True):

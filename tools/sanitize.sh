@@ -76,6 +76,20 @@ s.stage_a(q2, 5)
 assert s.stats()["stage_a_fallbacks"] == 1
 s.stage_a(q2, 10)
 s.similarity(0, q2[:3])
+# the screen with the lo plane on the host at each cap's last slot (tests/test_gpu_screen_caps.py): 256 candidates
+# for every query of an m-tile, 8 saturated tiles (the ragged last one among them), 48 staged rows in one column and
+# in every column of an m-tile; each exact, without a fallback
+from tests import test_gpu_screen_caps as caps
+for name in ("candidates at cap", "saturated tiles at cap", "48 staged rows in a column",
+             "48 saturated tiles in an m-tile"):
+    w = caps.CASES[name][0]()
+    c = hb.Engine(0, fact_device_bytes=caps._lo_budget(), fact_lo_on_host=True)
+    c.load_embeddings(w["E"], w["E"][:4])
+    c.reset_stats()
+    idx, _, _ = c.stage_a(w["Q"][w["calls"][name]], 8)
+    assert c.stats()["stage_a_fallbacks"] == 0, name
+    assert np.array_equal(idx, caps.exact_outputs(caps.CASES[name][0])[0][w["calls"][name]]), name
+    c.close()
 print("driver ok", ids.shape)
 PY
 compute-sanitizer --tool $TOOL --error-exitcode 7 python /tmp/hrag_sanitize_driver.py 2>&1 | tail -15
