@@ -96,14 +96,6 @@ int p2p_signal(hrag_t* h) {
     StageTimer tc(h, ST_COMM);
     return epoch_signal(sy, h->stream);
 }
-// one fp16 sweep + its exchange: fused peer stores (K5) when the peers are mapped, NCCL all-gather otherwise
-int mixed_sweep_x(hrag_t* h, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_part,
-                  int* overflow) {
-    HRAG_TRY(mixed_sweep(h->g, mode, io, alpha, w, t, n_part, overflow, peers_for(h, io.yh), sync_for_sweep(h),
-                         h->stream));
-    if (!h->p2p) HRAG_TRY(exchange_rows_bytes(h, io.yh, 32 * 2));
-    return 0;
-}
 
 }  // namespace hrag
 

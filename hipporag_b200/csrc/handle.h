@@ -589,9 +589,11 @@ int check_index_private(const hrag_t* h, const std::string& who);
 void index_share_destroy(hrag_t* h);
 
 int exchange_rows(hrag_t* h, float* y, int B);
+int exchange_rows_bytes(hrag_t* h, void* y, size_t row_bytes);
+// a sweep's fused exchange (K5): the peers' copies of y, and the sweep's epoch (null flags when the peers are not mapped)
+PeerOut peers_for(hrag_t* h, void* y);
+SweepSync sync_for_sweep(hrag_t* h);
 int p2p_wait(hrag_t* h);
 int p2p_signal(hrag_t* h);
-int mixed_sweep_x(hrag_t* h, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_part,
-                  int* overflow);
 
 }  // namespace hrag

@@ -82,15 +82,13 @@ struct MixedSweepIO {
     float* partials = nullptr;
     int x0c = 0;
 };
-int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_partials,
-                int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t stream);
+// n = 2 (single GPU, no peers): the same sweep on two states at once.  One walk of each row's non-zeros feeds both, and
+// each state gets exactly the bytes, column sums and partials a sweep of it alone would give it.  The two states are
+// interleaved row by row in [N, 2, 32] buffers: io[1]'s xh / prevh / yh (and a dense rhs_h) point 64 B after io[0]'s; a
+// compact rhs_h, v32, col_scale, slot_map and partials are each state's own.
+int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO* io, int n, float alpha, float w, float t,
+                int* n_partials, int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t stream);
 int mixed_partial_rows(const PprGraph& g);
-// The same sweep on two states at once (single GPU): one walk of each row's non-zeros feeds both, and each state gets
-// exactly the bytes, column sums and partials mixed_sweep would give it.  The two states are interleaved row by row in
-// [N, 2, 32] buffers: io[1]'s xh / prevh / yh (and a dense rhs_h) point 64 B after io[0]'s; a compact rhs_h, v32,
-// col_scale, slot_map and partials are each state's own.
-int mixed_sweep2(const PprGraph& g, int mode, const MixedSweepIO (&io)[2], float alpha, float w, float t,
-                 int* n_partials, int* overflow, cudaStream_t stream);
 // vsum[32] <- column sums of V32 [n_rows, 32] (>= 0; `partials` = scratch of >= 1024*32 floats);
 // scale[b] = 2^floor(log2(32768 (1 - alpha) / vsum[b])) -- overflow-proof, see ppr_mixed.cu;
 // V16 = fp16(scale * V32).

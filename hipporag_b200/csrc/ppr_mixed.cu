@@ -725,97 +725,75 @@ static SweepArgs sweep_args(const PprGraph& g, const MixedSweepIO& io, float alp
     return a;
 }
 
-// One fp16 sweep (mode 0) or the residual sweep (mode 1) over the owned rows.
-int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO& io, float alpha, float w, float t, int* n_partials,
-                int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t st) {
+// One fp16 sweep (mode 0) or the residual sweep (mode 1) of n = 1 or 2 states over the owned rows.
+int mixed_sweep(const PprGraph& g, int mode, const MixedSweepIO* io, int n, float alpha, float w, float t,
+                int* n_partials, int* overflow, const PeerOut& peers, const SweepSync& sync, cudaStream_t st) {
     HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep: graph not loaded");
     HRAG_CHECK(kB <= g.max_batch, "mixed_sweep: segment partials too small for 32 columns");
-    HRAG_CHECK(io.x0c == kX0Dense || (io.slot_map && sync.flags == nullptr && mode == 0),
-               "mixed_sweep: the compact first iterate needs a compact rhs on a single GPU");
+    const bool sharded = sync.flags != nullptr;
+    HRAG_CHECK(n == 1 || (n == 2 && !sharded && peers.n == 0), "mixed_sweep: the paired sweep runs on a single GPU");
+    for (int k = 1; k < n; ++k)
+        HRAG_CHECK((io[k].partials == nullptr) == (io[0].partials == nullptr),
+                   "mixed_sweep: partials for all states or none");
+    for (int k = 0; k < n; ++k)
+        HRAG_CHECK(io[k].x0c == io[0].x0c && (io[k].x0c == kX0Dense || (io[k].slot_map && !sharded && mode == 0)),
+                   "mixed_sweep: the compact first iterate needs a compact rhs for every state on a single GPU");
     const SweepGrid grid(g, kGPB);
-    const SweepArgs a = sweep_args(g, io, alpha, w, t, overflow);
     SweepSync sy = sync;
     // sharded (fused exchange): a persistent grid of 6 CTAs per SM, so each CTA pays one system-scope fence per sweep
     // and the epoch is published by the last CTA of the sweep itself, with no extra launch (see k_sweep_h_push).  The
     // staging ring is double-buffered so a block's bulk copies overlap the next block's gathers: without the second
     // buffer a CTA would sit on its slot until the TMA engine has drained its copies into a congested link.
-    const bool sharded = sync.flags != nullptr;
     const int grid_rows = sharded ? std::min(grid.nb_rows, g.num_sms * 6) : grid.nb_rows;
     sy.total_ctas = (unsigned)(grid_rows + grid.nb_long);
     F8* segp = reinterpret_cast<F8*>(g.seg_partial);
-    if (g.n_long) {     // only waits: the segment kernel writes no exchanged rows
-        if (io.x0c == kX0AsX)
-            k_sweep_long_segments_h<kLPR, RhsRows><<<grid.nb_seg, kThreads, 0, st>>>(
-                g.n_seg, g.segs, g.cv, RhsRows{a.slot_map, a.rhs_h}, segp, sy);
-        else k_sweep_long_segments_h<><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, a.xh, segp, sy);
-        count_launch();
-    }
-    SweepArgs al = a;
-    al.partials = a.partials ? a.partials + (size_t)grid.nb_rows * kB : nullptr;
-    with_bools([&](auto cheb, auto resid, auto fin, auto x0x, auto x0p) {
+    const int x0c = io[0].x0c;
+    with_bools([&](auto cheb, auto resid, auto fin, auto x0x, auto x0p, auto pair) {
         // the residual (mode 1) has no Chebyshev form; sweep 1 (x0 as x) is a plain sweep, sweep 2 (x0 as prev) a
         // Chebyshev one
         if constexpr (!(cheb && resid) && !(x0x && (cheb || resid)) && !(x0p && (!cheb || resid))) {
-            constexpr int M = resid ? 1 : 0;
+            constexpr int NS = pair ? 2 : 1, M = resid ? 1 : 0;
             constexpr int X0C = x0x ? kX0AsX : x0p ? kX0AsPrev : kX0Dense;
+            SweepArgs a[NS];
+            for (int k = 0; k < NS; ++k) a[k] = sweep_args(g, io[k], alpha, w, t, overflow);
+            // the long rows of state k: the single-state segment and finalize kernels on the state's rows (NS * kLPR
+            // uint4 apart); seg_partial is reused in stream order.  The segment kernel only waits: it writes no
+            // exchanged rows.
+            auto segments = [&](int k) {
+                if constexpr (X0C == kX0AsX)
+                    k_sweep_long_segments_h<kLPR, RhsRows><<<grid.nb_seg, kThreads, 0, st>>>(
+                        g.n_seg, g.segs, g.cv, RhsRows{a[k].slot_map, a[k].rhs_h}, segp, sy);
+                else k_sweep_long_segments_h<NS * kLPR><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv,
+                                                                                            a[k].xh, segp, sy);
+                count_launch();
+            };
+            auto finalize = [&](int k) {
+                SweepArgs al = a[k];
+                al.partials = al.partials ? al.partials + (size_t)grid.nb_rows * kB : nullptr;
+                k_sweep_long_finalize_h<cheb, M, fin, NS * kLPR, X0C == kX0AsPrev><<<grid.nb_long, kThreads, 0, st>>>(
+                    g.n_long, g.long_rows, g.long_seg_ptr, segp, al, peers, sy);
+                count_launch();
+            };
+            // one state: the segments first, so the finalize follows the short rows directly
+            if (NS == 1 && grid.nb_long) segments(0);
             if (grid.nb_rows) {
-                if constexpr (X0C == kX0Dense) {
-                    if (sharded) k_sweep_h_push<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a, peers, sy);
-                    else k_sweep_h<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a);
+                if (sharded) {               // one state with a dense first iterate (checked above)
+                    if constexpr (NS == 1 && X0C == kX0Dense)
+                        k_sweep_h_push<cheb, M, fin><<<grid_rows, kThreads, 0, st>>>(a[0], peers, sy);
                 } else {
-                    k_sweep_h<cheb, M, fin, X0C><<<grid_rows, kThreads, 0, st>>>(a);
+                    if constexpr (NS == 1) k_sweep_h<cheb, M, fin, X0C><<<grid_rows, kThreads, 0, st>>>(a[0]);
+                    else k_sweep_h2<cheb, M, fin, X0C><<<grid_rows, kThreads, 0, st>>>(a[0], a[1]);
                 }
                 count_launch();
             }
-            if (grid.nb_long) {
-                k_sweep_long_finalize_h<cheb, M, fin, kLPR, X0C == kX0AsPrev><<<grid.nb_long, kThreads, 0, st>>>(
-                    g.n_long, g.long_rows, g.long_seg_ptr, segp, al, peers, sy);
-                count_launch();
+            for (int k = 0; k < NS && grid.nb_long; ++k) {
+                if (NS == 2) segments(k);
+                finalize(k);
             }
         }
-    }, mode == 0 && (io.prevh != nullptr || io.x0c == kX0AsPrev), mode == 1, io.partials != nullptr,
-       io.x0c == kX0AsX, io.x0c == kX0AsPrev);
+    }, mode == 0 && (io[0].prevh != nullptr || x0c == kX0AsPrev), mode == 1, io[0].partials != nullptr,
+       x0c == kX0AsX, x0c == kX0AsPrev, n == 2);
     if (grid.nb_rows + grid.nb_long == 0 && sharded) HRAG_TRY(epoch_signal(sy, st));
-    if (n_partials) *n_partials = grid.nb_rows + grid.nb_long;
-    HRAG_CUDA(cudaGetLastError());
-    return 0;
-}
-
-int mixed_sweep2(const PprGraph& g, int mode, const MixedSweepIO (&io)[2], float alpha, float w, float t,
-                 int* n_partials, int* overflow, cudaStream_t st) {
-    HRAG_CHECK(g.row_ptr && g.cv, "mixed_sweep2: graph not loaded");
-    HRAG_CHECK(kB <= g.max_batch, "mixed_sweep2: segment partials too small for 32 columns");
-    HRAG_CHECK((io[0].partials == nullptr) == (io[1].partials == nullptr), "mixed_sweep2: partials for both or neither");
-    HRAG_CHECK(io[0].x0c == io[1].x0c && (io[0].x0c == kX0Dense || (io[0].slot_map && io[1].slot_map && mode == 0)),
-               "mixed_sweep2: the compact first iterate needs a compact rhs for both states");
-    const SweepGrid grid(g, kGPB);
-    const SweepArgs a[2] = {sweep_args(g, io[0], alpha, w, t, overflow), sweep_args(g, io[1], alpha, w, t, overflow)};
-    F8* segp = reinterpret_cast<F8*>(g.seg_partial);
-    with_bools([&](auto cheb, auto resid, auto fin, auto x0x, auto x0p) {
-        if constexpr (!(cheb && resid) && !(x0x && (cheb || resid)) && !(x0p && (!cheb || resid))) {
-            constexpr int M = resid ? 1 : 0;
-            constexpr int X0C = x0x ? kX0AsX : x0p ? kX0AsPrev : kX0Dense;
-            if (grid.nb_rows) {
-                k_sweep_h2<cheb, M, fin, X0C><<<grid.nb_rows, kThreads, 0, st>>>(a[0], a[1]);
-                count_launch();
-            }
-            // long rows: the single-state segment and finalize kernels, once per state (seg_partial is reused in
-            // stream order)
-            for (int k = 0; k < 2 && grid.nb_long; ++k) {
-                SweepArgs al = a[k];
-                al.partials = al.partials ? al.partials + (size_t)grid.nb_rows * kB : nullptr;
-                if constexpr (X0C == kX0AsX)
-                    k_sweep_long_segments_h<kLPR, RhsRows><<<grid.nb_seg, kThreads, 0, st>>>(
-                        g.n_seg, g.segs, g.cv, RhsRows{al.slot_map, al.rhs_h}, segp, SweepSync());
-                else k_sweep_long_segments_h<kRS2><<<grid.nb_seg, kThreads, 0, st>>>(g.n_seg, g.segs, g.cv, al.xh,
-                                                                                      segp, SweepSync());
-                k_sweep_long_finalize_h<cheb, M, fin, kRS2, X0C == kX0AsPrev><<<grid.nb_long, kThreads, 0, st>>>(
-                    g.n_long, g.long_rows, g.long_seg_ptr, segp, al, PeerOut(), SweepSync());
-                count_launch(2);
-            }
-        }
-    }, mode == 0 && (io[0].prevh != nullptr || io[0].x0c == kX0AsPrev), mode == 1, io[0].partials != nullptr,
-       io[0].x0c == kX0AsX, io[0].x0c == kX0AsPrev);
     if (n_partials) *n_partials = grid.nb_rows + grid.nb_long;
     HRAG_CUDA(cudaGetLastError());
     return 0;

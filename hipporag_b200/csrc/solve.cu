@@ -193,8 +193,11 @@ static int mixed_sweep_n(hrag_t* h, const StateLayout& L, int n, int mode, const
         io[k].partials = final ? h->mixed_part[k].as<float>() : nullptr;
     }
     int* overflow = h->rho.p ? &h->rho.as<MixedRho>()->overflow : nullptr;
-    if (n == 1) return mixed_sweep_x(h, mode, io[0], alpha, w, t, n_part, overflow);
-    return mixed_sweep2(h->g, mode, io, alpha, w, t, n_part, overflow, h->stream);
+    // the exchange (sharded, n = 1): fused peer stores when the peers are mapped, an NCCL all-gather otherwise
+    HRAG_TRY(mixed_sweep(h->g, mode, io, n, alpha, w, t, n_part, overflow, peers_for(h, io[0].yh), sync_for_sweep(h),
+                         h->stream));
+    if (!h->p2p) HRAG_TRY(exchange_rows_bytes(h, io[0].yh, 32 * 2));
+    return 0;
 }
 
 // Column sums of sub-batch k of the last final sweep -> its MixedSums' `which`
